@@ -1,8 +1,9 @@
 """Benchmark of the hot path named by BASELINE.json: GAIL Hopper, 1024 replica-envs per GPU (weak scaling over the
 replica axis), one full loop iteration per step = rollout (actor forward, env step, replay append) + replay gather x2
-+ discriminator update + reward relabel + SAC update, for every replica. Prints ONE JSON line (see the task contract).
++ discriminator update + reward relabel + SAC update, for every replica. Prints ONE JSON line.
 
-  python bench.py --gpus 1 --steps 20 --warmup 3                      # this arm (B200 kernels)
+  python bench.py --gpus 1 --steps 20 --warmup 3                      # this arm (sm_90a kernels on an H100)
+  python bench.py --gpus 1 --steps 20 --warmup 3 --dump-outputs DIR   # + what the last timed step computed, as DIR/<name>.npy
   python bench.py --impl reference --gpus 1 --steps 20 --warmup 3     # the reference's CPU path (oracle port loop)
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 """
@@ -32,7 +33,7 @@ def parse():
   p.add_argument('--batch-size', type=int, default=256)
   p.add_argument('--start', type=int, default=300, help='update-free prefill steps before the timed region (training.start)')
   p.add_argument('--gemm-mode', default=os.environ.get('IL_GEMM_MODE', 'tf32x3'), choices=['fp32', 'tf32x3', 'tf32'],
-                 help='arithmetic of the 256x256 layers: tf32x3 = 3xTF32 split on tcgen05 (fp32-level accuracy, parity-tested), fp32 = FFMA engine')
+                 help='arithmetic of the 256x256 layers: tf32x3 = 3xTF32 split on wgmma (fp32-level accuracy, parity-tested), fp32 = FFMA engine')
   p.add_argument('--total-replicas', type=int, default=1024, help='strong-scaling record: this many replica-envs split over the N ranks (SURVEY §8d config 2)')
   p.add_argument('--eval-episodes', type=int, default=30, help='eval record: greedy episodes per replica (conf/train_config.yaml:23)')
   p.add_argument('--no-strong', action='store_true')
@@ -40,6 +41,9 @@ def parse():
   p.add_argument('--no-e2e', action='store_true')
   p.add_argument('--no-cpu-baseline', action='store_true')
   p.add_argument('--ref-steps-per-step', type=int, default=10, help='reference arm: oracle loop iterations per bench step and worker')
+  p.add_argument('--dump-outputs', metavar='DIR', default=None,
+                 help='after the timed steps, write what the last timed step left in the trainer (losses, log-probs, Q-values, relabelled rewards, rollout state, '
+                      'temperature, a fixed seeded sample of the parameters) as DIR/<name>.npy, float32; same arguments -> same inputs (seed 0, device RNG streams)')
   return p.parse_args()
 
 
@@ -47,7 +51,7 @@ def workload(a):
   return dict(workload=f'{a.algorithm} {a.env}, {a.replicas} replica-envs per GPU (one reference-equivalent agent + env + replay each), batch {a.batch_size}, '
                        f'256x2 actor/critic, conf/algorithm/{a.algorithm}.yaml defaults',
               algorithm=a.algorithm, env=a.env, replicas_per_gpu=a.replicas, batch_size=a.batch_size, parallelism=f'replica-sharded x{a.gpus} (no data-path collective)',
-              l2='working set per step (parameters + Adam state + activations, > 8 GB at 1024 replicas) exceeds the 126 MB L2; no flush needed')
+              l2='working set per step (parameters + Adam state + activations, > 8 GB at 1024 replicas) exceeds the 50 MB L2 of an H100; no flush needed')
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -116,6 +120,7 @@ class Clocks:
     end_idx = len(self.rows)
     time.sleep(0.05)
     self.proc.terminate()
+    self.proc.wait()
     rows, note = self.rows[self.mark_idx:max(end_idx, self.mark_idx + 1)], None
     if not rows:  # timed region shorter than the sampling period: fall back to the samples taken under the same load just before it
       rows, note = self.rows[-8:], 'no sample landed inside the timed region; these are the last samples of the warm-up under the same load'
@@ -194,6 +199,7 @@ def run_b200(a):
   clocks.mark()
   ms, launches = timed(K)
   clk = clocks.stop()
+  if a.dump_outputs and rank == 0: dump_outputs(tr, a.dump_outputs, a.algorithm)
   value = R * world * K / (ms / 1e3)
 
   # ---- per-kernel roofline of the dominant kernel (the dense 256x256 grouped GEMMs), measured with CUDA events around
@@ -241,6 +247,27 @@ def run_b200(a):
                 gemm_mode=a.gemm_mode, eval=ev, strong=strong)
     print(json.dumps(line), flush=True)
   distributed.barrier()
+
+
+PARAM_SAMPLE = 1 << 18  # entries of each flat parameter buffer kept by --dump-outputs (1 MB per buffer)
+
+
+def dump_outputs(tr, out_dir, a_algorithm):
+  """What a caller of Trainer.train_step() holds after the last timed step, as float32 .npy files (a few MB in all): the per-replica
+  results in full, the flat parameter buffers as a fixed seeded sample of their entries."""
+  import numpy as np
+  import torch
+  os.makedirs(out_dir, exist_ok=True)
+  torch.cuda.synchronize()
+  full = dict(sac_losses=tr.sac_out['losses'], sac_log_probs=tr.sac_out['log_probs'], sac_q_values=tr.sac_out['q_values'], gail_losses=tr.gail_losses,
+              relabelled_rewards=tr.batch['rewards'], last_return=tr.last_return, state=tr.state, action=tr.action, log_alpha=tr.log_alpha)
+  for name, t in full.items(): np.save(os.path.join(out_dir, f'{name}.npy'), t.detach().float().cpu().numpy())
+  nets = dict(actor_params=tr.actor.mlp.flat, critic_params=tr.critic.mlp.flat, target_critic_params=tr.target_critic.mlp.flat)
+  if a_algorithm == 'GAIL': nets['discriminator_params'] = tr.discriminator.parameters()[0]  # one flat buffer (g, and h when reward shaping is on)
+  for name, t in nets.items():
+    flat = t.detach().reshape(-1)
+    idx = np.sort(np.random.default_rng(0).choice(flat.numel(), min(PARAM_SAMPLE, flat.numel()), replace=False))
+    np.save(os.path.join(out_dir, f'{name}.npy'), flat[torch.from_numpy(idx).to(flat.device)].float().cpu().numpy())
 
 
 def measure_eval(tr, a, world):
@@ -319,32 +346,22 @@ def measure_dense_gemm(tr, a):
   lib.il_profile_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
   lib.il_profile_bytes(h, C.byref(nbytes))
   tr.use_graphs = saved
-  peaks = {}
-  try:
-    peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
-  except Exception:
-    pass
-  bf16 = peaks.get('bf16_tflops_sustained')
-  t_peak, t_src = (bf16, 'MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)') if bf16 else (1400.0, 'fallback 1.4 PFLOP/s sustained (B200_PROFILING.md)')
-  hbm = peaks.get('hbm_gbs')
-  h_peak, h_src = (hbm, 'MEASURED_PEAKS.json hbm_gbs (copy bandwidth)') if hbm else (6500.0, 'fallback 6.5 TB/s (B200_PROFILING.md)')
+  # denominators: NVIDIA's data-sheet figures for the H100 SXM (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 (tf32: half of that)
+  t_peak, t_src = 989.0, 'H100 SXM data sheet, dense bf16 (not a measured rate)'
+  h_peak, h_src = 3350.0, 'H100 SXM data sheet, HBM3 bandwidth (not a measured rate)'
   if not ms.value > 0: return dict(bound='hbm', achieved=None, peak=h_peak, unit='GB/s', frac=None, traffic=None)
   sec = ms.value * 1e-3
   tflops = flops.value / sec / 1e12
   gbs = nbytes.value / sec / 1e9
-  traffic = None
-  try:
-    traffic = json.load(open(os.path.join(ROOT, 'profiles', 'dense_gemm_traffic.json'))).get('dram_bytes_per_launch')
-  except Exception:
-    pass
-  # Which roof binds: fp32 operands in and out give 2*256^3 flops per 768 KB, i.e. the minimum HBM time of a launch
-  # (bytes / peak bandwidth) is ~5x its minimum tensor time at the bf16 dense peak -> the kernel is HBM-bound.
-  t_hbm, t_tensor = nbytes.value / (h_peak * 1e9), flops.value / (t_peak * 1e12)
+  traffic = None  # DRAM bytes per launch as a profiler counts them: not measured
+  # Which roof binds: fp32 operands in and out give 2*256^3 flops per 768 KB; the larger of the minimum HBM time of a launch
+  # (bytes / peak bandwidth) and its minimum tensor time at the data-sheet rate of the arithmetic used names the bound.
+  t_hbm, t_tensor = nbytes.value / (h_peak * 1e9), flops.value * (3 if a.gemm_mode == 'tf32x3' else 1) / (t_peak / 2 * 1e12)
   tensor = dict(achieved=tflops, peak=t_peak, unit='TFLOP/s', frac=tflops / t_peak, peak_source=t_src, arithmetic=a.gemm_mode,
                 mma_tflops=tflops * (3 if a.gemm_mode == 'tf32x3' else 1),
                 note='tf32x3 issues 3 tf32 MMAs per algorithmic product (fp32-level accuracy); dense tf32 peak is half the bf16 denominator, so the ceiling '
                      'of this arithmetic is peak/6 algorithmic TFLOP/s' if a.gemm_mode == 'tf32x3' else None)
-  return dict(bound='hbm' if t_hbm >= t_tensor else 'tensor', kernel='tc_gemm_kernel: grouped dense-layer GEMM (256x256x256 per net, fwd(+head) / dX / dW) of the SAC update',
+  return dict(bound='hbm' if t_hbm >= t_tensor else 'tensor', bound_source='the larger of the two minimum times at data-sheet rates; neither rate was measured', kernel='tc_gemm_kernel: grouped dense-layer GEMM (256x256x256 per net, fwd(+head) / dX / dW) of the SAC update',
               achieved=gbs, peak=h_peak, unit='GB/s', frac=gbs / h_peak, traffic=traffic, launches=int(n.value), avg_launch_ms=ms.value / max(n.value, 1),
               algorithmic_bytes_per_launch=nbytes.value / max(n.value, 1), algorithmic_flops_per_launch=flops.value / max(n.value, 1), peak_source=h_src,
               min_time_ratio_hbm_over_tensor=t_hbm / t_tensor, tensor=tensor)

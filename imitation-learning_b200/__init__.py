@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) hot path of Kaixhin/imitation-learning behind the reference's Python surface.
+"""H100-native (sm_90a) hot path of Kaixhin/imitation-learning behind the reference's Python surface.
 
 Importing the package does not need a GPU; creating a handle (any compute call) does — there is no CPU fallback.
 """

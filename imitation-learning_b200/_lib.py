@@ -1,7 +1,7 @@
-"""ctypes binding of the C ABI in include/il_b200.h (the sm_100a shared library csrc/libil_b200.so).
+"""ctypes binding of the C ABI in include/il_b200.h (the sm_90a shared library csrc/libil_b200.so).
 
 PyTorch is used for device memory, streams and torch.distributed only; every hot-path computation goes through
-the entry points bound here. There is no CPU fallback: creating a handle without a B200 raises.
+the entry points bound here. There is no CPU fallback: creating a handle without an H100 raises.
 """
 from __future__ import annotations
 
@@ -178,7 +178,7 @@ _handles: Dict[int, int] = {}
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-  """Compiles csrc/*.cu for sm_100a in-tree (nvcc cross-compiles without a GPU)."""
+  """Compiles csrc/*.cu for sm_90a in-tree (nvcc cross-compiles without a GPU)."""
   import importlib.util
   spec = importlib.util.spec_from_file_location('il_b200_csrc_build', os.path.join(_HERE, 'csrc', 'build.py'))
   mod = importlib.util.module_from_spec(spec)
@@ -209,9 +209,9 @@ def check(rc: int):
 
 
 def handle(device: Optional[int] = None) -> int:
-  """One library handle per CUDA device; fails loudly when there is no B200 (no CPU fallback)."""
+  """One library handle per CUDA device; fails loudly when there is no H100 (no CPU fallback)."""
   if not torch.cuda.is_available():
-    raise RuntimeError('il_b200: no CUDA device available; the hot path only exists as sm_100a kernels (no CPU fallback)')
+    raise RuntimeError('il_b200: no CUDA device available; the hot path only exists as sm_90a kernels (no CPU fallback)')
   device = torch.cuda.current_device() if device is None else device
   with _lock:
     h = _handles.get(device)

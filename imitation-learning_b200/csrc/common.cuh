@@ -1,4 +1,4 @@
-// Shared device/host helpers for the sm_100a hot path. Compiled only for sm_100a (see build.py).
+// Shared device/host helpers for the sm_90a hot path. Compiled only for sm_90a (see build.py).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -18,17 +18,15 @@ struct il_handle {
   int device;
   int sm_count;
   int gemm_mode;
-  int tc_pair_groups;                   // co-resident 2-CTA clusters of the tcgen05 pair kernel (0 = not queried yet)
   int thin_hoist;                       // K-thin kernel: hoisted mask loads for the masked (dX) variant (IL_THIN_HOIST=0/1)
-  int tc_pairs;                         // tcgen05 engine: use CTA pairs (cta_group::2) when rows are a multiple of 256 (IL_TC_PAIRS=0 disables)
   int wide_tn;                          // first-layer weight gradient: 128-bit row-group kernel (IL_WIDE_TN=0 keeps the column-streaming kernel)
-  int first_layer_fast;                 // first MLP layer: specialised FFMA2 kernel for K <= 16 (IL_FIRST_LAYER_FAST=0 keeps the generic K-thin kernel)
+  int first_layer_fast;                 // first MLP layer: specialised k-pair FFMA kernel for K <= 16 (IL_FIRST_LAYER_FAST=0 keeps the generic K-thin kernel)
   int mask_bits;                        // ReLU masks of the MLP backward as sign-bit words written by the forward kernels (IL_MASK_BITS=0: fp32 activations as masks)
   int head_fused;                       // MLP backward: fused head kernel (dZ, dW_L, db_L, db_{L-1} in one pass; IL_HEAD_FUSED=0 disables)
   int debug_sync;                       // IL_DEBUG_SYNC=1: multi-kernel programs synchronise after every stage and name the one that failed
   int adam_tma;                         // AdamW: TMA-staged (cp.async.bulk) streaming kernel for large flat buffers (IL_ADAM_TMA=1 enables)
   int gail_tiled;                       // GAIL update: register-tiled kernel for d <= 32 (IL_GAIL_TILED=0 keeps the first kernel)
-  int tc_fuse_l1;                       // tcgen05 engine: compute the first MLP layer inside the producers of the second (IL_TC_FUSE_L1=0 disables)
+  int tc_fuse_l1;                       // wgmma engine: compute the first MLP layer in place of the A operand loads of the second (IL_TC_FUSE_L1=1 enables)
   long long launches;
   int profiling;                        // il_profile_begin/end: CUDA events around every dense-layer GEMM launch
   std::vector<ProfiledLaunch> profiled;
@@ -191,23 +189,23 @@ struct GemmArgs {
   int accumulate;        // C += result (before activation; only with act == -1)
   int M, N, K, G;
   // ReLU sign bits instead of fp32 activations where only the derivative mask is needed (1/32 of the bytes): word [m][n / 32], bit n % 32 set <=> output (m, n) > 0
-  const uint32_t* mask_bits;  // alternative to `mask` (mask_act == relu); honoured by the tcgen05 engine
+  const uint32_t* mask_bits;  // alternative to `mask` (mask_act == relu); honoured by the wgmma engine
   int64_t mask_bits_gs;       // words per group
-  uint32_t* bits_out;         // optional extra output of the kernels that support it (first_layer_reg_kernel, the fused-head tcgen05 launch)
+  uint32_t* bits_out;         // optional extra output of the kernels that support it (first_layer_reg_kernel, the fused-head wgmma launch)
   int64_t bits_out_gs;
 };
 int launch_gemm(il_handle* h, const GemmArgs& a, cudaStream_t stream);
-bool gemm_uses_tc(const il_handle* h, const GemmArgs& a);                  // the dense tcgen05 engine takes this launch
+bool gemm_uses_tc(const il_handle* h, const GemmArgs& a);                  // the dense wgmma engine takes this launch
 bool gemm_first_layer_emits_bits(const il_handle* h, const GemmArgs& a);   // first_layer_reg_kernel takes this launch (bits_out supported)
 double gemm_algorithmic_bytes(const GemmArgs& a, bool stores_c);
 int profile_open(il_handle* h, ProfiledLaunch* pl, double flops, double bytes, cudaStream_t stream);
 int profile_close(il_handle* h, ProfiledLaunch* pl, cudaStream_t stream);
 
-// tcgen05 engine (tc_gemm.cu): dense M%128==0 (CTA pairs when M%256==0), N==256, K%16==0 problems when il_set_gemm_mode != IL_GEMM_FP32
+// wgmma engine (tc_gemm.cu): dense M%128==0, N==256, K%16==0 problems when il_set_gemm_mode != IL_GEMM_FP32
 bool tc_gemm_eligible(const GemmArgs& a);
 int launch_tc_gemm(il_handle* h, const GemmArgs& a, cudaStream_t stream);
 int tc_gemm_init();
-// First MLP layer fused into the producers of the tcgen05 engine: the A operand of the dense product is
+// First MLP layer fused into the operand staging of the wgmma engine: the A operand of the dense product is
 // relu(X W1^T + b1) (K0 = x_k <= 16 input columns), computed chunk by chunk into the operand tile instead of being read from HBM.
 struct TcFuseL1 {
   const float* x;        // input rows: element (g, m, j) at x + (g / x_gdiv) * x_gs + m * x_ld + j

@@ -13,7 +13,7 @@
 
 // Up to 8 episodes per replica the whole actor runs in one weight-streaming kernel; above that (the reference's 30 evaluation episodes,
 // conf/train_config.yaml:23) the per-layer grouped GEMM program is used: the single-kernel path is bound by its shared-memory operand
-// loads (measured 0.93 ms per loop iteration at R = 1024 x 30 episodes; numbers for both in profiles/README.md).
+// loads.
 constexpr int EVAL_SMALL_MAX = 8;
 
 struct EvalCounters {  // device-resident loop state
@@ -90,7 +90,7 @@ __global__ void __launch_bounds__(128) eval_step_kernel(const EvalStepParams p) 
   }
 }
 
-// rows [E, EP) of every replica's input block stay zero: they only pad the row count of the grouped GEMMs to the tile height of the tcgen05 engine
+// rows [E, EP) of every replica's input block stay zero: they only pad the row count of the grouped GEMMs to the tile height of the wgmma engine
 __global__ void eval_pad_rows_kernel(const float* __restrict__ state, float* __restrict__ xpad, int R, int E, int EP, int S) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (int64_t)R * E * S) return;
@@ -151,7 +151,7 @@ void il_eval_release(il_handle* h) {
 
 // Builds  [reset] -> while (episodes running) { greedy actor forward ; env step + accumulate + loop condition }
 // Rows per replica of the greedy forward: the episode count, or — when the grouped GEMM program is used and the tensor-core engine is on and
-// applicable (256-wide hidden layers) — the next multiple of the 128-row tcgen05 tile.
+// applicable (256-wide hidden layers) — the next multiple of the 128-row wgmma tile.
 static int eval_padded_rows(const il_handle* h, const il_eval_args* a) {
   const int E = a->episodes, L = a->actor.n_layers;
   if (E <= EVAL_SMALL_MAX || h->gemm_mode == IL_GEMM_FP32 || L < 2) return E;
@@ -181,8 +181,8 @@ static int eval_build_impl(il_handle* h, EvalGraph* eg, const il_eval_args* a, f
   // node 0: reset of returns / finished flags / counters, captured into the top-level graph
   IL_CUDA(cudaStreamBeginCaptureToGraph(st, eg->graph, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
   // E > 8 episodes per replica: the greedy forward is a grouped GEMM program; with the tensor-core engine on, the rows of every replica are padded to a
-  // multiple of 128 (zero rows) so that the 256-wide layers run on tcgen05 tiles instead of the fp32 FFMA engine (30 rows -> 128: 4x the MMA work, still
-  // ~3x faster than the FFMA path: the loop body is bound by streaming every replica's weights once per step)
+  // multiple of 128 (zero rows) so that the 256-wide layers run on wgmma tiles instead of the fp32 FFMA engine (30 rows -> 128: 4x the MMA work; the
+  // loop body is bound by streaming every replica's weights once per step)
   const int EP = eval_padded_rows(h, a);
   float* xpad = nullptr;
   eval_init_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a->returns, finished, a->traj_len, ctr, n, EP != E ? reinterpret_cast<float*>(ws) : nullptr, EP != E ? (int64_t)R * EP * S : 0);

@@ -2,7 +2,7 @@
 // column sums). One launch covers all replicas (groups): the reference's per-network nn.Linear forward /
 // autograd backward (models.py:48-69 as used by training.py:14-54) batched over the replica axis.
 //
-// This is the exact-fp32 (FFMA) engine. The dense H x H layers can instead be routed to the tcgen05 engine
+// This is the exact-fp32 (FFMA) engine. The dense H x H layers can instead be routed to the wgmma engine
 // (tc_gemm.cu) by il_set_gemm_mode; everything thin (K = state size, N = 1 or 2A) stays here.
 #include "common.cuh"
 
@@ -246,7 +246,7 @@ __global__ void __launch_bounds__(256, 2) gemm_grouped_kernel(const GemmArgs p) 
 // the last layer (K = head width). These products are pure output bandwidth, so the tile loop of the general kernel is
 // replaced by: B (K x 256) and 32 rows of A in shared memory, 8 x 4 outputs per thread, 128-bit coalesced stores.
 constexpr int TK_MAXK = 32, TK_ROWS = 32, TK_ITERS = 4, TK_COLS = 256, TK_LDA = TK_MAXK + 4;  // a CTA covers 4 x 32 rows
-// (8 x 32 rows per CTA with a coalesced, bank-spread staging of the [N, K] weights measured 1.4 % slower on the whole step.)
+// (8 x 32 rows per CTA with a coalesced, bank-spread staging of the [N, K] weights was not faster on the whole step.)
 // HOIST_MASK: the activation-derivative mask rows of an iteration are loaded before the FMA loop (8 x 128-bit loads in
 // flight per thread, 2 CTAs/SM) instead of one by one inside the store loop (the masked variant is latency-bound).
 template <bool B_KMAJOR, bool HOIST_MASK>
@@ -335,19 +335,28 @@ __global__ void __launch_bounds__(256, HOIST_MASK ? 2 : 3) gemm_thin_k_kernel(co
 
 
 // First MLP layer, specialised: C = relu(A W^T + b) with K <= 16 input columns (state or state + action), N a multiple of 256, M a multiple
-// of 32. The generic K-thin kernel above is instruction-issue bound on this shape (ncu: 154 M warp instructions for 67 M FMAs); here the
-// contraction runs on packed FFMA2 over k-pairs ({a_k, a_k+1} x {w_k, w_k+1} accumulate the even / odd partial sums, added at the end), the
+// of 32. The generic K-thin kernel above is instruction-issue bound on this shape; here the
+// contraction runs on two FFMA chains over k-pairs ({a_k, a_k+1} x {w_k, w_k+1} accumulate the even / odd partial sums, added at the end), the
 // activation is compile-time and there are no bounds checks in the inner loops: ~3x fewer issued instructions, so the kernel is bound by
 // its 128-bit output stores instead.
 constexpr int FL_K = 16, FL_ROWS = 32, FL_ITERS = 4, FL_COLS = 256;
+// Packed pairs of fp32 travel as one 64-bit register pair (128-bit shared-memory loads deliver two of them); sm_90 has no packed
+// fp32 arithmetic, so each half is one IEEE fp32 FMA / multiply.
 __device__ __forceinline__ unsigned long long fl_fma2(unsigned long long a, unsigned long long b, unsigned long long c) {
+  float ax, ay, bx, by, cx, cy;
   unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
+  asm("mov.b64 {%0, %1}, %2;" : "=f"(ax), "=f"(ay) : "l"(a));
+  asm("mov.b64 {%0, %1}, %2;" : "=f"(bx), "=f"(by) : "l"(b));
+  asm("mov.b64 {%0, %1}, %2;" : "=f"(cx), "=f"(cy) : "l"(c));
+  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(fmaf(ax, bx, cx)), "f"(fmaf(ay, by, cy)));
   return d;
 }
 __device__ __forceinline__ unsigned long long fl_mul2(unsigned long long a, unsigned long long b) {
+  float ax, ay, bx, by;
   unsigned long long d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
+  asm("mov.b64 {%0, %1}, %2;" : "=f"(ax), "=f"(ay) : "l"(a));
+  asm("mov.b64 {%0, %1}, %2;" : "=f"(bx), "=f"(by) : "l"(b));
+  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(__fmul_rn(ax, bx)), "f"(__fmul_rn(ay, by)));
   return d;
 }
 __global__ void __launch_bounds__(256, 2) first_layer_relu_kernel(const GemmArgs p) {
@@ -421,8 +430,8 @@ __global__ void __launch_bounds__(256, 2) first_layer_relu_kernel(const GemmArgs
 // Register-resident variant for N == 256 (one CTA = one net's whole [<= 256 rows] x [256 columns] first-layer output): each thread keeps the
 // K x 4 weights of its 4 columns packed as k-pairs in registers for all of its rows, the net's input rows sit in shared memory (one stage, one
 // barrier), and the row loop has no barriers and only warp-broadcast shared loads: per 2 rows x 4 columns 2*ceil(K/4) LDS.128 + 8*ceil(K/2)
-// FFMA2 + 2 STG.128. (ncu on first_layer_relu_kernel: 16 resident warps, issue-active 40 %, stalled on the shared-memory pipe — two 128-bit
-// weight loads per 8 FFMA2 — its per-32-row barriers and the strided weight prologue.) K is a template parameter so the weight registers are
+// k-pair FFMA + 2 STG.128. (first_layer_relu_kernel pays two 128-bit shared-memory
+// weight loads per 8 k-pair FFMA, per-32-row barriers and a strided weight prologue.) K is a template parameter so the weight registers are
 // statically indexed.
 template <int K, bool BITS>
 __global__ void __launch_bounds__(256, 2) first_layer_reg_kernel(const GemmArgs p) {
@@ -671,14 +680,14 @@ __global__ void __launch_bounds__(256, 2) wide_tn_kernel(const GemmArgs p) {
   for (int j = 0; j < WT_MAXN; ++j) acc[j] = make_float4(0.f, 0.f, 0.f, 0.f);
   if (active) {
     for (int k0 = tr; k0 < K; k0 += 16) {
-      fetch(dn, k0 + 16);  // the next 4 rows are in flight while these 4 are consumed (ncu: 4.4 long-scoreboard stalls per issue without the prefetch)
+      fetch(dn, k0 + 16);  // the next 4 rows are in flight while these 4 are consumed
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         const int k = k0 + 4 * u;
         if (k >= K) continue;
         cs.x += d[u].x; cs.y += d[u].y; cs.z += d[u].z; cs.w += d[u].w;
         // the whole (zero padded) row of the small operand first — four independent broadcast loads — then the FMAs: with one load in front of each
-        // group of 16 FMAs the warp stalled on the shared-memory scoreboard four times per row (ncu: 2.4 short-scoreboard stalls per issue)
+        // group of 16 FMAs the warp stalled on the shared-memory scoreboard four times per row
         float4 xv[WT_MAXN / 4];
 #pragma unroll
         for (int q = 0; q < WT_MAXN / 4; ++q) xv[q] = *reinterpret_cast<const float4*>(xs + k * WT_MAXN + 4 * q);
@@ -864,7 +873,7 @@ int launch_gemm(il_handle* h, const GemmArgs& a, cudaStream_t stream) {
   IL_CHECK(!(a.colsum && a.a_kmajor), "gemm: colsum needs the [K, M] operand layout");
   IL_CHECK(!(a.accumulate && a.act >= 0), "gemm: accumulate with activation is not supported");
   const bool plain = !a.bias && a.act < 0 && !a.mask && !a.mask_bits && !a.accumulate;
-  IL_CHECK(!a.mask_bits || gemm_uses_tc(h, a), "gemm: sign-bit masks need the tcgen05 engine (M=%d N=%d K=%d)", a.M, a.N, a.K);
+  IL_CHECK(!a.mask_bits || gemm_uses_tc(h, a), "gemm: sign-bit masks need the wgmma engine (M=%d N=%d K=%d)", a.M, a.N, a.K);
   IL_CHECK(!a.bits_out || gemm_first_layer_emits_bits(h, a), "gemm: this launch cannot emit sign-bit words (M=%d N=%d K=%d)", a.M, a.N, a.K);
   if (h->wide_tn && row_dot_eligible(a)) {
     const dim3 grid((a.M + RD_ROWS - 1) / RD_ROWS, a.G);

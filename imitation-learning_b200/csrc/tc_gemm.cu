@@ -1,197 +1,126 @@
-// tcgen05 engine for the dense H x H layers of the replica-batched MLPs (sm_100a only).
+// wgmma engine for the dense H x H layers of the replica-batched MLPs (sm_90a).
 //
 //   C[g] (M x N) = A[g] (M x K) * B[g] (K x N), fp32 in / fp32 out, tensor-core arithmetic:
-//     IL_GEMM_TF32X3 : each operand is split x = hi + lo (hi = trunc_tf32(x), the top 19 bits the tensor core reads
-//                      anyway; lo = x - hi, exact in fp32) and the product is lo*hi + hi*lo + hi*hi with fp32
-//                      accumulation in TMEM — fp32-level accuracy (error ~2^-21 per product, the dropped lo*lo term)
-//                      at 3 MMAs per product ("3xTF32").
+//     IL_GEMM_TF32X3 : each operand is split x = hi + lo (hi = the top 19 bits of x, i.e. x truncated to tf32; lo = x - hi,
+//                      exact in fp32) and the product is lo*hi + hi*lo + hi*hi with fp32 accumulation — fp32-level
+//                      accuracy (error ~2^-21 per product, the dropped lo*lo term) at 3 MMAs per product ("3xTF32").
 //     IL_GEMM_TF32   : hi*hi only (10-bit mantissa operands).
 //
-// Structure (persistent, one CTA per SM, 13 warps; CG = 2: the two CTAs of a 2-CTA cluster share one 256 x 256 tile):
-//   warps 5..12  producers : cp.async (16 B, L2 only) copies raw fp32 chunks from either operand layout straight into the
-//                            canonical UMMA shared-memory layout of a RAW ring slot (K-major SWIZZLE_64B rows of 16
-//                            floats, or MN-major SWIZZLE_128B_BASE32B — no transposes); when the copies of a k-block
-//                            have landed the same thread derives the LO tile of its own chunks into a short second
-//                            ring, fence.proxy.async, mbarrier arrive (on the leader CTA's barrier in pair mode).
-//   warp  4      MMA issuer: warp-uniform loop, one elected lane issues tcgen05.mma.kind::tf32 (M128 x N256 x K8, or
-//                            cta_group::2 M256 x N256 x K8 for the pair) on shared-memory descriptors, accumulating in
-//                            TMEM; tcgen05.commit (multicast to both CTAs in pair mode) releases slots / publishes tiles.
-//   warps 0..3   epilogue  : tcgen05.ld (32 lanes x 32 columns) -> bias / activation / activation-derivative mask /
-//                            fused final linear layer -> transposed through shared memory -> coalesced 128-bit stores.
-//   TMEM holds two 128 x 256 fp32 accumulators (512 columns) so the epilogue of tile i overlaps the MMAs of tile i+1.
-// A TMA path is not used because every operand needs the hi/lo split (a CUDA-core pass over the tile) anyway and cp.async
-// already lands the data in its final layout.
+// Structure: one CTA of two warpgroups per 128 x 256 output tile; warpgroup w owns rows [64 w, 64 w + 64) as the 128
+// fp32 accumulator registers per thread of wgmma.mma_async m64n256k8.tf32. wgmma reads 32-bit operands from shared memory
+// in K-major layout only, and every operand needs the hi/lo split (a CUDA-core pass) anyway, so the operands go global ->
+// registers -> shared memory: all 256 threads load the raw fp32 chunks of k-block i + 1 (16 floats of k) while the
+// wgmmas of k-block i run, split them and store the hi and lo tiles into the other of two shared-memory stages in the
+// canonical K-major SWIZZLE_64B layout. Operands stored [K, rows] in global memory are transposed on the way: a thread
+// loads a 4 (k) x 4 (rows) block with four coalesced 128-bit loads and stores four 16-byte k-chunks, in a per-thread
+// rotated order that keeps the shared-memory stores conflict-free.
+// The epilogue works on the accumulator fragments in registers (bias / activation / activation-derivative mask /
+// fused final linear layer, reduced over the four lanes that share a row) and stores 8-byte pairs; the four lanes of a
+// row fill one 32-byte sector.
+// TMA is not used because the tensor core cannot consume the raw tile: the split pass has to see every element.
+// The pipeline is the simplest correct one — two stages, wgmma.wait_group 0 and one CTA barrier per k-block, one CTA per SM — and
+// its depth has not been tuned on an H100.
 #include "common.cuh"
 #include <cstdio>
 #include <cstdlib>
 
 namespace {
 
-#ifndef IL_TC_BK
-#define IL_TC_BK 16
-#endif
-constexpr int BM = 128, BN = 256, BK = IL_TC_BK;   // tile: 128 x 256 outputs; k-blocks of 16 floats (64 B rows, SWIZZLE_64B) or 32 (128 B)
-#ifndef IL_TC_NH
-#define IL_TC_NH 6
-#endif
-#ifndef IL_TC_NL
-#define IL_TC_NL 2
-#endif
-// The raw (hi) tiles and the derived lo tiles live in separate rings: NH raw slots keep NH - 1 k-blocks of global loads
-// in flight (the kernel is bound by loaded HBM latency, not by the tensor pipe), the lo tiles only exist between the
-// split pass and the MMAs that read them, so NL = 2 slots suffice.
-static_assert(BK == 16, "the hi/lo rings are laid out for 64-byte k-blocks");
-constexpr int KM_CHUNKS = BK / 4;                  // 16-byte chunks per K-major row
-constexpr int KM_ROW_BYTES = BK * 4;
-constexpr uint32_t KM_LAYOUT = BK == 16 ? 4u : 2u; // UMMA LayoutType: SWIZZLE_64B = 4, SWIZZLE_128B = 2
-#ifndef IL_TC_PW
-#define IL_TC_PW 8
-#endif
-constexpr int N_PRODUCER_WARPS = IL_TC_PW, N_EPI_WARPS = 4;
-constexpr int THREADS = (N_EPI_WARPS + 1 + N_PRODUCER_WARPS) * 32;  // 416
-constexpr int A_BYTES = BM * BK * 4;                                 // 8 KB per k-block (hi or lo copy)
-// Per-CTA geometry for CG = 1 (one CTA computes a 128 x 256 tile) and CG = 2 (a CTA pair computes 256 x 256 with
-// tcgen05.mma.cta_group::2: each CTA stages its own 128 rows of A and HALF of B, i.e. 128 of the 256 output columns'
-// operand rows, so per-CTA shared-memory and L2 traffic per flop drop by a third and the rings get deeper).
-// FUSE (pair mode only): the A operand is not loaded but COMPUTED by the producers — the previous (first) MLP layer
-// relu(X W1^T + b1) with K0 <= 16 input columns, evaluated chunk by chunk straight into the swizzled operand slot — so
-// the first hidden activation never round-trips HBM. The raw ring then carries only B (the weights), and the computed
-// hi tile of A lives next to the lo tiles in the short second ring.
-constexpr int L1_MAXK = 16, L1_ROWS = 256;
-constexpr int L1_W_BYTES = L1_ROWS * L1_MAXK * 4, L1_B_BYTES = L1_ROWS * 4;
-template <int CG, bool FUSE = false>
-struct Geo {
-  static_assert(!FUSE || CG == 2, "the fused first layer is implemented for CTA pairs");
-  static constexpr int BNL = BN / CG;                                // rows of the B operand tile staged by this CTA
-  static constexpr int B_BYTES = BNL * BK * 4;                       // 16 KB / 8 KB
-  static constexpr int RAW_BYTES = FUSE ? B_BYTES : A_BYTES + B_BYTES;                 // raw slot: one k-block of [A | B] (24 / 16 KB), or [B] alone
-  static constexpr int RAW_B_OFF = FUSE ? 0 : A_BYTES;
-  static constexpr int LO_BYTES = FUSE ? 2 * A_BYTES + B_BYTES : A_BYTES + B_BYTES;    // lo slot: [A_lo | B_lo] (+ [A_hi] when A is computed)
-  static constexpr int NH = FUSE ? 10 : (CG == 1 ? IL_TC_NH : 9), NL = CG == 1 ? IL_TC_NL : 3;
-  static constexpr int RING_BYTES = NH * RAW_BYTES + NL * LO_BYTES;  // 192 KB (FUSE: 152 KB)
-  static constexpr int L1_BYTES = FUSE ? 2 * (L1_W_BYTES + L1_B_BYTES) : 0;            // double-buffered W1 [256][16] (zero padded, chunk-swizzled) + b1 [256]
-};
-constexpr int RING_BYTES = Geo<1>::RING_BYTES;
-static_assert(Geo<2>::RING_BYTES <= RING_BYTES, "the pair kernel uses the same shared-memory carve-up");
-static_assert(Geo<2, true>::RING_BYTES + Geo<2, true>::L1_BYTES <= RING_BYTES, "the fused-first-layer variant fits the same carve-up");
-constexpr int EPI_LD = 36;                                           // padded row of the epilogue staging tile: 144-byte rows keep 128-bit accesses aligned and conflict-free
-constexpr int EPI_BYTES = N_EPI_WARPS * 32 * EPI_LD * 4;
+constexpr int BM = 128, BN = 256, BK = 16;        // tile: 128 x 256 outputs; k-blocks of 16 floats (64-byte rows, SWIZZLE_64B)
+constexpr int THREADS = 256;                      // two warpgroups
+constexpr int A_BYTES = BM * BK * 4, B_BYTES = BN * BK * 4;          // 8 KB / 16 KB per k-block (hi or lo copy)
+constexpr int A_HI = 0, A_LO = A_BYTES, B_HI = 2 * A_BYTES, B_LO = 2 * A_BYTES + B_BYTES;
+constexpr int STAGE_BYTES = 2 * (A_BYTES + B_BYTES);                 // 48 KB
+constexpr int N_STAGES = 2;
 constexpr int HEAD_MAX = 8;                                          // fused head: up to 8 output units (N = 1 critic, 2A <= 8 actor)
 constexpr int HEAD_BYTES = (BN + HEAD_MAX * BN) * 4;                 // bias [256] + head weights [8][256]
-constexpr int SMEM_BYTES = 1024 + RING_BYTES + EPI_BYTES + 256 + HEAD_BYTES;
-constexpr uint32_t TMEM_COLS = 512;
+// FUSE: the A operand is not loaded but COMPUTED — the previous (first) MLP layer relu(X W1^T + b1) with K0 <= 16 input
+// columns, evaluated chunk by chunk straight into the swizzled operand tile — so the first hidden activation never
+// round-trips HBM. W1 [256][16] (zero padded), b1 [256] and the tile's input rows [128][16] are staged once per CTA.
+constexpr int L1_MAXK = 16, L1_ROWS = 256;
+constexpr int L1_W_BYTES = L1_ROWS * L1_MAXK * 4, L1_B_BYTES = L1_ROWS * 4, L1_X_BYTES = BM * L1_MAXK * 4;
+constexpr int HEAD_OFF = N_STAGES * STAGE_BYTES, L1_OFF = HEAD_OFF + HEAD_BYTES;
+constexpr int smem_bytes(bool fuse) { return 1024 + L1_OFF + (fuse ? L1_W_BYTES + L1_B_BYTES + L1_X_BYTES : 0); }  // the first-layer staging only where it is used
 
 // ---- PTX wrappers ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count)); }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_LOOP:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE;\n\t"
-      "bra WAIT_LOOP;\n\t"
-      "DONE:\n\t}" ::"r"(bar),
-      "r"(parity)
-      : "memory");
-}
-// CTA pairs: arrive on the barrier at the same offset in CTA `cta` of the cluster. Default (.release.cta) semantics as in
-// cutlass::arch::ClusterBarrier::arrive(cta_id): a .release.cluster arrive waits for the thread's in-flight cp.async
-// groups as well, which collapses the load pipeline to one k-block (measured: 0.61 ms instead of 0.33 ms per launch).
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(bar),
-      "r"(cta)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_LOOP:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE;\n\t"
-      "bra WAIT_LOOP;\n\t"
-      "DONE:\n\t}" ::"r"(bar),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// `leader` != 0 on the one elected lane that issues (the rest of the warp executes the same uniform code predicated off)
-template <int CG>
-__device__ __forceinline__ void tc_commit(uint32_t bar, uint32_t leader) {
-  if (CG == 1)
-    asm volatile(
-        "{\n\t.reg .pred q;\n\t"
-        "setp.ne.b32 q, %1, 0;\n\t"
-        "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar),
-        "r"(leader)
-        : "memory");
-  else  // arrives on the barrier at this offset in BOTH CTAs of the pair
-    asm volatile(
-        "{\n\t.reg .pred q;\n\t.reg .b16 m;\n\t"
-        "setp.ne.b32 q, %1, 0;\n\t"
-        "mov.b16 m, 3;\n\t"
-        "@q tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], m;\n\t}" ::"r"(bar),
-        "r"(leader)
-        : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D (64 x 256, fp32, 128 registers per thread) += A (64 x 8, K-major in shared memory) * B (8 x 256, K-major in shared memory)
+__device__ __forceinline__ void wgmma_tf32(float (&d)[128], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127 "
+      "}, %128, %129, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a_desc), "l"(b_desc));
 }
-template <int CG>
-__device__ __forceinline__ void tc_mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate, uint32_t leader) {
-  if (CG == 1)
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "setp.ne.b32 q, %5, 0;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(leader)
-        : "memory");
-  else
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "setp.ne.b32 q, %5, 0;\n\t"
-        "@q tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(leader)
-        : "memory");
+// Shared-memory matrix descriptor of a K-major SWIZZLE_64B tile: start >> 4 | LBO >> 4 at bit 16 (unused by swizzled K-major
+// layouts) | SBO >> 4 at bit 32 (512 B: the next 8-row atom) | layout type at bit 62 (2 = SWIZZLE_64B).
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(512 >> 4) << 32) | ((uint64_t)2 << 62);
 }
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start >> 4 | LBO >> 4 at bit 16 | SBO >> 4 at bit 32 |
-// version 1 at bit 46 | layout type at bit 61 (2 = SWIZZLE_128B for K-major, 1 = SWIZZLE_128B_BASE32B for MN-major tf32).
-//   K-major : LBO unused (1), SBO = 1024 (next 8-row atom).   MN-major: LBO = 512 (next 32-row atom along MN),
-//   SBO = bytes between groups of 4 k rows.
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;                 // descriptor version (Blackwell)
-  d |= (uint64_t)layout_type << 61;
-  return d;
+// byte offset of 16-byte chunk `c` of row `r` inside a K-major SWIZZLE_64B tile (64-byte rows, 8-row atoms of 512 B;
+// Swizzle<2,4,3>: chunk ^= (r / 2) % 4 — address bits [7,9) are (r >> 1) & 3)
+__device__ __forceinline__ uint32_t sw64(int r, int c) { return (uint32_t)((r >> 3) * 512 + (r & 7) * 64 + ((c ^ ((r >> 1) & 3)) << 4)); }
+__device__ __forceinline__ void sts128(uint32_t addr, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
 }
-// byte offset of 16-byte chunk `c` of row `r` inside a K-major swizzled tile (8-row atoms; Swizzle<3,4,3> on 128 B rows:
-// chunk ^= r % 8; Swizzle<2,4,3> on 64 B rows: chunk ^= (r / 2) % 4 — address bits [7,9) are (r >> 1) & 3 there)
-__device__ __forceinline__ uint32_t sw128(int r, int c) {
-  const int x = BK == 32 ? (r & 7) : ((r >> 1) & 3);
-  return (uint32_t)((r >> 3) * (8 * KM_ROW_BYTES) + (r & 7) * KM_ROW_BYTES + ((c ^ x) << 4));
+__device__ __forceinline__ uint4 lds128(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ uint4 ldg128(const float* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
+__device__ __forceinline__ uint32_t hi_of(uint32_t x) { return x & 0xFFFFE000u; }
+__device__ __forceinline__ uint32_t lo_of(uint32_t x) { return __float_as_uint(__uint_as_float(x) - __uint_as_float(x & 0xFFFFE000u)); }
+// one 16-byte chunk (4 consecutive k of one row) into the hi tile and, for 3xTF32, the lo tile at the same offset
+__device__ __forceinline__ void store_chunk(uint32_t hi_tile, uint32_t lo_tile, uint32_t off, uint4 v, bool split) {
+  sts128(hi_tile + off, hi_of(v.x), hi_of(v.y), hi_of(v.z), hi_of(v.w));
+  if (split) sts128(lo_tile + off, lo_of(v.x), lo_of(v.y), lo_of(v.z), lo_of(v.w));
+}
+// A 4 (k) x 4 (rows) block of an operand stored [K, rows]: v[k] holds rows 4 c4 .. 4 c4 + 3 at k = 4 kg + k. Transposed in
+// registers into the four k-chunks of those rows. Row j of the block is stored at step (j - c4 / 2) % 4, so that the 8
+// threads of a quarter warp (consecutive c4) write 8 rows with distinct r % 8, i.e. 8 distinct 16-byte bank groups.
+__device__ __forceinline__ void store_block_t(uint32_t hi_tile, uint32_t lo_tile, int c4, int kg, const uint4 (&v)[4], bool split) {
+  uint4 q0 = make_uint4(v[0].x, v[1].x, v[2].x, v[3].x), q1 = make_uint4(v[0].y, v[1].y, v[2].y, v[3].y);
+  uint4 q2 = make_uint4(v[0].z, v[1].z, v[2].z, v[3].z), q3 = make_uint4(v[0].w, v[1].w, v[2].w, v[3].w);
+  const int s = (c4 >> 1) & 3;
+  if (s & 1) { const uint4 t = q0; q0 = q1; q1 = q2; q2 = q3; q3 = t; }
+  if (s & 2) { uint4 t = q0; q0 = q2; q2 = t; t = q1; q1 = q3; q3 = t; }
+  store_chunk(hi_tile, lo_tile, sw64(4 * c4 + (s & 3), kg), q0, split);
+  store_chunk(hi_tile, lo_tile, sw64(4 * c4 + ((s + 1) & 3), kg), q1, split);
+  store_chunk(hi_tile, lo_tile, sw64(4 * c4 + ((s + 2) & 3), kg), q2, split);
+  store_chunk(hi_tile, lo_tile, sw64(4 * c4 + ((s + 3) & 3), kg), q3, split);
 }
 
 struct TcParams {
   GemmArgs g;
   int tiles_m;      // M / BM
-  int n_tiles;      // G * tiles_m
   int split;        // 1: 3xTF32, 0: single TF32
   // EPI 4 (bias + ReLU + fused linear head): head_out[g, m, j] = sum_n head_w[g, j, n] * relu(C[g, m, n] + bias[n]) + head_b[g, j]
   const float* head_w;
@@ -201,519 +130,257 @@ struct TcParams {
   int head_n, store_c;           // head units (<= HEAD_MAX); store_c == 0: the hidden output itself is not needed (no backward)
   int head_js, head_ns;          // strides (floats) of head_w between head units j and between the BN contraction indices n: [head_n][BN] row-major = (BN, 1)
   TcFuseL1 l1;                   // FUSE: the first layer whose output is this product's A operand
-  int l1_vec;                    // W1 rows are 16-byte multiples (K0 % 4 == 0): 16-byte staging copies
-};
-
-// packed fp32 pairs (FFMA2: two IEEE fp32 FMAs per issue slot on sm_100)
-__device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
-  unsigned long long r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2(unsigned long long v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ void sts128(uint32_t addr, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
-}
-// Per-thread, kernel-invariant addressing of one k-block (16 floats of k) of the operand tiles:
-//  K-major source  (element (r, k) at src[r * ld + k]) -> canonical K-major SWIZZLE_64B tile: row r = 64 B, 8-row atoms
-//                   512 B apart (SBO), 16-byte chunk c stored at c ^ ((r / 2) % 4).
-//  MN-major source (element (r, k) at src[k * ld + r]) -> no transpose: the canonical MN-major layout for 32-bit
-//                   operands, SWIZZLE_128B_BASE32B (cute Layout_MN_SW128_32B_Atom, the only MN-major layout tf32 has):
-//                   atom = 4 k-rows x 128 B (32 consecutive r), 32-byte chunk q of a row stored at q ^ (k % 4);
-//                   atoms along r 512 B apart (LBO), groups of 4 k (ROWS / 32) * 512 B apart (SBO).
-constexpr int PT = N_PRODUCER_WARPS * 32;                       // producer threads
-constexpr int A_CHUNKS = BM * KM_CHUNKS;                        // 16-byte chunks of the A tile per k-block
-constexpr bool A_SPLIT_STATIC = A_CHUNKS % PT == 0;             // chunk j of every thread belongs to the same operand
-template <int BNL>
-struct ChunkMap {  // chunk j of a thread: global chunk id ptid + j * PT over [A chunks | B chunks]
-  static constexpr int B_CHUNKS = BNL * KM_CHUNKS;
-  static constexpr int CPT = (A_CHUNKS + B_CHUNKS) / PT;        // chunks per producer thread per k-block
-  static_assert(CPT * PT == A_CHUNKS + B_CHUNKS, "producer threads must divide the chunks of a k-block");
-  uint32_t goff[CPT];   // global offset (floats) relative to the operand's tile origin at k-block 0
-  uint32_t soff[CPT];   // byte offset inside a ring slot (A tile at 0, B tile at A_BYTES)
-  uint32_t amask;       // bit j set: chunk j is an A chunk
-  __device__ __forceinline__ bool is_a(int j) const { return A_SPLIT_STATIC ? j < A_CHUNKS / PT : ((amask >> j) & 1u) != 0; }
-  __device__ __forceinline__ void init(int lda, bool a_km, int ldb, bool b_km, int ptid) {
-    amask = 0;
-#pragma unroll
-    for (int j = 0; j < CPT; ++j) {
-      int i = ptid + j * PT;
-      const bool isa = i < A_CHUNKS;
-      if (isa) amask |= 1u << j;
-      else i -= A_CHUNKS;
-      const int rows = isa ? BM : BNL, ld = isa ? lda : ldb;
-      const uint32_t base = isa ? 0u : (uint32_t)A_BYTES;
-      if (isa ? a_km : b_km) {
-        const int r = i / KM_CHUNKS, c = i % KM_CHUNKS;
-        goff[j] = (uint32_t)(r * ld + c * 4);
-        soff[j] = base + sw128(r, c);
-      } else {
-        const int CH = rows / 4;                // 16-byte chunks per k row
-        const int k = i / CH, c = i % CH;       // consecutive threads -> consecutive chunks of one k row (coalesced)
-        const int atom = c >> 3, q = (c & 7) >> 1, half = c & 1;  // 32-row atom along r, 32-byte chunk, 16-byte half
-        goff[j] = (uint32_t)(k * ld + c * 4);
-        soff[j] = base + (uint32_t)((k >> 2) * (rows / 32) * 512 + atom * 512 + (k & 3) * 128 + ((q ^ (k & 3)) << 5) + (half << 4));
-      }
-    }
-  }
 };
 
 // EPI: 0 plain store, 1 bias + relu, 2 relu-derivative mask, 3 generic (runtime bias / activation / mask), 5 relu-derivative mask from sign-bit words,
 //      6 = 5 followed by a fused thin product of the masked tile (the input-gradient slice dX = dZ_0 W_1[:, cols], <= 8 columns; the tile itself is not stored),
-//      4 bias + relu + fused linear head (the next, final layer of the MLP computed from the accumulator row in registers)
-template <int EPI, int CG, bool FUSE = false>
+//      4 bias + relu + fused linear head (the next, final layer of the MLP computed from the accumulator fragments in registers)
+template <int EPI, bool FUSE = false>
 __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
-  using G_ = Geo<CG, FUSE>;
-  constexpr int NH = G_::NH, NL = G_::NL, RAW_BYTES = G_::RAW_BYTES, LO_BYTES = G_::LO_BYTES, RAW_B_OFF = G_::RAW_B_OFF, LO_RING = NH * G_::RAW_BYTES, BNL = G_::BNL;
-  using CMap = ChunkMap<BNL>;
-  constexpr int CPT = CMap::CPT;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* stage_base = smem;
-  float* epi = reinterpret_cast<float*>(smem + RING_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + RING_BYTES + EPI_BYTES);
-  // bars: full[NH], empty[NH] (raw slots), lo_empty[NL], tmem_full[2], tmem_empty[2], then the TMEM base address
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * NH + NL + 4);
-  float* head_s = reinterpret_cast<float*>(smem + RING_BYTES + EPI_BYTES + 256);  // [BN] bias then [HEAD_MAX][BN] head weights
-  const uint32_t bar0 = smem_u32(bars);
-  auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (NH + s); };
-  auto lo_empty_bar = [&](int l) { return bar0 + 8u * (2 * NH + l); };
-  auto tfull_bar = [&](int a) { return bar0 + 8u * (2 * NH + NL + a); };
-  auto tempty_bar = [&](int a) { return bar0 + 8u * (2 * NH + NL + 2 + a); };
+  float* head_s = reinterpret_cast<float*>(smem + HEAD_OFF);  // [BN] bias then [HEAD_MAX][BN] head weights
+  const uint32_t stage0 = smem_u32(smem);
+  const uint32_t w1s = stage0 + L1_OFF, b1s = w1s + L1_W_BYTES, xs = b1s + L1_B_BYTES;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
   const GemmArgs& g = p.g;
   const int nkb = g.K / BK;
-  // CTA group (a single CTA, or the pair of a 2-CTA cluster): the unit that owns one (CG * 128) x 256 output tile
-  const uint32_t rank = CG == 1 ? 0u : cluster_ctarank();
-  const int gid = (int)blockIdx.x / CG, n_groups = (int)gridDim.x / CG;
-  // signals a barrier of the group's leader CTA (rank 0), which issues the MMAs for both CTAs
-  auto arrive_leader = [&](uint32_t bar) {
-    if (CG == 1) mbar_arrive(bar);
-    else mbar_arrive_remote(bar, 0u);
+  const int tile = blockIdx.x, grp = tile / p.tiles_m, m0 = (tile % p.tiles_m) * BM;
+  const bool a_km = FUSE || g.a_kmajor != 0, b_km = g.b_kmajor != 0, split = p.split != 0;
+
+  // ---- per-thread addressing of one k-block ----
+  // stored [rows, K]: 16-byte chunk fc of rows fr + 64 j (A: j < 2, B: j < 4)
+  // stored [K, rows]: 4 x 4 blocks, rows 4 c4 .. 4 c4 + 3 at k = 4 kg .. 4 kg + 3 (A: 128 blocks on the first warpgroup, B: 256 blocks)
+  const int fr = tid >> 2, fc = tid & 3;
+  const int a_c4 = tid & 31, a_kg = (tid >> 5) & 3, b_c4 = tid & 63, b_kg = tid >> 6;
+  const float* a_ptr = nullptr;
+  if (!FUSE) {
+    const float* A = g.A + (int64_t)(grp / g.a_gdiv) * g.a_gs;
+    a_ptr = a_km ? A + (int64_t)(m0 + fr) * g.lda + fc * 4 : A + (int64_t)(a_kg * 4) * g.lda + m0 + a_c4 * 4;
+  }
+  const float* Bg = g.B + (int64_t)(grp / g.b_gdiv) * g.b_gs;
+  const float* b_ptr = b_km ? Bg + (int64_t)fr * g.ldb + fc * 4 : Bg + (int64_t)(b_kg * 4) * g.ldb + b_c4 * 4;
+  const int64_t a_kstep = a_km ? BK : (int64_t)BK * g.lda, b_kstep = b_km ? BK : (int64_t)BK * g.ldb;  // floats per k-block
+  const uint32_t km_off = sw64(fr, fc);  // rows fr + 64 j: + j * 4096 bytes (64 rows = 8 atoms)
+
+  uint4 ra[4], rb[4];
+  auto load_kb = [&]() {  // raw chunks of the next k-block into registers
+    if (!FUSE) {
+      if (a_km) {
+        ra[0] = ldg128(a_ptr);
+        ra[1] = ldg128(a_ptr + (int64_t)64 * g.lda);
+      } else if (wg == 0) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) ra[k] = ldg128(a_ptr + (int64_t)k * g.lda);
+      }
+      a_ptr += a_kstep;
+    }
+    if (b_km) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) rb[j] = ldg128(b_ptr + (int64_t)(64 * j) * g.ldb);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) rb[k] = ldg128(b_ptr + (int64_t)k * g.ldb);
+    }
+    b_ptr += b_kstep;
+  };
+  float* hstore = nullptr;
+  if (FUSE && p.l1.store) hstore = p.l1.store + (int64_t)grp * p.l1.store_gs + (int64_t)(m0 + fr) * g.K + fc * 4;
+  auto store_kb = [&](int kb, uint32_t st) {  // split + store the registers (FUSE: compute the A chunks of k-block kb) into stage `st`
+    if (FUSE) {
+      // A chunk values: relu(b1[k] + sum_j x[j] W1[k][j]) for k = 16 kb + 4 fc + {0..3}, rows fr and fr + 64
+      const int k0 = kb * BK + fc * 4;
+      const uint4 bq = lds128(b1s + (uint32_t)k0 * 4u);
+      float c0[4] = {__uint_as_float(bq.x), __uint_as_float(bq.y), __uint_as_float(bq.z), __uint_as_float(bq.w)};
+      float c1[4] = {c0[0], c0[1], c0[2], c0[3]};
+      const int np = (p.l1.x_k + 3) >> 2;
+#pragma unroll
+      for (int c4 = 0; c4 < L1_MAXK / 4; ++c4) {
+        if (c4 < np) {
+          const uint4 x0 = lds128(xs + sw64(fr, c4)), x1 = lds128(xs + sw64(fr + 64, c4));
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const uint4 w = lds128(w1s + (uint32_t)((k0 + q) * 64 + ((c4 ^ fc) << 4)));  // W1 row k: chunk c4 at c4 ^ ((k >> 2) & 3)
+            c0[q] = fmaf(__uint_as_float(x0.x), __uint_as_float(w.x), c0[q]); c1[q] = fmaf(__uint_as_float(x1.x), __uint_as_float(w.x), c1[q]);
+            c0[q] = fmaf(__uint_as_float(x0.y), __uint_as_float(w.y), c0[q]); c1[q] = fmaf(__uint_as_float(x1.y), __uint_as_float(w.y), c1[q]);
+            c0[q] = fmaf(__uint_as_float(x0.z), __uint_as_float(w.z), c0[q]); c1[q] = fmaf(__uint_as_float(x1.z), __uint_as_float(w.z), c1[q]);
+            c0[q] = fmaf(__uint_as_float(x0.w), __uint_as_float(w.w), c0[q]); c1[q] = fmaf(__uint_as_float(x1.w), __uint_as_float(w.w), c1[q]);
+          }
+        }
+      }
+      const uint4 a0 = make_uint4(__float_as_uint(fmaxf(c0[0], 0.f)), __float_as_uint(fmaxf(c0[1], 0.f)), __float_as_uint(fmaxf(c0[2], 0.f)), __float_as_uint(fmaxf(c0[3], 0.f)));
+      const uint4 a1 = make_uint4(__float_as_uint(fmaxf(c1[0], 0.f)), __float_as_uint(fmaxf(c1[1], 0.f)), __float_as_uint(fmaxf(c1[2], 0.f)), __float_as_uint(fmaxf(c1[3], 0.f)));
+      store_chunk(st + A_HI, st + A_LO, km_off, a0, split);
+      store_chunk(st + A_HI, st + A_LO, km_off + 4096u, a1, split);
+      if (hstore) {  // the first hidden activation, for the backward pass
+        *reinterpret_cast<uint4*>(hstore) = a0;
+        *reinterpret_cast<uint4*>(hstore + (int64_t)64 * g.K) = a1;
+        hstore += BK;
+      }
+    } else if (a_km) {
+      store_chunk(st + A_HI, st + A_LO, km_off, ra[0], split);
+      store_chunk(st + A_HI, st + A_LO, km_off + 4096u, ra[1], split);
+    } else if (wg == 0) {
+      store_block_t(st + A_HI, st + A_LO, a_c4, a_kg, ra, split);
+    }
+    if (b_km) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) store_chunk(st + B_HI, st + B_LO, km_off + (uint32_t)j * 4096u, rb[j], split);
+    } else {
+      store_block_t(st + B_HI, st + B_LO, b_c4, b_kg, rb, split);
+    }
   };
 
-  if (threadIdx.x == 0) {
-    // full / tmem_empty collect the arrivals of every CTA of the group on the leader; empty / lo_empty / tmem_full are
-    // signalled in every CTA by the (multicast) tcgen05.commit
-    for (int s = 0; s < NH; ++s) { mbar_init(full_bar(s), CG * N_PRODUCER_WARPS); mbar_init(empty_bar(s), 1); }
-    for (int l = 0; l < NL; ++l) mbar_init(lo_empty_bar(l), 1);
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), CG * N_EPI_WARPS); }
-    fence_barrier_init();
-  }
-  if (warp == N_EPI_WARPS) {  // TMEM allocation by the MMA warp (of every CTA)
-    if (CG == 1) {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
+  // ---- per-CTA staging: fused-head bias / weights, first-layer parameters and input rows ----
+  if (EPI == 4 || EPI == 6) {
+    const float* wsrc = p.head_w + (int64_t)grp * p.head_gs;
+    if (EPI == 4) {
+      const float* bsrc = g.bias + (int64_t)grp * g.bias_gs;
+      for (int i = tid; i < BN; i += THREADS) head_s[i] = __ldg(bsrc + i);
     }
+    for (int i = tid; i < p.head_n * BN; i += THREADS) head_s[BN + i] = __ldg(wsrc + (int64_t)(i / BN) * p.head_js + (int64_t)(i % BN) * p.head_ns);
   }
-  tc_fence_before();
-  if (CG == 1) __syncthreads();
-  else cluster_sync_all();  // the peer's barriers are initialised before anyone arrives on them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (FUSE) {
+    const int xk = p.l1.x_k;
+    const float* w1 = p.l1.w1 + (int64_t)grp * p.l1.gs;
+    const float* b1 = p.l1.b1 + (int64_t)grp * p.l1.gs;
+    const float* x = p.l1.x + (int64_t)(grp / p.l1.x_gdiv) * p.l1.x_gs + (int64_t)m0 * p.l1.x_ld;
+    float* w1f = reinterpret_cast<float*>(smem + L1_OFF);
+    float* b1f = reinterpret_cast<float*>(smem + L1_OFF + L1_W_BYTES);
+    float* xf = reinterpret_cast<float*>(smem + L1_OFF + L1_W_BYTES + L1_B_BYTES);
+    for (int i = tid; i < L1_ROWS * L1_MAXK; i += THREADS) {  // zero-padded to [256][16]
+      const int k = i / L1_MAXK, j = i % L1_MAXK;
+      w1f[k * L1_MAXK + ((((j >> 2) ^ ((k >> 2) & 3)) << 2) | (j & 3))] = (k < g.K && j < xk) ? __ldg(w1 + (int64_t)k * xk + j) : 0.f;
+    }
+    for (int i = tid; i < L1_ROWS; i += THREADS) b1f[i] = i < g.K ? __ldg(b1 + i) : 0.f;
+    for (int i = tid; i < BM * L1_MAXK; i += THREADS) {
+      const int r = i / L1_MAXK, j = i % L1_MAXK;
+      xf[(sw64(r, j >> 2) >> 2) + (j & 3)] = j < xk ? __ldg(x + (int64_t)r * p.l1.x_ld + j) : 0.f;
+    }
+    __syncthreads();
+  }
 
-  if (warp > N_EPI_WARPS) {
-    // ================= producers =================
-    // cp.async (16 B, L2-only) copies the raw fp32 chunks straight into the swizzled "hi" tile of the NEXT stage while
-    // this thread derives the "lo" tile of the CURRENT stage from the chunks it copied itself (thread-local: no
-    // cross-thread hazard). The tensor core reads only the top 19 bits of each 32-bit tf32 container, so the raw tile
-    // is the hi operand (truncated) and lo = x - trunc_tf32(x) is exact in fp32.
-    const int ptid = threadIdx.x - (N_EPI_WARPS + 1) * 32;
-    const bool a_km = FUSE || g.a_kmajor != 0, b_km = g.b_kmajor != 0, split = p.split != 0;
-    CMap cm;
-    cm.init(g.lda, a_km, g.ldb, b_km, ptid);
-    const int64_t a_kstep = a_km ? BK : (int64_t)BK * g.lda, b_kstep = b_km ? BK : (int64_t)BK * g.ldb;  // floats per k-block
-    const uint32_t stage0 = smem_u32(stage_base);
-    const int my_tiles = (p.n_tiles - gid + n_groups - 1) / n_groups;
-    const int total_kb = my_tiles * nkb;
-    // running position of the next k-block to copy (no divisions in the steady state)
-    int iss_tile = gid, iss_kb = 0, iss_slot = 0;
-    uint32_t iss_par = 1;  // parity to wait for on the slot's empty barrier (a fresh barrier passes parity 1)
-    const float *iss_a = nullptr, *iss_b = nullptr;
-    // FUSE: first-layer parameters of the tile's group are staged (double-buffered) with the copies of the tile's first
-    // k-block, so they have landed when that k-block's commit group has; W1 row k = 64 bytes, 16-byte chunk q at q ^ ((k >> 2) & 3)
-    constexpr int NA = FUSE ? A_CHUNKS / PT : 0;       // chunks of the (computed, not copied) A tile per thread
-    static_assert(!FUSE || (A_SPLIT_STATIC && NA == 2 && KM_CHUNKS == 4 && PT == 256), "fused first layer: 2 A chunks per producer thread (rows r and r + 64, same chunk)");
-    const uint32_t l1s = stage0 + (uint32_t)G_::RING_BYTES;   // W1s[2] then b1s[2]
-    uint32_t iss_buf = 0;
-    auto issue = [&]() {  // async copies of this CTA's next k-block into the next raw slot
-      if (iss_kb == 0) {
-        const int grp = iss_tile / p.tiles_m, m0 = (iss_tile % p.tiles_m) * (BM * CG) + (int)rank * BM, n0 = (int)rank * BNL;
-        if (!FUSE) iss_a = g.A + (int64_t)(grp / g.a_gdiv) * g.a_gs + (a_km ? (int64_t)m0 * g.lda : (int64_t)m0);
-        iss_b = g.B + (int64_t)(grp / g.b_gdiv) * g.b_gs + (b_km ? (int64_t)n0 * g.ldb : (int64_t)n0);  // this CTA's rows of the B operand
-      }
-      const float* A = iss_a;
-      const float* B = iss_b;
-      iss_a += a_kstep;
-      iss_b += b_kstep;
-      if (lane == 0) mbar_wait(empty_bar(iss_slot), iss_par);
-      __syncwarp();
-      const uint32_t st = stage0 + iss_slot * RAW_BYTES;
-      if (++iss_slot == NH) { iss_slot = 0; iss_par ^= 1u; }
-      if (FUSE) {
-        if (iss_kb == 0) {
-          const int grp = iss_tile / p.tiles_m, xk = p.l1.x_k;
-          const float* w1 = p.l1.w1 + (int64_t)grp * p.l1.gs;
-          const uint32_t wdst = l1s + iss_buf * (uint32_t)L1_W_BYTES;
-          if (p.l1_vec) {
-            const int cpr = xk >> 2, n16 = g.K * cpr;
-            for (int i = ptid; i < n16; i += PT) {
-              const int k = i / cpr, q = i - k * cpr;
-              asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(wdst + (uint32_t)(k * 64 + ((q ^ ((k >> 2) & 3)) << 4))), "l"(w1 + (int64_t)k * xk + q * 4) : "memory");
-            }
-          } else {
-            const int n4 = g.K * xk;
-            for (int i = ptid; i < n4; i += PT) {
-              const int k = i / xk, j = i - k * xk;
-              asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(wdst + (uint32_t)(k * 64 + (((j >> 2) ^ ((k >> 2) & 3)) << 4) + ((j & 3) << 2))), "l"(w1 + i) : "memory");
-            }
-          }
-          if (ptid * 4 < g.K)
-            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(l1s + 2u * L1_W_BYTES + iss_buf * (uint32_t)L1_B_BYTES + (uint32_t)ptid * 16u),
-                         "l"(p.l1.b1 + (int64_t)grp * p.l1.gs + ptid * 4) : "memory");
-          iss_buf ^= 1u;
-        }
+  float acc[128];
 #pragma unroll
-        for (int j = NA; j < CPT; ++j) asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(st + cm.soff[j] - (uint32_t)A_BYTES), "l"(B + cm.goff[j]) : "memory");
-      } else {
-#pragma unroll
-        for (int j = 0; j < CPT; ++j) asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(st + cm.soff[j]), "l"((cm.is_a(j) ? A : B) + cm.goff[j]) : "memory");
-      }
-      asm volatile("cp.async.commit_group;" ::: "memory");
-      if (++iss_kb == nkb) { iss_kb = 0; iss_tile += n_groups; }
-    };
-    auto lds128 = [&](uint32_t addr, uint32_t (&v)[4]) {
-      asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(addr));
-    };
-    auto lo_of = [](uint32_t x) { return __float_as_uint(__uint_as_float(x) - __uint_as_float(x & 0xFFFFE000u)); };
-    // FUSE: per-tile state of the computed A operand — this thread's two input rows (registers), the staging buffer parity
-    // and the optional global store of the first hidden activation
-    unsigned long long x0[L1_MAXK / 2], x1[L1_MAXK / 2];  // packed pairs {x[2i], x[2i + 1]}
-    const int fr = ptid >> 2, fc = ptid & 3;   // A chunks of this thread: rows fr and fr + 64 of the CTA's 128, 16-byte chunk fc of the k-block
-    int cons_tile = gid, cons_kb = 0;
-    uint32_t cons_buf = 0;
-    float* hstore = nullptr;
-    auto load_x = [&](int tile) {
-      const int grp = tile / p.tiles_m, m0 = (tile % p.tiles_m) * (BM * CG) + (int)rank * BM;
-      const float* xp = p.l1.x + (int64_t)(grp / p.l1.x_gdiv) * p.l1.x_gs + (int64_t)(m0 + fr) * p.l1.x_ld;
-      const float* xq = xp + (int64_t)64 * p.l1.x_ld;
-#pragma unroll
-      for (int j = 0; j < L1_MAXK; j += 2) {
-        x0[j >> 1] = pack2(j < p.l1.x_k ? __ldg(xp + j) : 0.f, j + 1 < p.l1.x_k ? __ldg(xp + j + 1) : 0.f);
-        x1[j >> 1] = pack2(j < p.l1.x_k ? __ldg(xq + j) : 0.f, j + 1 < p.l1.x_k ? __ldg(xq + j + 1) : 0.f);
-      }
-    };
-    if (FUSE) {
-      // pad columns (j >= K0) of the W1 staging buffers are never written by the copies: zero them once, before any copy is issued
-      for (int i = ptid; i < 2 * L1_W_BYTES / 16; i += PT) sts128(l1s + (uint32_t)i * 16u, 0u, 0u, 0u, 0u);
-      asm volatile("bar.sync 2, %0;" ::"n"(PT) : "memory");
-      if (total_kb > 0) load_x(gid);
-    }
-    // NH - 1 k-blocks of copies are kept in flight; one commit group per loop iteration (empty at the tail) keeps the
-    // wait_group bookkeeping uniform
-    for (int i = 0; i < NH - 1; ++i) {
-      if (i < total_kb) issue();
-      else asm volatile("cp.async.commit_group;" ::: "memory");
-    }
-    int hs = 0, ls = 0;
-    uint32_t lo_par = 1;
-    for (int idx = 0; idx < total_kb; ++idx) {
-      asm volatile("cp.async.wait_group %0;" ::"n"(NH - 2) : "memory");  // this thread's copies of k-block idx have landed
-      const uint32_t st = stage0 + hs * RAW_BYTES;
-      if (FUSE) {
-        if (cons_kb == 0) {
-          // every producer's staging copies of this tile's W1 / b1 have landed (they share the commit group of k-block 0)
-          asm volatile("bar.sync 2, %0;" ::"n"(PT) : "memory");
-          if (p.l1.store) {
-            const int grp = cons_tile / p.tiles_m, m0 = (cons_tile % p.tiles_m) * (BM * CG) + (int)rank * BM;
-            hstore = p.l1.store + (int64_t)grp * p.l1.store_gs + (int64_t)(m0 + fr) * g.K + fc * 4;
-          }
-        }
-        // A chunk values: relu(b1[k] + sum_j x[j] W1[k][j]) for k = 16 kb + 4 fc + {0..3}, rows fr and fr + 64
-        const uint32_t wb = l1s + cons_buf * (uint32_t)L1_W_BYTES + (uint32_t)((cons_kb * 16 + fc * 4) * 64);
-        const int np = (p.l1.x_k + 3) >> 2;
-        uint32_t bq[4];
-        lds128(l1s + 2u * L1_W_BYTES + cons_buf * (uint32_t)L1_B_BYTES + (uint32_t)((cons_kb * 16 + fc * 4) * 4), bq);
-        // 8 accumulator pairs {even-j partial sum, odd-j partial sum} (2 rows x 4 k); per 4-column slice of the input: the 4
-        // weight chunks are loaded together, then 16 packed FMAs on independent chains
-        unsigned long long c0[4], c1[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) c0[q] = c1[q] = pack2(__uint_as_float(bq[q]), 0.f);
-#pragma unroll
-        for (int c4 = 0; c4 < L1_MAXK / 4; ++c4) {
-          if (c4 < np) {
-            unsigned long long w[4][2];
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-              asm volatile("ld.shared.v2.b64 {%0, %1}, [%2];" : "=l"(w[q][0]), "=l"(w[q][1]) : "r"(wb + (uint32_t)(q * 64 + ((c4 ^ fc) << 4))));
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              c0[q] = fma2(x0[c4 * 2], w[q][0], c0[q]);
-              c1[q] = fma2(x1[c4 * 2], w[q][0], c1[q]);
-              c0[q] = fma2(x0[c4 * 2 + 1], w[q][1], c0[q]);
-              c1[q] = fma2(x1[c4 * 2 + 1], w[q][1], c1[q]);
-            }
-          }
-        }
-        uint32_t a0[4], a1[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          float e, o;
-          unpack2(c0[q], e, o);
-          a0[q] = __float_as_uint(fmaxf(e + o, 0.f));
-          unpack2(c1[q], e, o);
-          a1[q] = __float_as_uint(fmaxf(e + o, 0.f));
-        }
-        if (++cons_kb == nkb) {  // the input rows of the next tile load while this k-block is finished
-          cons_kb = 0; cons_tile += n_groups; cons_buf ^= 1u;
-          if (idx + 1 < total_kb) load_x(cons_tile);
-        }
-        uint32_t v[CPT][4];
-#pragma unroll
-        for (int j = NA; j < CPT; ++j) lds128(st + cm.soff[j] - (uint32_t)A_BYTES, v[j]);
-        if (lane == 0) mbar_wait(lo_empty_bar(ls), lo_par);  // the MMAs that read this slot NL k-blocks ago are done
-        __syncwarp();
-        const uint32_t lo = stage0 + LO_RING + ls * LO_BYTES, ahi = lo + (uint32_t)(A_BYTES + G_::B_BYTES);
-        if (++ls == NL) { ls = 0; lo_par ^= 1u; }
-        sts128(ahi + cm.soff[0], a0[0], a0[1], a0[2], a0[3]);
-        sts128(ahi + cm.soff[1], a1[0], a1[1], a1[2], a1[3]);
-        if (split) {
-          sts128(lo + cm.soff[0], lo_of(a0[0]), lo_of(a0[1]), lo_of(a0[2]), lo_of(a0[3]));
-          sts128(lo + cm.soff[1], lo_of(a1[0]), lo_of(a1[1]), lo_of(a1[2]), lo_of(a1[3]));
-#pragma unroll
-          for (int j = NA; j < CPT; ++j) sts128(lo + cm.soff[j], lo_of(v[j][0]), lo_of(v[j][1]), lo_of(v[j][2]), lo_of(v[j][3]));
-        }
-        if (hstore) {  // the first hidden activation, for the backward pass
-          *reinterpret_cast<uint4*>(hstore) = make_uint4(a0[0], a0[1], a0[2], a0[3]);
-          *reinterpret_cast<uint4*>(hstore + (int64_t)64 * g.K) = make_uint4(a1[0], a1[1], a1[2], a1[3]);
-          hstore += BK;
-        }
-      } else if (split) {  // all loads first (independent, in flight together), then the lo tiles into the next lo slot
-        uint32_t v[CPT][4];
-#pragma unroll
-        for (int j = 0; j < CPT; ++j) lds128(st + cm.soff[j], v[j]);
-        if (lane == 0) mbar_wait(lo_empty_bar(ls), lo_par);  // the MMAs that read this lo slot NL k-blocks ago are done
-        __syncwarp();
-        const uint32_t lo = stage0 + LO_RING + ls * LO_BYTES;
-        if (++ls == NL) { ls = 0; lo_par ^= 1u; }
-#pragma unroll
-        for (int j = 0; j < CPT; ++j) sts128(lo + cm.soff[j], lo_of(v[j][0]), lo_of(v[j][1]), lo_of(v[j][2]), lo_of(v[j][3]));
-      }
-      fence_proxy_async();  // generic-proxy / cp.async writes -> visible to the tensor core (async proxy)
-      __syncwarp();
-      if (lane == 0) arrive_leader(full_bar(hs));
-      if (++hs == NH) hs = 0;
-      if (idx + NH - 1 < total_kb) issue();  // waits for the MMAs that last read that raw slot, then refills it
-      else asm volatile("cp.async.commit_group;" ::: "memory");
-    }
-  } else if (warp == N_EPI_WARPS) {
-    // ================= MMA issuer =================
-    // The whole warp runs the (warp-uniform) control flow and address arithmetic so the descriptors stay in uniform
-    // registers; one elected lane issues the tcgen05 instructions. (Issuing from `if (lane == 0)` made the compiler wrap
-    // every MMA in a divergence loop and left the issuing thread, not the tensor pipe, as the bottleneck.)
-    uint32_t leader;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(leader));
-    if (rank == 0) {  // in a CTA pair only the leader CTA issues (for both)
-    // InstrDescriptor: D=F32 (1<<4), A=TF32 (2<<7), B=TF32 (2<<10), a_major bit 15, b_major bit 16 (1 = MN-major),
-    // N>>3 at bit 17, M>>4 at bit 24
-    const bool a_km = FUSE || g.a_kmajor != 0, b_km = g.b_kmajor != 0, split = p.split != 0;
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((a_km ? 0u : 1u) << 15) | ((b_km ? 0u : 1u) << 16) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)((BM * CG) >> 4) << 24);
-    // per-MMA (K = 8 tf32) advance: 32 bytes inside the swizzled 64-byte row (K-major) or two 4-k groups (MN-major)
-    const uint32_t a_lbo = a_km ? 16u : 512u, a_sbo = a_km ? 8u * KM_ROW_BYTES : (uint32_t)(BM / 32) * 512u, a_kadv = a_km ? 32u : 2u * a_sbo, a_lt = a_km ? KM_LAYOUT : 1u;
-    const uint32_t b_lbo = b_km ? 16u : 512u, b_sbo = b_km ? 8u * KM_ROW_BYTES : (uint32_t)(BNL / 32) * 512u, b_kadv = b_km ? 32u : 2u * b_sbo, b_lt = b_km ? KM_LAYOUT : 1u;
-    // descriptors = kernel-invariant part + (shared address >> 4) in the low 14 bits (shared addresses are < 256 KB)
-    const uint64_t a_desc0 = make_desc(0, a_lbo, a_sbo, a_lt), b_desc0 = make_desc(0, b_lbo, b_sbo, b_lt);
-    const uint32_t ring0 = smem_u32(stage_base);
-    uint32_t it = 0, hpar = 0;
-    int hs = 0, ls = 0;
-    for (int tile = gid; tile < p.n_tiles; tile += n_groups, ++it) {
-      const int acc = it & 1;
-      if (CG == 1) mbar_wait(tempty_bar(acc), ((it >> 1) & 1) ^ 1);
-      else mbar_wait_cluster(tempty_bar(acc), ((it >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-      for (int kb = 0; kb < nkb; ++kb) {
-        if (CG == 1) mbar_wait(full_bar(hs), hpar);
-        else mbar_wait_cluster(full_bar(hs), hpar);
-        tc_fence_after();
-        const uint32_t a_lo = ring0 + LO_RING + ls * LO_BYTES, b_lo = a_lo + A_BYTES, b_hi = ring0 + hs * RAW_BYTES + RAW_B_OFF;
-        const uint32_t a_hi = FUSE ? a_lo + (uint32_t)(A_BYTES + G_::B_BYTES) : ring0 + hs * RAW_BYTES;
-#pragma unroll
-        for (int kk = 0; kk < BK / 8; ++kk) {
-          const uint64_t ah = a_desc0 + ((a_hi + kk * a_kadv) >> 4), al = a_desc0 + ((a_lo + kk * a_kadv) >> 4);
-          const uint64_t bh = b_desc0 + ((b_hi + kk * b_kadv) >> 4), bl = b_desc0 + ((b_lo + kk * b_kadv) >> 4);
-          const uint32_t first = (kb == 0 && kk == 0) ? 0u : 1u;
-          if (split) {
-            tc_mma_tf32<CG>(d_tmem, al, bh, idesc, first, leader);
-            tc_mma_tf32<CG>(d_tmem, ah, bl, idesc, 1u, leader);
-            tc_mma_tf32<CG>(d_tmem, ah, bh, idesc, 1u, leader);
-          } else {
-            tc_mma_tf32<CG>(d_tmem, ah, bh, idesc, first, leader);
-          }
-        }
-        tc_commit<CG>(empty_bar(hs), leader);  // frees the raw slot once these MMAs have read it (implicit before_thread_sync fence)
-        if (split || FUSE) { tc_commit<CG>(lo_empty_bar(ls), leader); if (++ls == NL) ls = 0; }
-        if (++hs == NH) { hs = 0; hpar ^= 1u; }
-      }
-      tc_commit<CG>(tfull_bar(acc), leader);  // accumulator complete -> epilogue
-    }
-    }
-    __syncwarp();
-  } else {
-    // ================= epilogue (warps 0..3 <-> TMEM lanes 32w .. 32w+31) =================
-    const uint32_t stg = smem_u32(epi) + (uint32_t)(warp * 32 * EPI_LD * 4);
-    const int cq = (lane & 7) * 4, rsub = lane >> 3;
-    uint32_t it = 0;
-    for (int tile = gid; tile < p.n_tiles; tile += n_groups, ++it) {
-      const int acc = it & 1;
-      const int grp = tile / p.tiles_m, m0 = (tile % p.tiles_m) * (BM * CG) + (int)rank * BM;
-      mbar_wait(tfull_bar(acc), (it >> 1) & 1);
-      tc_fence_after();
-      float* C = g.C + (int64_t)grp * g.c_gs + (int64_t)(m0 + warp * 32 + rsub) * g.ldc + cq;
-      float hacc[HEAD_MAX];
-      if (EPI == 4 || EPI == 6) {  // stage this group's bias and head weights once per tile for the 4 epilogue warps
-        asm volatile("bar.sync 1, 128;" ::: "memory");  // previous tile's readers are done
-        const int et = threadIdx.x;  // 0..127
-        const float* wsrc = p.head_w + (int64_t)grp * p.head_gs;
-        if (EPI == 4) {
-          const float* bsrc = g.bias + (int64_t)grp * g.bias_gs;
-          for (int i = et; i < BN; i += 128) head_s[i] = __ldg(bsrc + i);
-        }
-        for (int i = et; i < p.head_n * BN; i += 128) head_s[BN + i] = __ldg(wsrc + (int64_t)(i / BN) * p.head_js + (int64_t)(i % BN) * p.head_ns);
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-#pragma unroll
-        for (int j = 0; j < HEAD_MAX; ++j) hacc[j] = 0.f;
-      }
-      const float* bias = (EPI == 1 || (EPI == 3 && g.bias)) ? g.bias + (int64_t)grp * g.bias_gs + cq : nullptr;
-      const float* mask = (EPI == 2 || (EPI == 3 && g.mask)) ? g.mask + (int64_t)grp * g.mask_gs + (int64_t)(m0 + warp * 32 + rsub) * g.ldmask + cq : nullptr;
+  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+
+  // ---- main loop: the loads and the split pass of k-block kb + 1 overlap the wgmmas of k-block kb ----
+  load_kb();
+  store_kb(0, stage0);
+  fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
+  __syncthreads();
+  const uint64_t a_desc0 = make_desc(stage0 + (uint32_t)wg * 4096u), b_desc0 = make_desc(stage0);  // this warpgroup's 64 rows of A
 #pragma unroll 1
-      for (int cb = 0; cb < BN / 32; ++cb) {
-        uint32_t r[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(acc * BN + cb * 32);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "
-            "%26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]),
-              "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-              "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-            : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (EPI == 4) {  // bias + ReLU in registers (lane = row), then the head dot products with smem-broadcast weights
-          const float4* bs = reinterpret_cast<const float4*>(head_s + cb * 32);  // 128-bit broadcast loads: the shared-memory pipe is the contended unit of this kernel
+  for (int kb = 0; kb < nkb; ++kb) {
+    const uint32_t cur = (uint32_t)(kb & 1) * STAGE_BYTES, nxt = STAGE_BYTES - cur;
+    const bool more = kb + 1 < nkb;
+    if (more) load_kb();
+    wgmma_fence();
 #pragma unroll
-          for (int c4 = 0; c4 < 8; ++c4) {
-            const float4 b = bs[c4];
-            r[4 * c4] = __float_as_uint(fmaxf(__uint_as_float(r[4 * c4]) + b.x, 0.f));
-            r[4 * c4 + 1] = __float_as_uint(fmaxf(__uint_as_float(r[4 * c4 + 1]) + b.y, 0.f));
-            r[4 * c4 + 2] = __float_as_uint(fmaxf(__uint_as_float(r[4 * c4 + 2]) + b.z, 0.f));
-            r[4 * c4 + 3] = __float_as_uint(fmaxf(__uint_as_float(r[4 * c4 + 3]) + b.w, 0.f));
-          }
-#pragma unroll
-          for (int j = 0; j < HEAD_MAX; ++j) {
-            if (j < p.head_n) {
-              const float4* ws = reinterpret_cast<const float4*>(head_s + BN + j * BN + cb * 32);
-              float a = hacc[j];
-#pragma unroll
-              for (int c4 = 0; c4 < 8; ++c4) {
-                const float4 w = ws[c4];
-                a = fmaf(__uint_as_float(r[4 * c4]), w.x, a); a = fmaf(__uint_as_float(r[4 * c4 + 1]), w.y, a);
-                a = fmaf(__uint_as_float(r[4 * c4 + 2]), w.z, a); a = fmaf(__uint_as_float(r[4 * c4 + 3]), w.w, a);
-              }
-              hacc[j] = a;
-            }
-          }
-          if (g.bits_out) {  // sign bits of this row's 32 hidden outputs: all a dX-only backward pass needs of them (1/32 of the bytes)
-            uint32_t word = 0;
-#pragma unroll
-            for (int c = 0; c < 32; ++c) word |= (__uint_as_float(r[c]) > 0.f ? 1u : 0u) << c;
-            g.bits_out[(int64_t)grp * g.bits_out_gs + (int64_t)(m0 + warp * 32 + lane) * (BN / 32) + cb] = word;
-          }
-          if (!p.store_c) continue;
-        }
-        if (EPI == 5 || EPI == 6) {  // ReLU derivative from the sign-bit words the forward kernel wrote (lane = row, register c = column cb * 32 + c)
-          const uint32_t word = __ldg(g.mask_bits + (int64_t)grp * g.mask_bits_gs + (int64_t)(m0 + warp * 32 + lane) * (BN / 32) + cb);
-#pragma unroll
-          for (int c = 0; c < 32; ++c) r[c] = (word >> c) & 1u ? r[c] : 0u;
-        }
-        if (EPI == 6) {  // the next (thin) product on the masked row in registers: hacc[j] += sum_c r[c] * W[c, j]
-#pragma unroll
-          for (int j = 0; j < HEAD_MAX; ++j) {
-            if (j < p.head_n) {
-              const float4* ws = reinterpret_cast<const float4*>(head_s + BN + j * BN + cb * 32);
-              float a = hacc[j];
-#pragma unroll
-              for (int c4 = 0; c4 < 8; ++c4) {
-                const float4 w = ws[c4];
-                a = fmaf(__uint_as_float(r[4 * c4]), w.x, a); a = fmaf(__uint_as_float(r[4 * c4 + 1]), w.y, a);
-                a = fmaf(__uint_as_float(r[4 * c4 + 2]), w.z, a); a = fmaf(__uint_as_float(r[4 * c4 + 3]), w.w, a);
-              }
-              hacc[j] = a;
-            }
-          }
-          if (!p.store_c) continue;
-        }
-        // lane = row (32 rows of this warp), registers = 32 consecutive columns -> staging tile [row][col] (36-float rows: the 128-bit stores of a quarter warp hit 32 distinct banks)
-        const uint32_t wrow = stg + (uint32_t)(lane * EPI_LD * 4);
-#pragma unroll
-        for (int c = 0; c < 32; c += 4) asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(wrow + c * 4), "r"(r[c]), "r"(r[c + 1]), "r"(r[c + 2]), "r"(r[c + 3]) : "memory");
-        __syncwarp();
-        float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (bias) bv = __ldg(reinterpret_cast<const float4*>(bias + cb * 32));
-        // coalesced write-out: 8 lanes cover one 128-byte row segment, 4 rows per pass
-#pragma unroll
-        for (int pass = 0; pass < 8; ++pass) {
-          const uint32_t rrow = stg + (uint32_t)(((pass * 4 + rsub) * EPI_LD + cq) * 4);
-          float4 v;
-          asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(rrow));
-          const int64_t ro = (int64_t)(pass * 4) * g.ldc + cb * 32;
-          if (EPI == 1) {
-            v.x = fmaxf(v.x + bv.x, 0.f); v.y = fmaxf(v.y + bv.y, 0.f); v.z = fmaxf(v.z + bv.z, 0.f); v.w = fmaxf(v.w + bv.w, 0.f);
-          } else if (EPI == 2) {
-            const float4 mv = __ldg(reinterpret_cast<const float4*>(mask + (int64_t)(pass * 4) * g.ldmask + cb * 32));
-            v.x = mv.x > 0.f ? v.x : 0.f; v.y = mv.y > 0.f ? v.y : 0.f; v.z = mv.z > 0.f ? v.z : 0.f; v.w = mv.w > 0.f ? v.w : 0.f;
-          } else if (EPI == 3) {
-            if (bias) { v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w; }
-            if (g.act >= 0) { v.x = act_apply(v.x, g.act); v.y = act_apply(v.y, g.act); v.z = act_apply(v.z, g.act); v.w = act_apply(v.w, g.act); }
-            if (mask) {
-              const float4 mv = __ldg(reinterpret_cast<const float4*>(mask + (int64_t)(pass * 4) * g.ldmask + cb * 32));
-              v.x *= act_grad_from_output(mv.x, g.mask_act); v.y *= act_grad_from_output(mv.y, g.mask_act);
-              v.z *= act_grad_from_output(mv.z, g.mask_act); v.w *= act_grad_from_output(mv.w, g.mask_act);
-            }
-          }
-          *reinterpret_cast<float4*>(C + ro) = v;
-        }
-        __syncwarp();
+    for (int kk = 0; kk < BK / 8; ++kk) {  // per MMA (K = 8 tf32): 32 bytes further inside the swizzled 64-byte rows
+      const uint32_t o = cur + kk * 32;
+      const uint64_t ah = a_desc0 + ((o + A_HI) >> 4), al = a_desc0 + ((o + A_LO) >> 4), bh = b_desc0 + ((o + B_HI) >> 4), bl = b_desc0 + ((o + B_LO) >> 4);
+      if (split) {
+        wgmma_tf32(acc, al, bh);
+        wgmma_tf32(acc, ah, bl);
       }
-      if (EPI == 4 || EPI == 6) {
-        float* ho = p.head_out + (int64_t)grp * p.head_out_gs + (int64_t)(m0 + warp * 32 + lane) * p.head_n;
-        const float* hb = p.head_b ? p.head_b + (int64_t)grp * p.head_gs : nullptr;
-#pragma unroll
-        for (int j = 0; j < HEAD_MAX; ++j)
-          if (j < p.head_n) ho[j] = hacc[j] + (hb ? __ldg(hb + j) : 0.f);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) arrive_leader(tempty_bar(acc));  // accumulator drained
+      wgmma_tf32(acc, ah, bh);
     }
+    wgmma_commit();
+    if (more) store_kb(kb + 1, stage0 + nxt);  // that stage was last read by the wgmmas of k-block kb - 1, complete in both warpgroups before the barrier below
+    wgmma_wait_all();
+    fence_proxy_async();
+    __syncthreads();
   }
 
-  tc_fence_before();
-  if (CG == 1) __syncthreads();
-  else cluster_sync_all();  // the peer may still be signalling this CTA's barriers / reading its operands until here
-  if (warp == N_EPI_WARPS) {
-    tc_fence_after();
-    if (CG == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
+  // ---- epilogue on the accumulator fragments: acc[4 i + {0, 1}] = row r0, columns 8 i + 2 (lane % 4) + {0, 1}; acc[4 i + {2, 3}] = row r0 + 8 ----
+  const int r0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), cl = (lane & 3) * 2;
+  float* C = g.C + (int64_t)grp * g.c_gs + (int64_t)r0 * g.ldc + cl;
+  const int64_t c8 = (int64_t)8 * g.ldc;
+  const float* bias = (EPI == 1 || (EPI == 3 && g.bias)) ? g.bias + (int64_t)grp * g.bias_gs + cl : nullptr;
+  const float* mask = (EPI == 2 || (EPI == 3 && g.mask)) ? g.mask + (int64_t)grp * g.mask_gs + (int64_t)r0 * g.ldmask + cl : nullptr;
+  const int64_t m8 = (int64_t)8 * g.ldmask;
+  const uint32_t* mbits = (EPI == 5 || EPI == 6) ? g.mask_bits + (int64_t)grp * g.mask_bits_gs + (int64_t)r0 * (BN / 32) : nullptr;
+  float h0[HEAD_MAX], h1[HEAD_MAX];
+#pragma unroll
+  for (int j = 0; j < HEAD_MAX; ++j) h0[j] = h1[j] = 0.f;
+  uint32_t word0 = 0, word1 = 0;  // sign-bit words of the two rows: read (EPI 5 / 6) or built (EPI 4) 32 columns at a time
+#pragma unroll
+  for (int i = 0; i < BN / 8; ++i) {
+    float v00 = acc[4 * i], v01 = acc[4 * i + 1], v10 = acc[4 * i + 2], v11 = acc[4 * i + 3];
+    const int col = 8 * i, bit = (i & 3) * 8 + cl;  // column of v*0 is col + cl; its bit inside the 32-column word
+    if (EPI == 5 || EPI == 6) {  // ReLU derivative from the sign-bit words the forward kernel wrote
+      if ((i & 3) == 0) { word0 = __ldg(mbits + (i >> 2)); word1 = __ldg(mbits + 8 * (BN / 32) + (i >> 2)); }
+      v00 = (word0 >> bit) & 1u ? v00 : 0.f; v01 = (word0 >> (bit + 1)) & 1u ? v01 : 0.f;
+      v10 = (word1 >> bit) & 1u ? v10 : 0.f; v11 = (word1 >> (bit + 1)) & 1u ? v11 : 0.f;
+    }
+    if (EPI == 4) {
+      const float2 b = *reinterpret_cast<const float2*>(head_s + col + cl);
+      v00 = fmaxf(v00 + b.x, 0.f); v01 = fmaxf(v01 + b.y, 0.f); v10 = fmaxf(v10 + b.x, 0.f); v11 = fmaxf(v11 + b.y, 0.f);
+      if (g.bits_out) {  // sign bits of the hidden outputs: all a dX-only backward pass needs of them (1/32 of the bytes)
+        if ((i & 3) == 0) word0 = word1 = 0;
+        word0 |= (v00 > 0.f ? 1u : 0u) << bit | (v01 > 0.f ? 1u : 0u) << (bit + 1);
+        word1 |= (v10 > 0.f ? 1u : 0u) << bit | (v11 > 0.f ? 1u : 0u) << (bit + 1);
+        if ((i & 3) == 3) {  // the four lanes of a row hold 8 bits each of the word
+          word0 |= __shfl_xor_sync(0xffffffffu, word0, 1); word0 |= __shfl_xor_sync(0xffffffffu, word0, 2);
+          word1 |= __shfl_xor_sync(0xffffffffu, word1, 1); word1 |= __shfl_xor_sync(0xffffffffu, word1, 2);
+          if ((lane & 3) == 0) {
+            uint32_t* bo = g.bits_out + (int64_t)grp * g.bits_out_gs + (int64_t)r0 * (BN / 32) + (i >> 2);
+            bo[0] = word0;
+            bo[8 * (BN / 32)] = word1;
+          }
+        }
+      }
+    }
+    if (EPI == 4 || EPI == 6) {  // the next (thin) product on the fragment: h[j] += sum_c v[c] * W[j][c]
+#pragma unroll
+      for (int j = 0; j < HEAD_MAX; ++j) {
+        if (j < p.head_n) {
+          const float2 w = *reinterpret_cast<const float2*>(head_s + BN + j * BN + col + cl);
+          h0[j] = fmaf(v00, w.x, h0[j]); h0[j] = fmaf(v01, w.y, h0[j]);
+          h1[j] = fmaf(v10, w.x, h1[j]); h1[j] = fmaf(v11, w.y, h1[j]);
+        }
+      }
+      if (!p.store_c) continue;
+    }
+    if (EPI == 1) {
+      const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
+      v00 = fmaxf(v00 + b.x, 0.f); v01 = fmaxf(v01 + b.y, 0.f); v10 = fmaxf(v10 + b.x, 0.f); v11 = fmaxf(v11 + b.y, 0.f);
+    } else if (EPI == 2) {
+      const float2 ma = __ldg(reinterpret_cast<const float2*>(mask + col)), mb = __ldg(reinterpret_cast<const float2*>(mask + m8 + col));
+      v00 = ma.x > 0.f ? v00 : 0.f; v01 = ma.y > 0.f ? v01 : 0.f; v10 = mb.x > 0.f ? v10 : 0.f; v11 = mb.y > 0.f ? v11 : 0.f;
+    } else if (EPI == 3) {
+      if (bias) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
+        v00 += b.x; v01 += b.y; v10 += b.x; v11 += b.y;
+      }
+      if (g.act >= 0) { v00 = act_apply(v00, g.act); v01 = act_apply(v01, g.act); v10 = act_apply(v10, g.act); v11 = act_apply(v11, g.act); }
+      if (mask) {
+        const float2 ma = __ldg(reinterpret_cast<const float2*>(mask + col)), mb = __ldg(reinterpret_cast<const float2*>(mask + m8 + col));
+        v00 *= act_grad_from_output(ma.x, g.mask_act); v01 *= act_grad_from_output(ma.y, g.mask_act);
+        v10 *= act_grad_from_output(mb.x, g.mask_act); v11 *= act_grad_from_output(mb.y, g.mask_act);
+      }
+    }
+    *reinterpret_cast<float2*>(C + col) = make_float2(v00, v01);
+    *reinterpret_cast<float2*>(C + c8 + col) = make_float2(v10, v11);
+  }
+  if (EPI == 4 || EPI == 6) {  // the four lanes of a row each hold the partial sums of a quarter of the columns
+    float* ho = p.head_out + (int64_t)grp * p.head_out_gs + (int64_t)r0 * p.head_n;
+    const float* hb = p.head_b ? p.head_b + (int64_t)grp * p.head_gs : nullptr;
+#pragma unroll
+    for (int j = 0; j < HEAD_MAX; ++j) {
+      if (j < p.head_n) {
+        float s0 = h0[j], s1 = h1[j];
+        s0 += __shfl_xor_sync(0xffffffffu, s0, 1); s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
+        s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+        if ((lane & 3) == 0) {
+          const float b = hb ? __ldg(hb + j) : 0.f;
+          ho[j] = s0 + b;
+          ho[(int64_t)8 * p.head_n + j] = s1 + b;
+        }
+      }
+    }
   }
 }
 
@@ -739,60 +406,24 @@ bool tc_gemm_eligible(const GemmArgs& a) {
   return true;
 }
 
-template <int EPI, int CG, bool FUSE = false>
+template <int EPI, bool FUSE = false>
 int tc_set_attr() {
-  IL_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<EPI, CG, FUSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+  IL_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<EPI, FUSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(FUSE)));
   return 0;
 }
 
 int tc_gemm_init() {
-  IL_TRY((tc_set_attr<0, 1>())); IL_TRY((tc_set_attr<1, 1>())); IL_TRY((tc_set_attr<2, 1>())); IL_TRY((tc_set_attr<3, 1>())); IL_TRY((tc_set_attr<4, 1>()));
-  IL_TRY((tc_set_attr<0, 2>())); IL_TRY((tc_set_attr<1, 2>())); IL_TRY((tc_set_attr<2, 2>())); IL_TRY((tc_set_attr<3, 2>())); IL_TRY((tc_set_attr<4, 2>()));
-  IL_TRY((tc_set_attr<4, 2, true>()));
-  IL_TRY((tc_set_attr<5, 1>())); IL_TRY((tc_set_attr<5, 2>())); IL_TRY((tc_set_attr<6, 1>())); IL_TRY((tc_set_attr<6, 2>()));
+  IL_TRY((tc_set_attr<0>())); IL_TRY((tc_set_attr<1>())); IL_TRY((tc_set_attr<2>())); IL_TRY((tc_set_attr<3>())); IL_TRY((tc_set_attr<4>()));
+  IL_TRY((tc_set_attr<4, true>())); IL_TRY((tc_set_attr<5>())); IL_TRY((tc_set_attr<6>()));
   return 0;
 }
 
-// CTA pairs (tcgen05.mma.cta_group::2, one 256 x 256 tile per 2-CTA cluster) whenever the rows come in multiples of 256
-static bool tc_use_pairs(const il_handle* h, const GemmArgs& a) { return h->tc_pairs && a.M % (2 * BM) == 0 && h->sm_count >= 2; }
-
+// one CTA per 128 x 256 tile; the tiles of a group are adjacent, so its B operand is read from HBM once and from L2 after that
 template <int EPI, bool FUSE = false>
 static int tc_launch(il_handle* h, TcParams& p, cudaStream_t stream) {
   const GemmArgs& a = p.g;
-  const bool pairs = tc_use_pairs(h, a);
-  const int cg = pairs ? 2 : 1;
-  p.tiles_m = a.M / (BM * cg);
-  p.n_tiles = a.G * p.tiles_m;
-  if (!pairs) {
-    IL_CHECK(!FUSE, "tc_gemm: the fused first layer needs CTA pairs (rows %% 256 == 0)");
-    const int groups = p.n_tiles < h->sm_count ? p.n_tiles : h->sm_count;
-    IL_LAUNCH(h, (tc_gemm_kernel<EPI, 1>), groups, THREADS, SMEM_BYTES, stream, p);
-    return 0;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(h->sm_count & ~1);
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  // The persistent grid must be co-resident: a 2-CTA cluster needs both SMs of a TPC, and on parts with TPCs that
-  // have a single enabled SM fewer than sm_count / 2 clusters fit at once (a second wave would double the time).
-  if (h->tc_pair_groups == 0) {
-    int n = 0;
-    IL_CUDA(cudaOccupancyMaxActiveClusters(&n, tc_gemm_kernel<EPI, 2, FUSE>, &cfg));
-    IL_CHECK(n >= 1, "tc_gemm: no 2-CTA cluster of the tcgen05 kernel fits on this device");
-    h->tc_pair_groups = n;
-    if (getenv("IL_TC_VERBOSE")) fprintf(stderr, "[il_b200] tcgen05 pair kernel: %d co-resident 2-CTA clusters on %d SMs\n", n, h->sm_count);
-  }
-  const int groups = p.n_tiles < h->tc_pair_groups ? p.n_tiles : h->tc_pair_groups;
-  cfg.gridDim = dim3(groups * 2);
-  const cudaError_t e = cudaLaunchKernelEx(&cfg, tc_gemm_kernel<EPI, 2, FUSE>, p);
-  h->launches++;
-  if (e != cudaSuccess) IL_FAIL("cluster launch of tc_gemm_kernel<%d, 2> failed: %s", EPI, cudaGetErrorString(e));
+  p.tiles_m = a.M / BM;
+  IL_LAUNCH(h, (tc_gemm_kernel<EPI, FUSE>), a.G * p.tiles_m, THREADS, smem_bytes(FUSE), stream, p);
   return 0;
 }
 
@@ -800,10 +431,10 @@ bool tc_head_fusable(const il_handle* h, const GemmArgs& a, int head_n) {
   return h->gemm_mode != IL_GEMM_FP32 && tc_gemm_eligible(a) && a.bias && a.act == IL_ACT_RELU && !a.mask && !a.colsum && head_n >= 1 && head_n <= HEAD_MAX;
 }
 
-// The first layer can be computed by the producers when the dense product runs on CTA pairs and the staging buffers fit:
-// K0 <= 16 input columns, hidden width (the K of the dense product) <= 256 and deep enough to cover the load pipeline.
+// The first layer can be computed in place of the A operand loads when the staging buffers fit: K0 <= 16 input columns and
+// hidden width (the K of the dense product) <= 256.
 bool tc_l1_fusable(const il_handle* h, const GemmArgs& a, int x_k) {
-  return h->tc_fuse_l1 && tc_use_pairs(h, a) && x_k >= 1 && x_k <= L1_MAXK && a.K <= L1_ROWS && a.K / BK >= Geo<2, true>::NH && a.a_kmajor;
+  return h->tc_fuse_l1 && tc_gemm_eligible(a) && x_k >= 1 && x_k <= L1_MAXK && a.K <= L1_ROWS && a.a_kmajor;
 }
 
 int launch_tc_gemm_head(il_handle* h, const GemmArgs& a, const float* head_w, const float* head_b, int64_t head_gs, int head_n, float* head_out, int64_t head_out_gs, int store_c,
@@ -820,7 +451,6 @@ int launch_tc_gemm_head(il_handle* h, const GemmArgs& a, const float* head_w, co
     IL_CHECK(l1->x && l1->w1 && l1->b1 && (reinterpret_cast<uintptr_t>(l1->b1) & 15) == 0 && l1->gs % 4 == 0, "tc_gemm_head: bad first-layer buffers");
     IL_CHECK(!l1->store || ((reinterpret_cast<uintptr_t>(l1->store) & 15) == 0 && l1->store_gs % 4 == 0), "tc_gemm_head: unaligned hidden store");
     p.l1 = *l1;
-    p.l1_vec = (l1->x_k % 4 == 0 && (reinterpret_cast<uintptr_t>(l1->w1) & 15) == 0) ? 1 : 0;
     // algorithmic traffic: the A operand is not read; X, W1, b1 are, and the hidden store (if any) is written
     const double gx = (a.G + l1->x_gdiv - 1) / l1->x_gdiv;
     bytes += -4.0 * a.G * (double)a.M * a.K + 4.0 * (gx * a.M * l1->x_k + (double)a.G * a.K * (l1->x_k + 1)) + (l1->store ? 4.0 * a.G * (double)a.M * a.K : 0.0);

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's models.py surface (same names / arguments / behaviour) over the sm_100a
+"""Host-side mirror of the reference's models.py surface (same names / arguments / behaviour) over the sm_90a
 kernels. Every class takes an extra `replicas` axis (default 1 = the reference's shapes).
 
 Cited lines are in the reference's models.py unless noted.

@@ -1,5 +1,5 @@
 /*
- * il_b200.h — C ABI of the B200-native (sm_100a) hot path of Kaixhin/imitation-learning.
+ * il_b200.h — C ABI of the H100-native (sm_90a) hot path of Kaixhin/imitation-learning.
  *
  * The reference has no FFI: its hot path sits behind Python signatures (SURVEY.md §8b). Each entry point
  * below is what a binding for that path would call; the comment on each cites the reference interface it
@@ -82,7 +82,7 @@ int         il_version(void);
 int         il_set_gemm_mode(il_handle* h, int mode);              /* IL_GEMM_* for the dense hidden layers */
 int64_t     il_launch_count(il_handle* h);                         /* kernels launched by this library so far */
 /* Kernel-selection toggles for A/B measurements and tests (defaults from the IL_* environment variables at il_create):
- * "tc_fuse_l1" (first MLP layer inside the tcgen05 producers), "gail_tiled", "tc_pairs", "thin_hoist". */
+ * "tc_fuse_l1" (first MLP layer inside the wgmma launch), "gail_tiled", "thin_hoist". */
 int         il_set_option(il_handle* h, const char* name, int value);
 int         il_struct_sizes(int32_t* out15);                       /* sizeof il_mlp, il_adam, il_batch, il_replay, il_sac_args, il_gail, il_gail_update_args, il_pwil, il_env, il_bc_args, il_eval_args, il_gailx, il_gailx_update_args, il_red, il_red_update_args */
 int         il_mlp_param_offsets(const int32_t* dims, int n_layers, int64_t* w_off, int64_t* b_off, int64_t* total);
@@ -98,7 +98,7 @@ int il_profile_bytes(il_handle* h, double* total_bytes);
 
 /* Test / diagnostics entry: one grouped GEMM C[g] = A[g] B[g] with the fused epilogues (bias, activation act >= 0,
  * activation-derivative mask, bias-gradient column sums), dispatched exactly like the MLP programs dispatch it
- * (fp32 FFMA engine, or the tcgen05 engine for eligible dense shapes when the gemm mode is tf32x3 / tf32).
+ * (fp32 FFMA engine, or the wgmma engine for eligible dense shapes when the gemm mode is tf32x3 / tf32).
  * a_kmajor: A stored [M, K] (else [K, M]); b_kmajor: B stored [N, K] (else [K, N]). */
 int il_debug_gemm(il_handle* h, int M, int N, int K, int G, const float* A, int64_t a_gs, int lda, int a_kmajor,
                   const float* B, int64_t b_gs, int ldb, int b_kmajor, float* C, int64_t c_gs, int ldc,

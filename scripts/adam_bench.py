@@ -1,6 +1,6 @@
 """AdamW (+ fused polyak) streaming kernel variants on the flat parameter buffers of the bench workload (critic: 2 nets x 1024 replicas, 9 streams with
 the target update; actor: 7 streams), against a plain device copy of the same number of bytes. CUDA events, L2 flushed between launches.
-  python scripts/adam_bench.py > profiles/rN_adam_variants.jsonl"""
+  python scripts/adam_bench.py > adam_variants.jsonl"""
 import ctypes as C
 import json
 import os

@@ -1,6 +1,6 @@
 """Build-container only: times the reference's REAL train.train() (oracle/ref_train.py) against the restated oracle loop
 (oracle/loop.py, the `cpu_baseline` / `--impl reference` arm) on one CPU thread — GAIL hopper, B = 256, 200 update
-steps after 300 update-free steps. Result of round 1: profiles/r1_cpu_reference_calibration.json."""
+steps after 300 update-free steps."""
 import os
 import sys
 

@@ -1,6 +1,6 @@
 """Kernel micro-benchmarks asked for by SURVEY §8d beyond the headline loop: the GMMIL pairwise-RBF reward at B = 256 and B = 1024 (halfcheetah,
 1024 replicas), the PWIL coupling step, the GAIL update and the evaluation rollout. CUDA events, L2 flushed between timed launches, JSON lines.
-  python scripts/microbench.py > profiles/r2_microbench.jsonl"""
+  python scripts/microbench.py > microbench.jsonl"""
 import ctypes as C
 import json
 import os
@@ -13,7 +13,7 @@ import il_b200
 from il_b200 import _lib
 from il_b200.memory import TransitionBatch
 
-FP32_PEAK = 148 * 128 * 2 * 1.965e9 / 1e12  # TFLOP/s: 148 SMs x 128 FMA lanes x 2 flop x 1.965 GHz (non-tensor fp32)
+FP32_PEAK = 132 * 128 * 2 * 1.98e9 / 1e12  # TFLOP/s: 132 SMs x 128 FMA lanes x 2 flop x 1.98 GHz (non-tensor fp32, H100 SXM)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device='cuda')
 
 
@@ -21,7 +21,7 @@ def timed(fn, iters=10, warmup=3):
   for _ in range(warmup): fn()
   ms = []
   for _ in range(iters):
-    flush.zero_()  # > 126 MB L2
+    flush.zero_()  # > 50 MB L2
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record(); fn(); e1.record()
     torch.cuda.synchronize()

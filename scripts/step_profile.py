@@ -1,6 +1,6 @@
 """Per-kernel durations INSIDE the running step (CUPTI activity records through torch.profiler: no serialisation, no cache flush, the
 CUDA graph replays as in bench.py) — the complement of the ncu launch list, whose per-launch times are cold and serialised.
-  python scripts/step_profile.py [steps] > profiles/rN_step_kernel_times.json"""
+  python scripts/step_profile.py [steps] > step_kernel_times.json"""
 import collections
 import json
 import os

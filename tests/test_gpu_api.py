@@ -276,7 +276,7 @@ def test_evaluate_agent_many_episodes_uses_the_general_mlp_path():
 
 def test_evaluate_agent_on_the_tensor_core_engine_pads_rows_and_matches_fp32():
   """30 episodes per replica with 256-wide nets and gemm_mode tf32x3 (train.py:213 at the benchmarked configuration): the greedy forward pads every
-  replica's rows to the 128-row tcgen05 tile (zero rows, ignored) — same returns as the fp32 FFMA engine, which runs the 30 rows unpadded."""
+  replica's rows to the 128-row wgmma tile (zero rows, ignored) — same returns as the fp32 FFMA engine, which runs the 30 rows unpadded."""
   import il_b200
   from il_b200 import _lib
   from il_b200.environments import D4RLEnv

@@ -120,7 +120,7 @@ def test_loop_matches_oracle(algorithm, env_name, extra):
 
 
 def test_loop_matches_oracle_at_the_benchmarked_configuration():
-  """The configuration bench.py times (VERDICT r1 weak #1): 256-wide actor / critic, batch 256, dense layers on the 3xTF32 tcgen05
+  """The configuration bench.py times (VERDICT r1 weak #1): 256-wide actor / critic, batch 256, dense layers on the 3xTF32 wgmma
   engine (incl. the first layer fused into its producers), the whole iteration replayed as a CUDA graph — 62 steps, 32 of them
   updates, 2 replicas, every noise draw and index injected on both sides."""
   err = _run('GAIL', 'hopper', steps=62, start=30, B=256, H=256, graphs=True, gemm_mode='tf32x3')

@@ -1,4 +1,4 @@
-"""The tcgen05 (3xTF32 / TF32) dense-layer engine against the exact-fp32 FFMA engine and a float64 reference, on all
+"""The wgmma (3xTF32 / TF32) dense-layer engine against the exact-fp32 FFMA engine and a float64 reference, on all
 three operand layouts the MLP programs use (forward, input-gradient, weight-gradient) with their fused epilogues."""
 import ctypes as C
 
@@ -53,7 +53,7 @@ def test_tc_gemm_matches_fp64(layout, mode, tol):
 
 
 def test_tc_gemm_many_groups_persistent():
-  """More tiles than SMs: exercises the persistent tile loop, both TMEM accumulators and the stage ring wrap."""
+  """More tiles than SMs: several waves of CTAs, every tile written."""
   torch.manual_seed(1)
   G, M, N, K = 200, 256, 256, 256
   X = torch.randn(G, M, K, device='cuda')
@@ -85,10 +85,9 @@ def test_golden_cases_with_tensor_core_engine(name, monkeypatch):
 
 
 def test_fused_first_layer_is_schedule_independent():
-  """The producers of the tensor-core engine compute the first MLP layer (K0 = 12 / 15 columns) chunk by chunk into the
-  operand tile of the second. 80 replicas with IDENTICAL inputs put several tiles on every CTA pair (persistent loop,
-  double-buffered W1 staging, per-tile input rows): every replica must reproduce replica 0 bit for bit, and replica 0
-  must match the reference fixture."""
+  """The tensor-core engine computes the first MLP layer (K0 = 12 / 15 columns) chunk by chunk into the
+  operand tile of the second. 80 replicas with IDENTICAL inputs fill more than one wave of CTAs (per-tile W1 / input
+  staging): every replica must reproduce replica 0 bit for bit, and replica 0 must match the reference fixture."""
   from conftest import load_golden
   from cuda_cases import run_cuda
   from il_b200 import _lib
@@ -96,7 +95,7 @@ def test_fused_first_layer_is_schedule_independent():
   lib, h = _lib.lib(), _lib.handle()
   inp = cases.make_inputs('sac_hopper')
   _lib.check(lib.il_set_gemm_mode(h, _lib.GEMM_MODE['tf32x3']))
-  _lib.set_option('tc_fuse_l1', 1)  # off by default (measured slower than the separate K-thin launch); kept correct for A/B
+  _lib.set_option('tc_fuse_l1', 1)  # off by default; kept correct for A/B
   try:
     outs = run_cuda('sac_hopper', [inp] * 80)
   finally:
@@ -111,7 +110,7 @@ def test_fused_first_layer_is_schedule_independent():
 
 
 def test_sign_bit_masks_equal_fp32_masks():
-  """ReLU derivative masks as sign-bit words (written by the first-layer kernel and the fused-head tcgen05 epilogue, read by the masked dX launches)
+  """ReLU derivative masks as sign-bit words (written by the first-layer kernel and the fused-head wgmma epilogue, read by the masked dX launches)
   against fp32 activations as masks: the same `> 0` predicate on the same values, so one SAC update of the 256-wide fixture is bit-identical
   (option 1); with the input-gradient slice fused into the masked dX launch (option 2, the default) only the summation order of that thin product
   changes."""

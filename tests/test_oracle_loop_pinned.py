@@ -2,15 +2,14 @@
 built on — against the reference's REAL `train.train(cfg)`: the unmodified train.py / environments.py / memory.py /
 models.py / training.py / evaluation.py run end to end (oracle/ref_train.py stubs only hydra, plotting and `gym.make`,
 which returns the synthetic-environment twin) and the oracle loop, fed by the same global torch / numpy RNG streams,
-must arrive at the same parameters after the same number of steps. Build container only (needs /root/reference)."""
+must arrive at the same parameters after the same number of steps. What the reference's train() wrote is stored in
+tests/golden/reference.npz (python -m oracle.ref_golden regenerates it next to the reference tree)."""
 import numpy as np
 import pytest
 import torch
 
 from il_b200 import config
-from oracle import loop, refstub
-
-pytestmark = pytest.mark.skipif(not refstub.available(), reason='reference tree not present (GPU box)')
+from oracle import loop, ref_golden
 
 STEPS, MAX_EPISODE_STEPS, B, H, START = 60, 25, 16, 32, 8
 ATOL = 2e-6  # fp32, same torch CPU ops on both sides; observed 3e-8 after 60 steps
@@ -73,13 +72,15 @@ CONFIGS = [
 ]
 
 
-@pytest.mark.parametrize('algorithm,env,extra,kwargs', CONFIGS, ids=[f'{a}-{e}-{i}' for i, (a, e, _, _) in enumerate(CONFIGS)])
-def test_restated_loop_equals_the_reference_train_function(algorithm, env, extra, kwargs):
-  from oracle import ref_train
-  seed = 3
-  cfg = _cfg(algorithm, env, seed, extra)
+CONFIG_IDS = [f'{a}-{e}-{i}' for i, (a, e, _, _) in enumerate(CONFIGS)]
+LOOP_SEED = 3
+
+
+@pytest.mark.parametrize('case_id,algorithm,env,extra,kwargs', [(i, *c) for i, c in zip(CONFIG_IDS, CONFIGS)], ids=CONFIG_IDS)
+def test_restated_loop_equals_the_reference_train_function(case_id, algorithm, env, extra, kwargs):
+  seed = LOOP_SEED
   raw = loop.synthesize_raw_dataset(env, True, 5, MAX_EPISODE_STEPS)
-  ref = ref_train.run_reference_train(cfg, raw, MAX_EPISODE_STEPS)
+  ref = ref_golden.load_train_result(case_id)  # the reference's train(_cfg(algorithm, env, seed, extra)) on the same raw dataset
 
   threads = torch.get_num_threads()
   torch.set_num_threads(1)
@@ -126,15 +127,21 @@ def test_restated_loop_equals_the_reference_train_function(algorithm, env, extra
   _close('entropies', ref['metrics']['entropies'][-1], -ol.last['sac']['log_probs'])
 
 
-@pytest.mark.parametrize('algorithm,iterations', [('BC', 25), ('GAIL', 7)])
+BC_CONFIGS, BC_SEED, BC_ENV = [('BC', 25), ('GAIL', 7)], 5, 'hopper'
+
+
+def _bc_cfg(algorithm, iterations):
+  return _cfg(algorithm, BC_ENV, BC_SEED, [f'bc_pretraining.iterations={iterations}', 'bc_pretraining.learning_rate=0.001', 'bc_pretraining.weight_decay=0.01'])
+
+
+@pytest.mark.parametrize('algorithm,iterations', BC_CONFIGS)
 def test_bc_pretraining_equals_the_reference(algorithm, iterations):
   """train.py:95-115: BC on shuffled expert minibatches (the DataLoader's shuffling stream restated in OracleLoop.bc_pretrain);
   algorithm=BC returns after pretraining + evaluation, any other algorithm continues into the loop with the pretrained actor."""
-  from oracle import port, ref_train
-  seed, env = 5, 'hopper'
-  cfg = _cfg(algorithm, env, seed, [f'bc_pretraining.iterations={iterations}', 'bc_pretraining.learning_rate=0.001', 'bc_pretraining.weight_decay=0.01'])
+  from oracle import port
+  seed, env = BC_SEED, BC_ENV
   raw = loop.synthesize_raw_dataset(env, True, 5, MAX_EPISODE_STEPS)
-  ref = ref_train.run_reference_train(cfg, raw, MAX_EPISODE_STEPS)
+  ref = ref_golden.load_train_result(f'bc-{algorithm}-{iterations}')  # the reference's train(_bc_cfg(algorithm, iterations))
   threads = torch.get_num_threads()
   torch.set_num_threads(1)
   try:
