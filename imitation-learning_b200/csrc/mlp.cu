@@ -406,8 +406,40 @@ __global__ void __launch_bounds__(256) mlp_small_forward_kernel(const SmallFwdAr
   }
 }
 
+// Per-replica hyper-parameters of a streaming AdamW pass (hyper-parameter sweeps). R == 0: the scalar coefficients for every float.
+// Otherwise every CTA first builds a table of R coefficient sets in shared memory — with exactly the expressions of the scalar path, once
+// per replica — and each float4 looks up its replica (replica_floats is a multiple of 4, so a float4 never straddles two replicas).
+struct AdamReplicas {
+  const double* lr_r;
+  const double* wd_r;
+  const float* tau_r;
+  int64_t rf;     // floats per replica
+  float inv_rf;   // 1 / rf, for the replica estimate
+  int R;
+};
+struct AdamCoef { float step_size, decay, tau, one_minus_tau; };  // decay == 1: no weight decay (x * 1.0f == x, so this equals the has_wd test)
+constexpr int ADAM_MAX_REPLICAS = 2048;                           // table of 32 KB per CTA
+__device__ __forceinline__ void adam_fill_table(AdamCoef* tab, const AdamReplicas& rp, double lr, double wd, double beta1_d, const int64_t* step, float tau) {
+  if (!rp.R) return;
+  const double bc1 = 1.0 - pow(beta1_d, (double)*step);
+  for (int r = threadIdx.x; r < rp.R; r += blockDim.x) {
+    const double l = rp.lr_r ? rp.lr_r[r] : lr, w = rp.wd_r ? rp.wd_r[r] : wd;
+    const float t = rp.tau_r ? rp.tau_r[r] : tau;
+    tab[r] = AdamCoef{(float)(l / bc1), w != 0.0 ? (float)(1.0 - l * w) : 1.f, t, (float)(1.0 - (double)t)};
+  }
+}
+// replica of float f: a float estimate (relative error < 2^-21, R <= ADAM_MAX_REPLICAS) corrected by one step, no 64-bit division
+__device__ __forceinline__ int adam_replica(int64_t f, const AdamReplicas& rp) {
+  int r = (int)((float)f * rp.inv_rf);
+  if ((int64_t)r * rp.rf > f) --r;
+  else if ((int64_t)(r + 1) * rp.rf <= f) ++r;
+  return r;
+}
+
 __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, const int64_t* __restrict__ step,
-                            double lr, double beta1_d, double beta2_d, double eps_d, double wd, int64_t n, float* __restrict__ target, float tau, float one_minus_tau) {
+                            double lr, double beta1_d, double beta2_d, double eps_d, double wd, int64_t n, float* __restrict__ target, float tau, float one_minus_tau,
+                            const AdamReplicas rp) {
+  extern __shared__ AdamCoef adam_tab[];
   __shared__ float s_step_size, s_bc2_sqrt;
   if (threadIdx.x == 0) {  // torch _single_tensor_adam: Python-double scalars, then cast to the tensor dtype
     const double t = (double)*step;
@@ -415,35 +447,43 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
     s_step_size = (float)(lr / bc1);
     s_bc2_sqrt = (float)sqrt(bc2);
   }
+  adam_fill_table(adam_tab, rp, lr, wd, beta1_d, step, tau);
   __syncthreads();
   const float step_size = s_step_size, bc2_sqrt = s_bc2_sqrt;
   const float decay = (float)(1.0 - lr * wd), w1 = (float)(1.0 - beta1_d), w2 = (float)(1.0 - beta2_d);
   const float beta2 = (float)beta2_d, eps = (float)eps_d;
   const bool has_wd = wd != 0.0;
-  auto upd = [&](float& pi, float& mi, float& vi, float gi) {
-    if (has_wd) pi = __fmul_rn(pi, decay);                                     // param.mul_(1 - lr * weight_decay)
+  auto upd = [&](float& pi, float& mi, float& vi, float gi, float ss, float dc, bool wdf) {
+    if (wdf) pi = __fmul_rn(pi, dc);                                           // param.mul_(1 - lr * weight_decay)
     mi = __fadd_rn(mi, __fmul_rn(w1, __fsub_rn(gi, mi)));                      // exp_avg.lerp_(grad, 1 - beta1)
     vi = __fadd_rn(__fmul_rn(vi, beta2), __fmul_rn(__fmul_rn(w2, gi), gi));    // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value=1 - beta2)
     const float denom = __fadd_rn(__fdiv_rn(sqrtf(vi), bc2_sqrt), eps);        // (exp_avg_sq.sqrt() / bias_correction2_sqrt).add_(eps)
-    pi = __fadd_rn(pi, __fmul_rn(-step_size, __fdiv_rn(mi, denom)));           // param.addcdiv_(exp_avg, denom, value=-step_size)
+    pi = __fadd_rn(pi, __fmul_rn(-ss, __fdiv_rn(mi, denom)));                  // param.addcdiv_(exp_avg, denom, value=-step_size)
   };
   // n is a multiple of 4 and all buffers are 16-byte aligned (flat parameter layout): 128-bit streams
   const int64_t n4 = n >> 2;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    float ss = step_size, dc = decay, ta = tau, omt = one_minus_tau;
+    bool wdf = has_wd;
+    if (rp.R) {
+      const AdamCoef c = adam_tab[adam_replica(i << 2, rp)];
+      ss = c.step_size; dc = c.decay; wdf = c.decay != 1.f; ta = c.tau; omt = c.one_minus_tau;
+    }
     float4 pv = reinterpret_cast<float4*>(p)[i], mv = reinterpret_cast<float4*>(m)[i], vv = reinterpret_cast<float4*>(v)[i];
     const float4 gv = reinterpret_cast<const float4*>(g)[i];
-    upd(pv.x, mv.x, vv.x, gv.x); upd(pv.y, mv.y, vv.y, gv.y); upd(pv.z, mv.z, vv.z, gv.z); upd(pv.w, mv.w, vv.w, gv.w);
+    upd(pv.x, mv.x, vv.x, gv.x, ss, dc, wdf); upd(pv.y, mv.y, vv.y, gv.y, ss, dc, wdf); upd(pv.z, mv.z, vv.z, gv.z, ss, dc, wdf); upd(pv.w, mv.w, vv.w, gv.w, ss, dc, wdf);
     reinterpret_cast<float4*>(p)[i] = pv; reinterpret_cast<float4*>(m)[i] = mv; reinterpret_cast<float4*>(v)[i] = vv;
     if (target) {  // fused update_target_network (models.py:81)
+      const float tau = ta, one_minus_tau = omt;
       float4 tv = reinterpret_cast<float4*>(target)[i];
       tv.x = __fadd_rn(__fmul_rn(tv.x, tau), __fmul_rn(one_minus_tau, pv.x)); tv.y = __fadd_rn(__fmul_rn(tv.y, tau), __fmul_rn(one_minus_tau, pv.y));
       tv.z = __fadd_rn(__fmul_rn(tv.z, tau), __fmul_rn(one_minus_tau, pv.z)); tv.w = __fadd_rn(__fmul_rn(tv.w, tau), __fmul_rn(one_minus_tau, pv.w));
       reinterpret_cast<float4*>(target)[i] = tv;
     }
   }
-  for (int64_t i = (n4 << 2) + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {  // tail (< 4 elements)
+  for (int64_t i = (n4 << 2) + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {  // tail (< 4 elements; uniform only)
     float pi = p[i], mi = m[i], vi = v[i];
-    upd(pi, mi, vi, g[i]);
+    upd(pi, mi, vi, g[i], step_size, decay, has_wd);
     p[i] = pi; m[i] = mi; v[i] = vi;
     if (target) target[i] = __fadd_rn(__fmul_rn(target[i], tau), __fmul_rn(one_minus_tau, pi));
   }
@@ -470,13 +510,15 @@ __device__ __forceinline__ void adam_mbar_wait(uint32_t bar, uint32_t parity) {
 template <int TILE, int STAGES>
 __global__ void __launch_bounds__(ADAM_CONSUMERS + 32) adam_tma_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
                                                                       const int64_t* __restrict__ step, double lr, double beta1_d, double beta2_d, double eps_d, double wd, int64_t n,
-                                                                      float* __restrict__ target, float tau, float one_minus_tau) {
+                                                                      float* __restrict__ target, float tau, float one_minus_tau, const AdamReplicas rp) {
   extern __shared__ __align__(128) uint8_t adam_smem[];
   float* buf = reinterpret_cast<float*>(adam_smem);                                  // [stage][stream][TILE]
+  AdamCoef* tab = reinterpret_cast<AdamCoef*>(adam_smem + adam_tma_smem<TILE, STAGES>());  // per-replica coefficients behind the ring
   const uint32_t smem0 = (uint32_t)__cvta_generic_to_shared(buf);
   const uint32_t full0 = smem0 + (uint32_t)(STAGES * ADAM_STREAMS * TILE * 4), done0 = full0 + 8u * STAGES;  // full[stage] (tx bytes), done[stage] (256 compute threads)
   __shared__ float s_step_size, s_bc2_sqrt;
   const int tid = threadIdx.x;
+  adam_fill_table(tab, rp, lr, wd, beta1_d, step, tau);
   if (tid == 0) {
     const double t = (double)*step;
     s_step_size = (float)(lr / (1.0 - pow(beta1_d, t)));
@@ -529,12 +571,12 @@ __global__ void __launch_bounds__(ADAM_CONSUMERS + 32) adam_tma_kernel(float* __
   const float step_size = s_step_size, bc2_sqrt = s_bc2_sqrt;
   const float decay = (float)(1.0 - lr * wd), w1 = (float)(1.0 - beta1_d), w2 = (float)(1.0 - beta2_d), beta2 = (float)beta2_d, eps = (float)eps_d;
   const bool has_wd = wd != 0.0;
-  auto upd = [&](float& pi, float& mi, float& vi, float gi) {
-    if (has_wd) pi = __fmul_rn(pi, decay);
+  auto upd = [&](float& pi, float& mi, float& vi, float gi, float ss, float dc, bool wdf) {
+    if (wdf) pi = __fmul_rn(pi, dc);
     mi = __fadd_rn(mi, __fmul_rn(w1, __fsub_rn(gi, mi)));
     vi = __fadd_rn(__fmul_rn(vi, beta2), __fmul_rn(__fmul_rn(w2, gi), gi));
     const float denom = __fadd_rn(__fdiv_rn(sqrtf(vi), bc2_sqrt), eps);
-    pi = __fadd_rn(pi, __fmul_rn(-step_size, __fdiv_rn(mi, denom)));
+    pi = __fadd_rn(pi, __fmul_rn(-ss, __fdiv_rn(mi, denom)));
   };
   for (int64_t k = 0; k < my_tiles; ++k) {
     const int stage = (int)(k % STAGES);
@@ -547,11 +589,18 @@ __global__ void __launch_bounds__(ADAM_CONSUMERS + 32) adam_tma_kernel(float* __
     float4* sv = reinterpret_cast<float4*>(buf + (stage * ADAM_STREAMS + 3) * TILE);
     float4* stg = reinterpret_cast<float4*>(buf + (stage * ADAM_STREAMS + 4) * TILE);
     for (int i = tid; i < nf4; i += ADAM_CONSUMERS) {
+      float ss = step_size, dc = decay, ta = tau, omt = one_minus_tau;
+      bool wdf = has_wd;
+      if (rp.R) {  // a tile may straddle replica boundaries: look up per float4
+        const AdamCoef c = tab[adam_replica(tile * TILE + 4 * i, rp)];
+        ss = c.step_size; dc = c.decay; wdf = c.decay != 1.f; ta = c.tau; omt = c.one_minus_tau;
+      }
       float4 pv = sp[i], mv = smm[i], vv = sv[i];
       const float4 gv = sg[i];
-      upd(pv.x, mv.x, vv.x, gv.x); upd(pv.y, mv.y, vv.y, gv.y); upd(pv.z, mv.z, vv.z, gv.z); upd(pv.w, mv.w, vv.w, gv.w);
+      upd(pv.x, mv.x, vv.x, gv.x, ss, dc, wdf); upd(pv.y, mv.y, vv.y, gv.y, ss, dc, wdf); upd(pv.z, mv.z, vv.z, gv.z, ss, dc, wdf); upd(pv.w, mv.w, vv.w, gv.w, ss, dc, wdf);
       sp[i] = pv; smm[i] = mv; sv[i] = vv;
       if (target) {  // fused update_target_network (models.py:81)
+        const float tau = ta, one_minus_tau = omt;
         float4 tv = stg[i];
         tv.x = __fadd_rn(__fmul_rn(tv.x, tau), __fmul_rn(one_minus_tau, pv.x)); tv.y = __fadd_rn(__fmul_rn(tv.y, tau), __fmul_rn(one_minus_tau, pv.y));
         tv.z = __fadd_rn(__fmul_rn(tv.z, tau), __fmul_rn(one_minus_tau, pv.z)); tv.w = __fadd_rn(__fmul_rn(tv.w, tau), __fmul_rn(one_minus_tau, pv.w));
@@ -564,11 +613,16 @@ __global__ void __launch_bounds__(ADAM_CONSUMERS + 32) adam_tma_kernel(float* __
 }
 
 template <int TILE, int STAGES>
-static int launch_adam_tma(il_handle* h, int ctas_per_sm, float* params, const float* grads, const il_adam* opt, int64_t n, cudaStream_t stream, float* polyak_target, float polyak_factor) {
+static int launch_adam_tma(il_handle* h, int ctas_per_sm, float* params, const float* grads, const il_adam* opt, int64_t n, cudaStream_t stream, float* polyak_target, float polyak_factor,
+                           const AdamReplicas& rp) {
   static bool attr_set = false;
-  if (!attr_set) { IL_CUDA(cudaFuncSetAttribute(adam_tma_kernel<TILE, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, adam_tma_smem<TILE, STAGES>())); attr_set = true; }
-  IL_LAUNCH(h, (adam_tma_kernel<TILE, STAGES>), h->sm_count * ctas_per_sm, ADAM_CONSUMERS + 32, (adam_tma_smem<TILE, STAGES>()), stream, params, grads, opt->m, opt->v, opt->step, opt->lr, opt->beta1,
-            opt->beta2, opt->eps, opt->weight_decay, n, polyak_target, polyak_factor, (float)(1.0 - (double)polyak_factor));
+  if (!attr_set) {
+    IL_CUDA(cudaFuncSetAttribute(adam_tma_kernel<TILE, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, adam_tma_smem<TILE, STAGES>() + ADAM_MAX_REPLICAS * (int)sizeof(AdamCoef)));
+    attr_set = true;
+  }
+  const size_t smem = (size_t)adam_tma_smem<TILE, STAGES>() + (size_t)rp.R * sizeof(AdamCoef);
+  IL_LAUNCH(h, (adam_tma_kernel<TILE, STAGES>), h->sm_count * ctas_per_sm, ADAM_CONSUMERS + 32, smem, stream, params, grads, opt->m, opt->v, opt->step, opt->lr, opt->beta1,
+            opt->beta2, opt->eps, opt->weight_decay, n, polyak_target, polyak_factor, (float)(1.0 - (double)polyak_factor), rp);
   return 0;
 }
 constexpr int ADAM_TMA_MIN_TILES = 4096;        // floats per CTA-iteration below which the plain kernel is used
@@ -714,26 +768,34 @@ int launch_actor_head(il_handle* h, const HeadFwdArgs& a, cudaStream_t stream) {
   return 0;
 }
 
-int launch_adam(il_handle* h, float* params, const float* grads, const il_adam* opt, int64_t n, cudaStream_t stream, float* polyak_target, float polyak_factor) {
+int launch_adam(il_handle* h, float* params, const float* grads, const il_adam* opt, int64_t n, cudaStream_t stream, float* polyak_target, float polyak_factor,
+                const float* polyak_r) {
   IL_CHECK(opt->m && opt->v && opt->step, "adam: null state");
   IL_CHECK(((reinterpret_cast<uintptr_t>(params) | reinterpret_cast<uintptr_t>(grads) | reinterpret_cast<uintptr_t>(opt->m) | reinterpret_cast<uintptr_t>(opt->v) |
              reinterpret_cast<uintptr_t>(polyak_target)) & 15) == 0, "adam: buffers must be 16-byte aligned");
+  AdamReplicas rp{opt->lr_r, opt->weight_decay_r, polyak_target ? polyak_r : nullptr, 0, 0.f, 0};
+  if (rp.lr_r || rp.wd_r || rp.tau_r) {
+    const int64_t rf = opt->replica_floats;
+    IL_CHECK(rf > 0 && rf % 4 == 0 && n % rf == 0, "adam: per-replica hyper-parameters need replica_floats (%lld) > 0, a multiple of 4 dividing n = %lld", (long long)rf, (long long)n);
+    IL_CHECK(n / rf <= ADAM_MAX_REPLICAS, "adam: %lld replicas with per-replica hyper-parameters exceed the limit of %d per buffer", (long long)(n / rf), ADAM_MAX_REPLICAS);
+    rp.rf = rf; rp.inv_rf = 1.f / (float)rf; rp.R = (int)(n / rf);
+  }
   if (h->adam_tma && n % 4 == 0 && n >= (int64_t)ADAM_TMA_MIN_TILES * h->sm_count * 2) {  // large flat buffers: TMA-staged streaming variant
     // The default is the 2-CTA-per-SM 2048 x 2 ring: its CTAs co-reside with the tail of the previous kernel and the head of the next
     // (scripts/adam_bench.py times the geometries in isolation).
     const int variant = h->adam_tma;
     switch (variant) {  // (tile floats, stages, CTAs per SM): 20 B/float of shared memory per stage
-      case 2: return launch_adam_tma<4096, 2>(h, 1, params, grads, opt, n, stream, polyak_target, polyak_factor);
-      case 3: return launch_adam_tma<2048, 3>(h, 1, params, grads, opt, n, stream, polyak_target, polyak_factor);
-      case 4: return launch_adam_tma<1024, 4>(h, 2, params, grads, opt, n, stream, polyak_target, polyak_factor);
-      case 5: return launch_adam_tma<1024, 3>(h, 3, params, grads, opt, n, stream, polyak_target, polyak_factor);
-      case 6: return launch_adam_tma<512, 4>(h, 4, params, grads, opt, n, stream, polyak_target, polyak_factor);
-      case 7: return launch_adam_tma<2048, 4>(h, 1, params, grads, opt, n, stream, polyak_target, polyak_factor);
-      default: return launch_adam_tma<2048, 2>(h, 2, params, grads, opt, n, stream, polyak_target, polyak_factor);
+      case 2: return launch_adam_tma<4096, 2>(h, 1, params, grads, opt, n, stream, polyak_target, polyak_factor, rp);
+      case 3: return launch_adam_tma<2048, 3>(h, 1, params, grads, opt, n, stream, polyak_target, polyak_factor, rp);
+      case 4: return launch_adam_tma<1024, 4>(h, 2, params, grads, opt, n, stream, polyak_target, polyak_factor, rp);
+      case 5: return launch_adam_tma<1024, 3>(h, 3, params, grads, opt, n, stream, polyak_target, polyak_factor, rp);
+      case 6: return launch_adam_tma<512, 4>(h, 4, params, grads, opt, n, stream, polyak_target, polyak_factor, rp);
+      case 7: return launch_adam_tma<2048, 4>(h, 1, params, grads, opt, n, stream, polyak_target, polyak_factor, rp);
+      default: return launch_adam_tma<2048, 2>(h, 2, params, grads, opt, n, stream, polyak_target, polyak_factor, rp);
     }
   }
-  IL_LAUNCH(h, adam_kernel, ew_blocks(n / 4 + 1, 256, h->sm_count), 256, 0, stream, params, grads, opt->m, opt->v, opt->step, opt->lr, opt->beta1, opt->beta2, opt->eps,
-            opt->weight_decay, n, polyak_target, polyak_factor, (float)(1.0 - (double)polyak_factor));
+  IL_LAUNCH(h, adam_kernel, ew_blocks(n / 4 + 1, 256, h->sm_count), 256, (size_t)rp.R * sizeof(AdamCoef), stream, params, grads, opt->m, opt->v, opt->step, opt->lr, opt->beta1, opt->beta2,
+            opt->eps, opt->weight_decay, n, polyak_target, polyak_factor, (float)(1.0 - (double)polyak_factor), rp);
   return 0;
 }
 
@@ -830,6 +892,12 @@ extern "C" int il_adam_step_polyak(il_handle* h, float* params, const float* gra
   IL_CHECK(h && params && grads && opt && target, "il_adam_step_polyak: null argument");
   IL_TRY(launch_tick(h, opt->step, nullptr, nullptr, (cudaStream_t)stream));
   return launch_adam(h, params, grads, opt, n, (cudaStream_t)stream, target, polyak_factor);
+}
+
+extern "C" int il_adam_step_polyak_r(il_handle* h, float* params, const float* grads, const il_adam* opt, int64_t n, float* target, const float* polyak_r, void* stream) {
+  IL_CHECK(h && params && grads && opt && target && polyak_r, "il_adam_step_polyak_r: null argument");
+  IL_TRY(launch_tick(h, opt->step, nullptr, nullptr, (cudaStream_t)stream));
+  return launch_adam(h, params, grads, opt, n, (cudaStream_t)stream, target, 0.f, polyak_r);
 }
 
 extern "C" int il_polyak(il_handle* h, float* target, const float* online, int64_t n, float polyak_factor, void* stream) {

@@ -323,9 +323,12 @@ class GAILDiscriminator(_Module):
   """:152-180. Accelerated configuration: the depth-1 relu `g` network of conf/algorithm/GAIL.yaml (no reward
   shaping / log-policy subtraction), with or without spectral norm."""
 
-  def __init__(self, state_size: int, action_size: int, imitation_cfg, discount: float, replicas: int = 1, rng: Optional[ReplicaRNG] = None, device=None):
+  def __init__(self, state_size: int, action_size: int, imitation_cfg, discount, replicas: int = 1, rng: Optional[ReplicaRNG] = None, device=None):
     model_cfg = imitation_cfg.discriminator
-    self.discount, self.state_only = discount, bool(imitation_cfg.state_only)
+    self.state_only = bool(imitation_cfg.state_only)
+    # reward-shaping discount (models.py:174): a float, or one value per replica (an [R] float32 device tensor, hyper-parameter sweeps)
+    self.discount = discount if isinstance(discount, (int, float)) else \
+        torch.as_tensor(discount, dtype=torch.float32).to(torch.device('cuda') if device is None else torch.device(device)).reshape(replicas).contiguous()
     self.reward_shaping, self.subtract_log_policy, self.reward_function = bool(model_cfg.reward_shaping), bool(model_cfg.subtract_log_policy), model_cfg.reward_function
     self.state_size, self.action_size, self.replicas = state_size, action_size, replicas
     self.spectral_norm = bool(imitation_cfg.spectral_norm)
@@ -420,7 +423,9 @@ class GAILDiscriminator(_Module):
     if self.spectral_norm:
       d.g_u, d.g_v, d.g_u_stride, d.g_v_stride = self.g_u.data_ptr(), self.g_v.data_ptr(), self.g_u.stride(0), self.g_v.stride(0)
       if self.h_mlp is not None: d.h_u, d.h_v, d.h_u_stride, d.h_v_stride = self.h_u.data_ptr(), self.h_v.data_ptr(), self.h_u.stride(0), self.h_v.stride(0)
-    d.state_only, d.reward_function, d.subtract_log_policy, d.discount = int(self.state_only), _lib.REWARD[self.reward_function], int(self.subtract_log_policy), self.discount
+    d.state_only, d.reward_function, d.subtract_log_policy = int(self.state_only), _lib.REWARD[self.reward_function], int(self.subtract_log_policy)
+    if isinstance(self.discount, (int, float)): d.discount = self.discount
+    else: d.discount_r = self.discount.data_ptr()  # per-replica shaping discount: an [R] float32 device tensor
     return d
 
   def _general_state_items(self):

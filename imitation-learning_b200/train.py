@@ -4,6 +4,9 @@
 calls on one CUDA stream with every piece of per-step state (env state, replay ring indices, optimiser step
 counts, RNG counters, the `step` counter) resident on the device — so both sequences are captured once as CUDA
 graphs and replayed without host involvement. Replica r is a reference-equivalent run with seed `cfg.seed + r`.
+
+`Trainer(per_replica={key: R values})` gives the replicas their own values of the shape-preserving hyper-parameters
+(config.VECTORISED); `main` runs a multirun sweep (`-m key=a,b,...`) as groups of such Trainers, one replica block per job.
 """
 from __future__ import annotations
 
@@ -11,14 +14,14 @@ import ctypes as C
 import os
 import sys
 import time
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 import torch
 from torch import Tensor
 
 from . import _lib, distributed
-from .config import Config, load_config
+from .config import Config, SweepJob, expand_sweep, get_key, group_jobs, load_config, split_per_replica
 from .environments import D4RLEnv, ENVS
 from .evaluation import evaluate_agent
 from .memory import ReplayMemory, TransitionBatch
@@ -56,10 +59,17 @@ def check_config(cfg: Config):
 
 
 class Trainer:
-  def __init__(self, cfg: Config, replicas: Optional[int] = None, seed_offset: int = 0, fast_init: bool = False, device=None):
+  def __init__(self, cfg: Config, replicas: Optional[int] = None, seed_offset: int = 0, fast_init: bool = False, device=None,
+               per_replica: Optional[Dict[str, Sequence[float]]] = None):
+    """per_replica: dotted config key (config.VECTORISED) -> R values, replica r training with value r; a key whose values are all equal
+    runs as that scalar. None: every replica uses the config's values."""
+    R = int(cfg.get('replicas', 1) if replicas is None else replicas)
+    self.per_replica: Dict[str, List[float]] = {}
+    if per_replica: cfg, self.per_replica = split_per_replica(cfg, per_replica, R)
+    for k in ('imitation.grad_penalty', 'imitation.entropy_bonus'): assert min(self.per_replica.get(k, [0.0])) >= 0, k  # train.py:48-49
     check_config(cfg)
     self.cfg = cfg
-    self.R = R = int(cfg.get('replicas', 1) if replicas is None else replicas)
+    self.R = R
     self.device = dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
     self.lib, self.h = _lib.lib(), _lib.handle(dev.index)
     _lib.check(self.lib.il_set_gemm_mode(self.h, _lib.GEMM_MODE[cfg.get('gemm_mode', 'fp32')]))
@@ -87,7 +97,17 @@ class Trainer:
     if fast_init and R > 1: self._replicate()
     self.log_alpha = torch.zeros(R, device=dev)
     self.target_critic, self.entropy_target = create_target_network(self.critic), cfg.reinforcement.target_temperature * A
-    lr, wd = cfg.training.learning_rate, cfg.training.weight_decay
+    # per-replica values: float64 lists for the optimisers (Python floats in the reference), float32 device tensors for the kernels, each
+    # rounded once from the double the scalar path computes
+    pr, f32 = self.per_replica, lambda vals: torch.tensor(vals, dtype=torch.float32, device=dev)
+    if 'reinforcement.target_temperature' in pr: self.entropy_target = f32([float(t) * A for t in pr['reinforcement.target_temperature']])
+    self.discount = f32(pr['reinforcement.discount']) if 'reinforcement.discount' in pr else cfg.reinforcement.discount
+    self.polyak_factor = f32(pr['reinforcement.polyak_factor']) if 'reinforcement.polyak_factor' in pr else cfg.reinforcement.polyak_factor
+    self.imitation_cfg = Config(dict(cfg.imitation, **{k.split('.')[1]: f32(pr[k]) for k in ('imitation.grad_penalty', 'imitation.entropy_bonus') if k in pr}))
+    self._grad_penalty_on = max(pr.get('imitation.grad_penalty', [cfg.imitation.get('grad_penalty', 0)])) > 0  # GAIL only (GAIL.yaml)
+    if self.algorithm == 'GAIL' and isinstance(self.discount, Tensor): self.discriminator.discount = self.discount  # reward shaping (models.py:174)
+    hp = lambda k: pr.get(k, get_key(cfg, k))
+    lr, wd = hp('training.learning_rate'), hp('training.weight_decay')
     self.actor_optimiser, self.critic_optimiser = AdamW(self.actor.parameters(), lr=lr, weight_decay=wd), AdamW(self.critic.parameters(), lr=lr, weight_decay=wd)
     self.temperature_optimiser = Adam([self.log_alpha], lr=lr)
     need = R * int(cfg.memory.size) * _lib.py_row_layout(S, A)[1] * 4
@@ -99,7 +119,7 @@ class Trainer:
     self.memory.seed = seed
     # train.py:70-84
     if self.algorithm in ('DRIL', 'GAIL', 'RED'):
-      self.discriminator_optimiser = AdamW(self.discriminator.parameters(), lr=cfg.imitation.learning_rate, weight_decay=cfg.imitation.weight_decay)  # train.py:83-84
+      self.discriminator_optimiser = AdamW(self.discriminator.parameters(), lr=hp('imitation.learning_rate'), weight_decay=hp('imitation.weight_decay'))  # train.py:83-84
     if self.algorithm == 'GAIL':
       self.discriminator.eval()  # train.py:147
     elif self.algorithm == 'AdRIL':
@@ -215,14 +235,14 @@ class Trainer:
       self.expert_memory.gather(self.idx_exp, out=self.expert_batch)
     if self.algorithm == 'GAIL':
       from .training import adversarial_imitation_update
-      if cfg.imitation.grad_penalty > 0 and not self.inject: self.rng.uniform(None, self.device, stream_id=5, out=self.eps_gp)
+      if self._grad_penalty_on and not self.inject: self.rng.uniform(None, self.device, stream_id=5, out=self.eps_gp)
       eps_mix = None
       if cfg.imitation.loss_function == 'Mixup':  # training.py:106: Beta(a, a) draws; a == 1 (all published configs) is U(0, 1)
         if float(cfg.imitation.mixup_alpha) != 1.0: raise NotImplementedError('mixup_alpha != 1 needs Beta draws; only mixup_alpha = 1 (the reference default) is on the graph-captured path')
         if not self.inject: self.rng.uniform(None, self.device, stream_id=8, out=self.eps_mix)
         eps_mix = self.eps_mix
       self.discriminator.train()  # train.py:178-180
-      adversarial_imitation_update(self.actor, self.discriminator, self.batch, self.expert_batch, self.discriminator_optimiser, cfg.imitation, eps_gp=self.eps_gp,
+      adversarial_imitation_update(self.actor, self.discriminator, self.batch, self.expert_batch, self.discriminator_optimiser, self.imitation_cfg, eps_gp=self.eps_gp,
                                    eps_mix=eps_mix, out_losses=self.gail_losses)
       self.discriminator.eval()
     if self.algorithm in ('GAIL', 'GMMIL'):
@@ -250,7 +270,7 @@ class Trainer:
       self.rng.normal(None, self.device, stream_id=6, out=self.eps_next)
       self.rng.normal(None, self.device, stream_id=7, out=self.eps_new)
     sac_update(self.actor, self.critic, self.log_alpha, self.target_critic, self.batch, self.actor_optimiser, self.critic_optimiser, self.temperature_optimiser,
-               cfg.reinforcement.discount, self.entropy_target, cfg.reinforcement.polyak_factor, eps_next=self.eps_next, eps_new=self.eps_new, out=self.sac_out)  # train.py:203
+               self.discount, self.entropy_target, self.polyak_factor, eps_next=self.eps_next, eps_new=self.eps_new, out=self.sac_out)  # train.py:203
 
   def bc_pretrain(self, iterations: Optional[int] = None) -> Tensor:
     """train.py:93-99: `iterations` behavioural-cloning steps on epoch-wise shuffled expert minibatches (drop_last), with a
@@ -259,7 +279,9 @@ class Trainer:
     from .training import behavioural_cloning_update
     cfg, B, n = self.cfg, self.B, self.expert_memory.size
     iterations = cfg.bc_pretraining.iterations if iterations is None else iterations
-    opt = AdamW(self.actor.parameters(), lr=cfg.bc_pretraining.learning_rate, weight_decay=cfg.bc_pretraining.weight_decay)
+    pr = self.per_replica
+    opt = AdamW(self.actor.parameters(), lr=pr.get('bc_pretraining.learning_rate', cfg.bc_pretraining.learning_rate),
+                weight_decay=pr.get('bc_pretraining.weight_decay', cfg.bc_pretraining.weight_decay))
     loss = torch.zeros(self.R, device=self.device)
     per_epoch = max(n // B, 1)
     perm = None
@@ -371,60 +393,123 @@ class Trainer:
     return dict(actor=self.actor.state_dict(), critic=self.critic.state_dict(), log_alpha=self.log_alpha.detach().clone().cpu())
 
 
+def _block(x, lo: int, hi: int, total: int):
+  """Replicas [lo, hi) of an output that a single-replica run writes without its replica axis (the reference's shapes)."""
+  if total == 1 or lo is None: return x
+  if isinstance(x, dict): return {k: _block(v, lo, hi, total) for k, v in x.items()}
+  return x[lo] if hi - lo == 1 else x[lo:hi]
+
+
 def train(cfg: Config, file_prefix: str = '') -> float:
   """train.py:26-243 (accelerated algorithms). Multi-GPU: launched one process per GPU (torch.distributed.run); the
   replica axis is split across ranks and evaluation returns are reduced over NCCL (distributed.py)."""
+  return _train(cfg, [(file_prefix, '', None, None)])[0]
+
+
+def _train(cfg: Config, blocks, per_replica: Optional[Dict[str, Sequence[float]]] = None) -> List[float]:
+  """The loop of train(). `blocks`: (file prefix, console label, lo, hi) per output set; lo = None is the whole run (and its shards
+  across ranks), otherwise replicas [lo, hi) of a single-rank run — one job of a sweep, written and scored as its own run."""
   rank, world = distributed.init('nccl')
   total = int(cfg.get('replicas', 1))
   lo, hi = distributed.shard(total, rank, world)
-  trainer = Trainer(cfg, replicas=hi - lo, seed_offset=lo)
-  metrics, score = trainer.metrics, trainer.score
+  trainer = Trainer(cfg, replicas=hi - lo, seed_offset=lo, per_replica=per_replica)
+  metrics, scores = trainer.metrics, [[] for _ in blocks]
+  cut = lambda x, b: _block(x, b[2], b[3], total)
+  part = lambda x, b: x if b[2] is None else x[b[2]:b[3]]  # outputs that keep the replica axis at one replica
+  flat_of = lambda b: (total if b[2] is None else b[3] - b[2]) == 1  # the reference's schema for a single replica (train.py:214-219)
+  stats_of = lambda returns, b: distributed.return_statistics(returns if b[2] is None else returns[b[2]:b[3]])
   start_time = time.time()
   if cfg.bc_pretraining.iterations > 0:  # train.py:93-112
     trainer.bc_pretrain()
     if cfg.algorithm == 'BC':
       returns = trainer.evaluate()
-      mean, std, n = distributed.return_statistics(returns)
       normalized = (returns.cpu().numpy() - trainer.normalization_min) / (trainer.normalization_max - trainer.normalization_min)
-      flat = total == 1
-      metrics['test_steps'], metrics['test_returns'], metrics['test_returns_normalized'] = [0], [returns.cpu().numpy().reshape(-1).tolist() if flat else returns.cpu().numpy().tolist()], \
-          [normalized.reshape(-1).tolist() if flat else normalized.tolist()]
-      if rank == 0:
-        print(f'BC: test return {mean:.3f} +- {std:.3f} over {n} episodes', flush=True)
-        torch.save(dict(actor=trainer.actor.state_dict()), f'{file_prefix}agent.pth')  # train.py:108
-        torch.save(metrics, f'{file_prefix}metrics.pth')
-      return float(np.mean(normalized))
+      out = []
+      for b in blocks:
+        mean, std, n = stats_of(returns, b)
+        r_b, n_b, flat = cut(returns.cpu().numpy(), b), cut(normalized, b), flat_of(b)
+        m = dict(metrics, test_steps=[0], test_returns=[r_b.reshape(-1).tolist() if flat else r_b.tolist()], test_returns_normalized=[n_b.reshape(-1).tolist() if flat else n_b.tolist()])
+        if rank == 0:
+          print(f'{b[1]}BC: test return {mean:.3f} +- {std:.3f} over {n} episodes', flush=True)
+          torch.save(dict(actor=cut(trainer.actor.state_dict(), b)), f'{b[0]}agent.pth')  # train.py:108
+          torch.save(m, f'{b[0]}metrics.pth')
+        out.append(float(np.mean(n_b)))
+      return out
   if cfg.algorithm in ('DRIL', 'RED'): trainer.pretrain_discriminator()  # train.py:117-133
   for step in range(1, cfg.steps + 1):
     trainer.train_step()
     if cfg.logging.interval > 0 and step % cfg.logging.interval == 0 and trainer._will_update(step): trainer.log_aux()  # train.py:205: only inside the update branch
     if step % cfg.evaluation.interval == 0 and not cfg.check_time_usage:  # train.py:213
       returns = trainer.evaluate()
-      mean, std, n = distributed.return_statistics(returns)
       normalized = (returns.cpu().numpy() - trainer.normalization_min) / (trainer.normalization_max - trainer.normalization_min)
-      score.append(float((mean - trainer.normalization_min) / (trainer.normalization_max - trainer.normalization_min)))
       metrics['test_steps'].append(step)
-      flat = total == 1  # the reference's schema: one list of `episodes` floats per evaluation (train.py:214-219); R > 1 keeps [R][episodes]
-      metrics['test_returns'].append(returns.cpu().numpy().reshape(-1).tolist() if flat else returns.cpu().numpy().tolist())
-      metrics['test_returns_normalized'].append(normalized.reshape(-1).tolist() if flat else normalized.tolist())
-      if rank == 0: print(f'step {step}: test return {mean:.3f} +- {std:.3f} over {n} episodes ({world} rank(s))', flush=True)
+      for i, b in enumerate(blocks):
+        mean, std, n = stats_of(returns, b)
+        scores[i].append(float((mean - trainer.normalization_min) / (trainer.normalization_max - trainer.normalization_min)))
+        r_b, n_b, flat = cut(returns.cpu().numpy(), b), cut(normalized, b), flat_of(b)
+        metrics.setdefault('_blocks', [dict(test_returns=[], test_returns_normalized=[]) for _ in blocks])
+        metrics['_blocks'][i]['test_returns'].append(r_b.reshape(-1).tolist() if flat else r_b.tolist())
+        metrics['_blocks'][i]['test_returns_normalized'].append(n_b.reshape(-1).tolist() if flat else n_b.tolist())
+        if rank == 0: print(f'{b[1]}step {step}: test return {mean:.3f} +- {std:.3f} over {n} episodes ({world} rank(s))', flush=True)
+  trainer.score = scores[0]
   if cfg.check_time_usage: metrics['training_time'] = time.time() - start_time  # train.py:229-230
   eps = trainer.episodes.cpu().numpy()
-  metrics['train_returns'] = (trainer.return_sum.cpu().numpy() / np.maximum(eps, 1)).tolist()
+  metrics['train_returns'] = trainer.return_sum.cpu().numpy() / np.maximum(eps, 1)
+  trajectories = None
   if cfg.save_trajectories:  # train.py:232-235: trajectories of the trained agent (every rank writes its own shard of the replica axis; rank 0 keeps the reference's file name)
     if cfg.render: raise NotImplementedError('render=true needs a PyBullet window (environments.py:52-53); the synthetic device env has none')
     _, trajectories = evaluate_agent(trainer.actor, trainer.eval_env, cfg.evaluation.episodes, return_trajectories=True)
-    torch.save(trajectories, f'{file_prefix}trajectories.pth' if rank == 0 else f'{file_prefix}trajectories.rank{rank}.pth')
-  if rank == 0:  # train.py:237-239
-    torch.save(trainer.state_dicts(), f'{file_prefix}agent.pth')
-    if cfg.algorithm in ('DRIL', 'GAIL', 'RED'): torch.save(trainer.discriminator.state_dict(), f'{file_prefix}discriminator.pth')  # train.py:238
-    torch.save(metrics, f'{file_prefix}metrics.pth')
-  return float(np.mean(score)) if score else float('nan')
+  per_block = metrics.pop('_blocks', [dict(test_returns=[], test_returns_normalized=[]) for _ in blocks])
+  for i, b in enumerate(blocks):
+    m = {k: ([cut(x, b) for x in v] if k == 'predicted_rewards' else [part(x, b) for x in v] if k in ('alphas', 'entropies', 'Q_values') else v) for k, v in metrics.items()}
+    m.update(per_block[i], train_returns=part(metrics['train_returns'], b).tolist())
+    if trajectories is not None: torch.save(cut(trajectories, b), f'{b[0]}trajectories.pth' if rank == 0 else f'{b[0]}trajectories.rank{rank}.pth')
+    if rank == 0:  # train.py:237-239
+      sd = trainer.state_dicts()
+      torch.save(dict(actor=cut(sd['actor'], b), critic=cut(sd['critic'], b), log_alpha=part(sd['log_alpha'], b)), f'{b[0]}agent.pth')
+      if cfg.algorithm in ('DRIL', 'GAIL', 'RED'): torch.save(cut(trainer.discriminator.state_dict(), b), f'{b[0]}discriminator.pth')  # train.py:238
+      torch.save(m, f'{b[0]}metrics.pth')
+  return [float(np.mean(sc)) if sc else float('nan') for sc in scores]
 
 
-def main(argv: Optional[List[str]] = None) -> float:
-  """`python train.py algorithm=<ALG> env=<ENV> [key=value ...]` (train.py:21-23, 246)."""
-  cfg = load_config(sys.argv[1:] if argv is None else argv)
+def run_sweep(jobs: List[SweepJob]) -> List[float]:
+  """A multirun on one GPU: the jobs are partitioned into groups (config.group_jobs); a group of J jobs is exactly the run
+  `train.py <group overrides> replicas=J*R` with job j's vectorised values given to replica block [jR, (j+1)R) — so replica jR+k starts
+  like a run with seed `seed + jR + k`. Groups run one after another. Job j writes the single-run files of its replicas, plus
+  overrides.yaml, to <output_dir>/<ALG>_<ENV>_sweeper/<timestamp>/<j>/ (hydra.sweep.dir). Returns the per-job scores."""
+  import yaml
+  if int(os.environ.get('WORLD_SIZE', '1')) > 1: raise NotImplementedError('a multirun sweep runs on one GPU; sweeps across ranks are not supported')
+  groups = group_jobs(jobs)
+  cfg0 = load_config(jobs[0].overrides)
+  base = os.path.join(cfg0.get('output_dir', './outputs'), f'{cfg0.algorithm}_{cfg0.env}_sweeper', time.strftime('%m-%d_%H-%M-%S'))
+  print(f'sweep: {len(jobs)} job(s) in {len(groups)} group(s)', flush=True)
+  scores: Dict[int, float] = {}
+  try:
+    for g in groups:
+      cfg = load_config(g.overrides)
+      R, J = int(cfg.get('replicas', 1)), len(g.jobs)
+      cfg.replicas = J * R
+      per_replica = {k: [v for v in vals for _ in range(R)] for k, vals in g.per_job.items()}
+      blocks = []
+      for i, j in enumerate(g.jobs):
+        d = os.path.join(base, str(j.num))
+        os.makedirs(d, exist_ok=True)
+        with open(os.path.join(d, 'overrides.yaml'), 'w') as f: yaml.safe_dump(j.overrides, f)
+        blocks.append((d + os.sep, f'job {j.num}: ', i * R, (i + 1) * R))
+      print(f'group of jobs {[j.num for j in g.jobs]}: {J} x {R} replica(s), per-replica {sorted(per_replica) or "none"}', flush=True)
+      for j, s in zip(g.jobs, _train(cfg, blocks, per_replica)): scores[j.num] = s
+  finally:
+    distributed.shutdown()
+  for j in jobs: print(f'job {j.num}: {" ".join(j.overrides)}: score {scores[j.num]:.4f}', flush=True)
+  return [scores[j.num] for j in jobs]
+
+
+def main(argv: Optional[List[str]] = None):
+  """`python train.py algorithm=<ALG> env=<ENV> [key=value ...]` (train.py:21-23, 246): returns the score. With `-m` / `--multirun` and
+  comma-separated values (`reinforcement.discount=0.97,0.98,0.99`): Hydra's basic sweep, run by run_sweep; returns the per-job scores."""
+  multirun, jobs = expand_sweep(sys.argv[1:] if argv is None else argv)
+  if multirun: return run_sweep(jobs)
+  cfg = load_config(jobs[0].overrides)
   out_dir = os.path.join(cfg.get('output_dir', './outputs'), f'{cfg.algorithm}_{cfg.env}', time.strftime('%m-%d_%H-%M-%S'))  # conf/train_config.yaml:54-60
   os.makedirs(out_dir, exist_ok=True)
   try:

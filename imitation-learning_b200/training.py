@@ -1,5 +1,9 @@
 """Host-side mirror of the reference's training.py (same function names and argument order); each call is one
-C-ABI entry point that runs the whole update for all replicas on the current CUDA stream."""
+C-ABI entry point that runs the whole update for all replicas on the current CUDA stream.
+
+The scalar hyper-parameters that leave every shape unchanged (discount, entropy_target, polyak_factor, grad_penalty,
+entropy_bonus) are a float (every replica) or an [R] tensor (one value per replica, for hyper-parameter sweeps). Keep such a
+tensor on the device and alive for as long as a CUDA graph that captured the call is replayed."""
 from __future__ import annotations
 
 import ctypes as C
@@ -27,6 +31,14 @@ def _workspace(owner, key: str, nbytes: int, device) -> Tensor:
   return ws
 
 
+def _per_replica(x, R: int, device) -> Tuple[float, Optional[Tensor]]:
+  """(scalar, None) for a float; (0.0, [R] float32 device tensor) for per-replica values."""
+  if isinstance(x, (int, float)): return float(x), None
+  t = torch.as_tensor(x, dtype=torch.float32).to(device).reshape(-1).contiguous()
+  assert t.numel() == R, f'per-replica hyper-parameter has {t.numel()} values for {R} replicas'
+  return 0.0, t
+
+
 def _as_batch(t: Union[TransitionBatch, Dict[str, Tensor]], device) -> Tuple[TransitionBatch, Optional[Tensor]]:
   if isinstance(t, TransitionBatch): return t, None
   tb = TransitionBatch.from_dict(t, device=device)
@@ -36,7 +48,7 @@ def _as_batch(t: Union[TransitionBatch, Dict[str, Tensor]], device) -> Tuple[Tra
 
 
 def sac_update(actor: SoftActor, critic: TwinCritic, log_alpha: Tensor, target_critic: TwinCritic, transitions, actor_optimiser: Adam, critic_optimiser: Adam,
-               temperature_optimiser: Adam, discount: float, entropy_target: float, polyak_factor: float, eps_next: Optional[Tensor] = None, eps_new: Optional[Tensor] = None,
+               temperature_optimiser: Adam, discount, entropy_target, polyak_factor, eps_next: Optional[Tensor] = None, eps_new: Optional[Tensor] = None,
                out: Optional[Dict[str, Tensor]] = None) -> Tuple[Tensor, Tensor]:
   """training.py:14-54. `eps_next` / `eps_new` inject the two policy noise draws (:21, :35); when omitted they are
   drawn on the device. Returns (new_log_probs, min(values_1, values_2)) like the reference (:54)."""
@@ -57,7 +69,9 @@ def sac_update(actor: SoftActor, critic: TwinCritic, log_alpha: Tensor, target_c
   a.log_alpha, a.batch = log_alpha.data_ptr(), batch.c_struct()
   a.absorbing, a.absorbing_from_state, a.R = _lib.ptr(absorbing), int(batch.absorbing and absorbing is None), R
   a.eps_next, a.eps_new = eps_next.data_ptr(), eps_new.data_ptr()
-  a.discount, a.entropy_target, a.polyak_factor = discount, entropy_target, polyak_factor
+  (a.discount, discount_r), (a.entropy_target, entropy_target_r), (a.polyak_factor, polyak_r) = (_per_replica(x, R, device) for x in (discount, entropy_target, polyak_factor))
+  a.discount_r, a.entropy_target_r, a.polyak_r = _lib.ptr(discount_r), _lib.ptr(entropy_target_r), _lib.ptr(polyak_r)
+  if polyak_r is not None: a.critic_opt.replica_floats = critic.mlp.flat.numel() // R  # the target shares the twin critic's layout
   a.out_log_probs, a.out_q_values, a.out_losses = out['log_probs'].data_ptr(), out['q_values'].data_ptr(), out['losses'].data_ptr()
   need = _lib.lib().il_sac_workspace_bytes(C.byref(a))
   ws = _workspace(actor, 'sac', need, device)
@@ -74,26 +88,29 @@ def adversarial_imitation_update(actor: SoftActor, discriminator: GAILDiscrimina
   pol, _ = _as_batch(transitions, device)
   exp, _ = _as_batch(expert_transitions, device)
   B = pol.B
-  loss_function, grad_penalty = imitation_cfg.loss_function, float(imitation_cfg.grad_penalty)
-  if grad_penalty > 0 and eps_gp is None: eps_gp = default_rng.uniform((R, B), device, stream_id=21)
+  loss_function = imitation_cfg.loss_function
+  (grad_penalty, grad_penalty_r), (entropy_bonus, entropy_bonus_r) = _per_replica(imitation_cfg.grad_penalty, R, device), _per_replica(imitation_cfg.entropy_bonus, R, device)
+  # per-replica grad_penalty: the gradient-penalty pass runs (replicas at 0 skip their contribution inside it)
+  if (grad_penalty > 0 or grad_penalty_r is not None) and eps_gp is None: eps_gp = default_rng.uniform((R, B), device, stream_id=21)
   if loss_function == 'Mixup' and eps_mix is None:
     alpha = float(imitation_cfg.mixup_alpha)  # training.py:106
     if alpha == 1.0: eps_mix = default_rng.uniform((R, B), device, stream_id=22)  # Beta(1, 1) = U(0, 1): every published config uses mixup_alpha 1
     else: eps_mix = torch.distributions.Beta(torch.full((R, B), alpha, device=device), torch.full((R, B), alpha, device=device)).sample()
   as_dev = lambda t: None if t is None else torch.as_tensor(t, dtype=torch.float32).to(device).reshape(R, B).contiguous()
   eps_gp, eps_mix = as_dev(eps_gp), as_dev(eps_mix)
+  hyper = (grad_penalty, grad_penalty_r, entropy_bonus, entropy_bonus_r)
   if discriminator.general:
-    return _general_adversarial_update(actor, discriminator, pol, exp, discriminator_optimiser, imitation_cfg, eps_gp, eps_mix, out_losses)
+    return _general_adversarial_update(actor, discriminator, pol, exp, discriminator_optimiser, imitation_cfg, hyper, eps_gp, eps_mix, out_losses)
   a = _lib.GailUpdateArgs()
   a.disc, a.opt, a.policy, a.expert = discriminator.c_struct(), discriminator_optimiser.c_struct(), pol.c_struct(), exp.c_struct()
   a.eps_gp, a.eps_mix, a.R, a.loss_function, a.training = _lib.ptr(eps_gp), _lib.ptr(eps_mix), R, _lib.LOSS[loss_function], int(discriminator.training)
-  a.grad_penalty, a.entropy_bonus = grad_penalty, float(imitation_cfg.entropy_bonus)
+  a.grad_penalty, a.grad_penalty_r, a.entropy_bonus, a.entropy_bonus_r = grad_penalty, _lib.ptr(grad_penalty_r), entropy_bonus, _lib.ptr(entropy_bonus_r)
   a.pos_class_prior, a.nonnegative_margin = float(imitation_cfg.pos_class_prior), float(imitation_cfg.nonnegative_margin)
   a.out_losses = _lib.ptr(out_losses)
   _lib.check(_lib.lib().il_gail_update(_lib.handle(), C.byref(a), _lib.stream()))
 
 
-def _general_adversarial_update(actor, disc: GAILDiscriminator, pol: TransitionBatch, exp: TransitionBatch, opt: Adam, imitation_cfg, eps_gp, eps_mix, out_losses):
+def _general_adversarial_update(actor, disc: GAILDiscriminator, pol: TransitionBatch, exp: TransitionBatch, opt: Adam, imitation_cfg, hyper, eps_gp, eps_mix, out_losses):
   """training.py:85-134 for the non-default discriminator configurations (reward shaping, subtract_log_policy, depth > 1, tanh / sigmoid):
   the log-policy inputs of make_gail_input (models.py:148, evaluated under no_grad) are computed first, then one il_gailx_update call."""
   R, B, device, lib = disc.replicas, pol.B, disc.device, _lib.lib()
@@ -113,7 +130,8 @@ def _general_adversarial_update(actor, disc: GAILDiscriminator, pol: TransitionB
   a.eps_gp, a.eps_mix = _lib.ptr(eps_gp), _lib.ptr(eps_mix)
   a.logp_policy, a.logp_expert, a.logp_mix = _lib.ptr(logp.get('policy')), _lib.ptr(logp.get('expert')), _lib.ptr(logp.get('mix'))
   a.R, a.loss_function, a.training = R, _lib.LOSS[loss_function], int(disc.training)
-  a.grad_penalty, a.entropy_bonus = float(imitation_cfg.grad_penalty), float(imitation_cfg.entropy_bonus)
+  grad_penalty, grad_penalty_r, entropy_bonus, entropy_bonus_r = hyper
+  a.grad_penalty, a.grad_penalty_r, a.entropy_bonus, a.entropy_bonus_r = grad_penalty, _lib.ptr(grad_penalty_r), entropy_bonus, _lib.ptr(entropy_bonus_r)
   a.pos_class_prior, a.nonnegative_margin = float(imitation_cfg.pos_class_prior), float(imitation_cfg.nonnegative_margin)
   a.out_losses = _lib.ptr(out_losses)
   need = lib.il_gailx_workspace_bytes(C.byref(a))

@@ -52,6 +52,12 @@ typedef struct il_adam {
   float*   v;                       /* exp_avg_sq */
   int64_t* step;                    /* device scalar, incremented by every update */
   double lr, beta1, beta2, eps, weight_decay;  /* Python floats in the reference; kept in double like torch does */
+  /* Per-replica hyper-parameters (hyper-parameter sweeps): [R] device arrays, NULL = the scalar above for every replica (bit for
+   * bit the scalar path). replica_floats = floats of the flat buffer owned by one replica (actor stride, 2 x stride for a twin
+   * critic, 1 for log_alpha, the discriminator stride); required (a multiple of 4 for the streaming kernels) when an array is set. */
+  const double* lr_r;
+  const double* weight_decay_r;
+  int64_t replica_floats;
 } il_adam;
 
 /* Packed transitions [R, B, row]: row = [state S | action A | reward | next_state S | terminal | timeout |
@@ -150,6 +156,9 @@ typedef struct il_sac_args {
   float* out_losses;                /* [R, 3] value, policy, temperature loss (may be NULL) */
   void*   workspace;
   int64_t workspace_bytes;
+  const float* discount_r;          /* [R] per-replica discount / entropy_target / polyak_factor; NULL = the scalar */
+  const float* entropy_target_r;
+  const float* polyak_r;
 } il_sac_args;
 int64_t il_sac_workspace_bytes(const il_sac_args* a);
 int il_sac_update(il_handle* h, const il_sac_args* a, void* stream);
@@ -213,6 +222,8 @@ int il_red_reward(il_handle* h, const il_red* disc, int R, const il_batch* batch
 int il_adam_step(il_handle* h, float* params, const float* grads, const il_adam* opt, int64_t n, void* stream);
 /* The same step with update_target_network fused (training.py:33 + models.py:78-81): target = polyak * target + (1 - polyak) * params_new. */
 int il_adam_step_polyak(il_handle* h, float* params, const float* grads, const il_adam* opt, int64_t n, float* target, float polyak_factor, void* stream);
+/* The same with a per-replica polyak factor polyak_r [n / opt->replica_floats] (the replica mapping of opt). */
+int il_adam_step_polyak_r(il_handle* h, float* params, const float* grads, const il_adam* opt, int64_t n, float* target, const float* polyak_r, void* stream);
 
 /* ---- ReplayMemory (memory.py:12-68) --------------------------------------------------------------------- */
 /* append (memory.py:40-44) of one transition per replica, with the train.py:157-162 flags: `terminal`
@@ -264,6 +275,10 @@ typedef struct il_gail_update_args {
   float* out_losses;                /* [R, 2] bce/mixup loss, gp loss (may be NULL) */
   void*   workspace;                /* il_gail_workspace_bytes */
   int64_t workspace_bytes;
+  /* [R] per-replica grad_penalty / entropy_bonus; NULL = the scalar. With grad_penalty_r the gradient-penalty pass is enabled by
+   * passing eps_gp (the caller passes it when any replica's value is > 0); a replica whose value is 0 skips it as in a uniform run. */
+  const float* grad_penalty_r;
+  const float* entropy_bonus_r;
 } il_gail_update_args;
 int64_t il_gail_workspace_bytes(const il_gail_update_args* a);
 /* adversarial_imitation_update (training.py:85-134) incl. the train()/eval() power-iteration semantics. */
@@ -286,6 +301,7 @@ typedef struct il_gailx {
   int32_t reward_function;          /* IL_REWARD_* */
   int32_t subtract_log_policy;      /* models.py:175 */
   float   discount;                 /* models.py:174 */
+  const float* discount_r;          /* [R] per-replica shaping discount; NULL = discount */
 } il_gailx;
 typedef struct il_gailx_update_args {
   il_gailx disc;
@@ -302,6 +318,10 @@ typedef struct il_gailx_update_args {
   float* out_losses;                /* [R, 2] (may be NULL) */
   void*   workspace;                /* il_gailx_workspace_bytes */
   int64_t workspace_bytes;
+  /* as in il_gail_update_args. The gradient-penalty pass of this program is batched over replicas: a replica whose value is 0 gets no
+   * penalty contribution, but its spectral-norm vectors still take the pass's power iteration, so sweeps keep grad_penalty uniform here. */
+  const float* grad_penalty_r;
+  const float* entropy_bonus_r;
 } il_gailx_update_args;
 int64_t il_gailx_workspace_bytes(const il_gailx_update_args* a);
 int il_gailx_update(il_handle* h, const il_gailx_update_args* a, void* stream);      /* training.py:85-134 */
