@@ -53,13 +53,15 @@ class BcArgs(C.Structure):
 
 
 class Gail(C.Structure):
-  _fields_ = [('g', Mlp), ('u', vp), ('v', vp), ('u_stride', C.c_int32), ('v_stride', C.c_int32), ('state_only', C.c_int32), ('reward_function', C.c_int32)]
+  _fields_ = [('g', Mlp), ('u', vp), ('v', vp), ('u_stride', C.c_int32), ('v_stride', C.c_int32), ('state_only', C.c_int32), ('reward_function', C.c_int32),
+              ('reward_function_r', vp), ('spectral_norm_r', vp)]
 
 
 class GailUpdateArgs(C.Structure):
   _fields_ = [('disc', Gail), ('opt', Adam), ('policy', Batch), ('expert', Batch), ('eps_gp', vp), ('eps_mix', vp), ('R', C.c_int32), ('loss_function', C.c_int32),
               ('training', C.c_int32), ('_pad', C.c_int32), ('grad_penalty', C.c_float), ('entropy_bonus', C.c_float), ('pos_class_prior', C.c_float),
-              ('nonnegative_margin', C.c_float), ('out_losses', vp), ('workspace', vp), ('workspace_bytes', C.c_int64), ('grad_penalty_r', vp), ('entropy_bonus_r', vp)]
+              ('nonnegative_margin', C.c_float), ('out_losses', vp), ('workspace', vp), ('workspace_bytes', C.c_int64), ('grad_penalty_r', vp), ('entropy_bonus_r', vp),
+              ('loss_function_r', vp), ('pos_class_prior_r', vp), ('nonnegative_margin_r', vp)]
 
 
 class Gailx(C.Structure):
@@ -121,6 +123,7 @@ SIGNATURES = {
   'il_fill_normal': (C.c_int, [vp, vp, i64, u64, u64, vp, vp]),
   'il_fill_uniform': (C.c_int, [vp, vp, i64, u64, u64, vp, vp]),
   'il_counter_add': (C.c_int, [vp, vp, u64, vp]),
+  'il_fill_beta': (C.c_int, [vp, vp, C.c_int, i64, vp, u64, u64, vp, vp]),
   'il_actor_workspace_bytes': (i64, [P(Mlp), C.c_int, C.c_int]),
   'il_actor_forward': (C.c_int, [vp, P(Mlp), C.c_int, C.c_int, vp, i64, C.c_int, vp, vp, vp, vp, vp, vp, vp, i64, vp]),
   'il_critic_workspace_bytes': (i64, [P(Mlp), C.c_int, C.c_int]),

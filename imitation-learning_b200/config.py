@@ -90,6 +90,14 @@ MULTIRUN_FLAGS = ('-m', '--multirun')
 VECTORISED = ('training.learning_rate', 'training.weight_decay', 'reinforcement.discount', 'reinforcement.target_temperature', 'reinforcement.polyak_factor',
               'imitation.learning_rate', 'imitation.weight_decay', 'imitation.grad_penalty', 'imitation.entropy_bonus', 'bc_pretraining.learning_rate',
               'bc_pretraining.weight_decay')
+# The GAIL discriminator's choices that leave every shape unchanged: per-replica values of the fused discriminator (csrc/gail.cu: one CTA per
+# replica branches on them). The general discriminator (csrc/gail_general.cu) takes only the Mixup alpha per replica.
+PER_REPLICA_DISCRIMINATOR = ('imitation.loss_function', 'imitation.discriminator.reward_function', 'imitation.spectral_norm', 'imitation.mixup_alpha',
+                             'imitation.pos_class_prior', 'imitation.nonnegative_margin')
+# Keys an algorithm never reads: jobs that differ only in them are the same run (GAILDiscriminator never passes its dropout to _create_fcnn,
+# models.py:157-162), so they neither split groups nor become per-replica values.
+UNUSED_KEYS = {'GAIL': ('imitation.discriminator.input_dropout', 'imitation.discriminator.dropout')}
+_CHOICES = {'imitation.loss_function': ('BCE', 'Mixup', 'PUGAIL'), 'imitation.discriminator.reward_function': ('AIRL', 'FAIRL', 'GAIL')}
 _SWEEP_FUNCTIONS = re.compile(r'^(range|choice|interval|glob|sort|shuffle|tag)\s*\(')
 
 
@@ -165,11 +173,15 @@ def expand_sweep(argv: Sequence[str]) -> Tuple[bool, List[SweepJob]]:
 
 
 def vectorised_keys(cfg: Config) -> Tuple[str, ...]:
-  """VECTORISED minus the keys a path of this configuration cannot take per replica: the general GAIL discriminator (csrc/gail_general.cu)
-  batches its gradient-penalty pass over replicas, so a replica with grad_penalty 0 would still take that pass's power iteration."""
+  """VECTORISED minus the keys a path of this configuration cannot take per replica, plus the discriminator choices for GAIL: the general GAIL
+  discriminator (csrc/gail_general.cu) batches its gradient-penalty pass over replicas, so a replica with grad_penalty 0 would still take that
+  pass's power iteration, and it takes only mixup_alpha of PER_REPLICA_DISCRIMINATOR."""
   d = cfg.imitation.get('discriminator') or {}
-  general = cfg.get('algorithm') == 'GAIL' and bool(d.get('reward_shaping') or d.get('subtract_log_policy') or d.get('depth', 1) != 1 or d.get('activation', 'relu') != 'relu')
-  return tuple(k for k in VECTORISED if not (general and k == 'imitation.grad_penalty'))
+  gail = cfg.get('algorithm') == 'GAIL'
+  general = gail and bool(d.get('reward_shaping') or d.get('subtract_log_policy') or d.get('depth', 1) != 1 or d.get('activation', 'relu') != 'relu')
+  keys = tuple(k for k in VECTORISED if not (general and k == 'imitation.grad_penalty'))
+  if gail: keys += ('imitation.mixup_alpha', ) if general else PER_REPLICA_DISCRIMINATOR
+  return keys
 
 
 def group_jobs(jobs: List[SweepJob], conf_dir: str = CONF_DIR) -> List[SweepGroup]:
@@ -184,7 +196,8 @@ def group_jobs(jobs: List[SweepJob], conf_dir: str = CONF_DIR) -> List[SweepGrou
   groups: Dict[Tuple, SweepGroup] = {}
   for j in jobs:
     ov = dict(o.partition('=')[::2] for o in j.overrides)
-    vec = set(vectorised_keys(load_config(j.overrides, conf_dir)))
+    cfg = load_config(j.overrides, conf_dir)
+    vec = set(vectorised_keys(cfg)) | set(UNUSED_KEYS.get(cfg.get('algorithm'), ()))
     key = tuple((k, ov.get(k)) for k in swept if k not in vec)
     g = groups.setdefault(key, SweepGroup([]))
     g.jobs.append(j)
@@ -209,16 +222,41 @@ def set_key(cfg: Dict[str, Any], dotted: str, value: Any):
   node[parts[-1]] = value
 
 
-def split_per_replica(cfg: Config, per_replica: Optional[Dict[str, Sequence[float]]], R: int) -> Tuple[Config, Dict[str, List[float]]]:
+def _per_replica_value(k: str, x: Any) -> Any:
+  """A per-replica value as the config holds it: a name of _CHOICES[k], a bool for spectral_norm, a float otherwise."""
+  if k in _CHOICES:
+    if x not in _CHOICES[k]: raise SweepError(f'{k}={x!r}: not one of {", ".join(_CHOICES[k])}')  # train.py:42,44
+    return x
+  if k == 'imitation.spectral_norm':
+    if not isinstance(x, bool): raise SweepError(f'{k}={x!r}: not true / false')
+    return x
+  if isinstance(x, (bool, str)): raise SweepError(f'{k}={x!r}: not a number')
+  return float(x)
+
+
+def _check_gail_replicas(cfg: Config, arrays: Dict[str, List[Any]], R: int):
+  """The reference's GAIL asserts (train.py:42-47) for every replica: alpha > 0 for Mixup replicas, 0 <= prior <= 1 and margin >= 0 for PUGAIL ones."""
+  val = lambda k, r: arrays[k][r] if k in arrays else get_key(cfg, k)
+  for r in range(R):
+    loss = val('imitation.loss_function', r)
+    if loss == 'Mixup' and not val('imitation.mixup_alpha', r) > 0: raise SweepError(f'replica {r}: Mixup needs imitation.mixup_alpha > 0')
+    if loss == 'PUGAIL':
+      if not 0 <= val('imitation.pos_class_prior', r) <= 1: raise SweepError(f'replica {r}: PUGAIL needs 0 <= imitation.pos_class_prior <= 1')
+      if not val('imitation.nonnegative_margin', r) >= 0: raise SweepError(f'replica {r}: PUGAIL needs imitation.nonnegative_margin >= 0')
+
+
+def split_per_replica(cfg: Config, per_replica: Optional[Dict[str, Sequence[Any]]], R: int) -> Tuple[Config, Dict[str, List[Any]]]:
   """(config, arrays) for Trainer(per_replica=...): a key whose R values are all equal becomes that scalar in a copy of the config (the
-  uniform path, bit for bit); the others stay per-replica lists. Keys outside vectorised_keys(cfg) are refused."""
+  uniform path, bit for bit); the others stay per-replica lists. Keys outside vectorised_keys(cfg) and values the reference's asserts refuse
+  (train.py:42-49, per replica for GAIL) are refused."""
   cfg = copy.deepcopy(cfg)
   arrays = {}
   allowed = vectorised_keys(cfg)
   for k, vals in (per_replica or {}).items():
     if k not in allowed: raise SweepError(f'{k} cannot take per-replica values in this configuration (per-replica keys: {", ".join(allowed)})')
-    vals = [float(x) for x in vals]
+    vals = [_per_replica_value(k, x) for x in vals]
     if len(vals) != R: raise SweepError(f'{k}: {len(vals)} values for {R} replicas')
     if all(x == vals[0] for x in vals): set_key(cfg, k, vals[0])
     else: arrays[k] = vals
+  if cfg.get('algorithm') == 'GAIL': _check_gail_replicas(cfg, arrays, R)
   return cfg, arrays

@@ -157,6 +157,57 @@ __global__ void fill_kernel(float* __restrict__ out, int64_t n, uint64_t seed, u
   }
 }
 
+// ---- Beta(alpha, alpha) draws (training.py:106) ------------------------------------------------------------------------------------
+constexpr int BETA_ATTEMPTS = 16;  // per gamma draw; Marsaglia-Tsang accepts > 95 % of proposals for shape >= 1
+
+// log of a Gamma(a) draw, a >= 1 (Marsaglia & Tsang 2000). Attempt k reads Philox at the element's own counter c under the stream id with
+// `tag | k` xor-ed into its high word, so the draws never advance the counter. *boost_u receives a (0, 1] uniform of attempt 0 that the
+// acceptance test does not use (the U of the alpha < 1 boost). Returns log(d) (the draw at normal 0) when every attempt is rejected.
+__device__ float log_gamma_mt(float a, uint64_t c, uint64_t stream_id, uint32_t tag, uint2 key, float* boost_u) {
+  const float d = a - 1.f / 3.f, cc = 1.f / sqrtf(9.f * d);
+  for (int k = 0; k < BETA_ATTEMPTS; ++k) {
+    const uint4 q = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), (uint32_t)stream_id, (uint32_t)(stream_id >> 32) ^ (tag | (uint32_t)k)), key);
+    if (k == 0) *boost_u = 1.f - u32_to_unit(q.w);
+    const float x = sqrtf(-2.f * logf(1.f - u32_to_unit(q.x))) * cospif(2.f * u32_to_unit(q.y));
+    const float t = fmaf(cc, x, 1.f);
+    if (t <= 0.f) continue;
+    const float lt = logf(t), v = t * t * t;
+    if (logf(1.f - u32_to_unit(q.z)) < 0.5f * x * x + d - d * v + 3.f * d * lt) return logf(d) + 3.f * lt;
+  }
+  return logf(d);
+}
+
+// One thread per element; element i of replica r = i / n uses counter (base + i / 4), lane i % 4 (the il_fill_uniform mapping).
+__global__ void beta_fill_kernel(float* __restrict__ out, int64_t total, int64_t n, const float* __restrict__ alpha_r, uint64_t seed, uint64_t stream_id,
+                                 const uint64_t* __restrict__ counter) {
+  const uint64_t base = counter ? *counter : 0ull;
+  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const uint64_t c = base + (uint64_t)(i >> 2);
+    const uint32_t lane = (uint32_t)(i & 3);
+    const float alpha = alpha_r[i / n];
+    float v;
+    if (alpha == 1.f) {  // Beta(1, 1) = U(0, 1): the il_fill_uniform value
+      const uint4 q = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), (uint32_t)stream_id, (uint32_t)(stream_id >> 32)), key);
+      v = u32_to_unit(lane == 0 ? q.x : lane == 1 ? q.y : lane == 2 ? q.z : q.w);
+    } else if (!(alpha > 0.f)) {
+      v = __int_as_float(0x7fc00000);  // Beta(alpha, alpha) needs alpha > 0
+    } else {
+      // X, Y ~ Gamma(alpha): shape alpha + 1 and the U^(1 / alpha) boost below 1; X / (X + Y) = 1 / (1 + exp(log Y - log X)) is 0 or 1
+      // where the logs are far apart, never NaN. Above 1/2 it is formed as 1 - (the smaller share): 1 + a tiny exp rounds on the coarser
+      // grid above 1, which would leave float values just below 1 unreachable.
+      const float a = alpha < 1.f ? alpha + 1.f : alpha;
+      float ux, uy;
+      float lx = log_gamma_mt(a, c, stream_id, 0x80000000u | (lane << 5), key, &ux);
+      float ly = log_gamma_mt(a, c, stream_id, 0x80000000u | (lane << 5) | 16u, key, &uy);
+      if (alpha < 1.f) { lx += logf(ux) / alpha; ly += logf(uy) / alpha; }
+      const float t = ly - lx;
+      v = t >= 0.f ? 1.f / (1.f + expf(t)) : 1.f - 1.f / (1.f + expf(-t));
+    }
+    out[i] = v;
+  }
+}
+
 __global__ void counter_add_kernel(uint64_t* c, uint64_t inc) { *c += inc; }
 
 int fill(il_handle* h, float* out, int64_t n, uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream, int normal) {
@@ -176,6 +227,16 @@ extern "C" int il_fill_normal(il_handle* h, float* out, int64_t n, uint64_t seed
 }
 extern "C" int il_fill_uniform(il_handle* h, float* out, int64_t n, uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream) {
   return fill(h, out, n, seed, stream_id, counter, stream, 0);
+}
+extern "C" int il_fill_beta(il_handle* h, float* out, int R, int64_t n_per_replica, const float* alpha_r, uint64_t seed, uint64_t stream_id, const uint64_t* counter,
+                            void* stream) {
+  IL_CHECK(h && out && alpha_r && R > 0 && n_per_replica >= 0, "il_fill_beta: bad argument");
+  const int64_t total = (int64_t)R * n_per_replica;
+  if (total == 0) return 0;
+  int64_t blocks = (total + 255) / 256;
+  if (blocks > (int64_t)h->sm_count * 16) blocks = (int64_t)h->sm_count * 16;
+  IL_LAUNCH(h, beta_fill_kernel, (unsigned)blocks, 256, 0, (cudaStream_t)stream, out, total, n_per_replica, alpha_r, seed, stream_id, counter);
+  return 0;
 }
 extern "C" int il_counter_add(il_handle* h, uint64_t* counter, uint64_t inc, void* stream) {
   IL_CHECK(h && counter, "il_counter_add: null argument");

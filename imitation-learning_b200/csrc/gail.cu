@@ -153,7 +153,7 @@ __device__ void forward_chunk(const GailDims& g, const GailSmem& s, int nb, floa
 }
 
 template <int NE>
-__global__ void __launch_bounds__(THREADS) gail_update_kernel(const GailUpdParams p) {
+__global__ void __launch_bounds__(THREADS, 2) gail_update_kernel(const GailUpdParams p) {
   extern __shared__ __align__(16) float sm[];
   const GailDims g = p.g;
   GailSmem s;
@@ -162,7 +162,7 @@ __global__ void __launch_bounds__(THREADS) gail_update_kernel(const GailUpdParam
   const int r = blockIdx.x, tid = threadIdx.x;
   const int H = g.H, d = g.d, B = g.B;
   float* prm = a.disc.g.params + (int64_t)r * a.disc.g.stride;
-  const bool sn = a.disc.u != nullptr;
+  const bool sn_r = a.disc.u != nullptr && (!a.disc.spectral_norm_r || a.disc.spectral_norm_r[r] != 0);  // a replica at 0 never touches its u / v slots
   const float* pol = a.policy.rows + (int64_t)r * a.policy.replica_stride;
   const float* exp_ = a.expert.rows + (int64_t)r * a.expert.replica_stride;
   const float* eps_gp = a.eps_gp ? a.eps_gp + (int64_t)r * B : nullptr;
@@ -176,18 +176,28 @@ __global__ void __launch_bounds__(THREADS) gail_update_kernel(const GailUpdParam
   for (int i = tid; i < H * d; i += THREADS) { s.W1[i] = prm[p.off_w1 + i]; s.G1[i] = 0.f; }
   for (int h = tid; h < H; h += THREADS) {
     s.b1[h] = prm[p.off_b1 + h]; s.w2[h] = prm[p.off_w2 + h]; s.G2[h] = 0.f; s.gb1[h] = 0.f;
-    if (sn) { s.u1[h] = a.disc.u[(int64_t)r * a.disc.u_stride + h]; s.v2[h] = a.disc.v[(int64_t)r * a.disc.v_stride + d + h]; }
+    if (sn_r) { s.u1[h] = a.disc.u[(int64_t)r * a.disc.u_stride + h]; s.v2[h] = a.disc.v[(int64_t)r * a.disc.v_stride + d + h]; }
   }
-  if (sn) for (int j = tid; j < d; j += THREADS) s.v1[j] = a.disc.v[(int64_t)r * a.disc.v_stride + j];
+  if (sn_r) for (int j = tid; j < d; j += THREADS) s.v1[j] = a.disc.v[(int64_t)r * a.disc.v_stride + j];
   const float b2 = prm[p.off_b2];
-  float u2 = sn ? a.disc.u[(int64_t)r * a.disc.u_stride + H] : 1.f;
+  float u2 = sn_r ? a.disc.u[(int64_t)r * a.disc.u_stride + H] : 1.f;
+  // the per-replica choices (sweeps) live in shared memory and are re-read where used: the register budget of the tiled variants has no room
+  // for them (scal[0:2] is the AdamW scratch at the end)
+  if (tid == 0) {
+    s.scal[2] = __int_as_float(a.loss_function_r ? a.loss_function_r[r] : a.loss_function);
+    s.scal[3] = a.pos_class_prior_r ? a.pos_class_prior_r[r] : a.pos_class_prior;
+    s.scal[4] = a.nonnegative_margin_r ? a.nonnegative_margin_r[r] : a.nonnegative_margin;
+    s.scal[5] = sn_r ? 1.f : 0.f;
+  }
   __syncthreads();
+  auto loss_function = [&] { return __float_as_int(s.scal[2]); };
+  auto sn = [&] { return s.scal[5] != 0.f; };
 
   // ---- pass schedule (training.py:94-127): [policy, expert] or [mixup], then the gradient-penalty mix -----
   int kinds[3], n_pass = 0;
   const float* pass_eps[3] = {nullptr, nullptr, nullptr};
   int gp_pass = -1;
-  if (a.loss_function == IL_LOSS_MIXUP) { kinds[n_pass] = PASS_MIX; pass_eps[n_pass++] = eps_mix; }
+  if (loss_function() == IL_LOSS_MIXUP) { kinds[n_pass] = PASS_MIX; pass_eps[n_pass++] = eps_mix; }
   else { kinds[n_pass++] = PASS_POLICY; kinds[n_pass++] = PASS_EXPERT; }
   if (grad_penalty > 0.f) { gp_pass = n_pass; kinds[n_pass] = PASS_MIX; pass_eps[n_pass++] = eps_gp; }
 
@@ -196,7 +206,7 @@ __global__ void __launch_bounds__(THREADS) gail_update_kernel(const GailUpdParam
   for (int k = 0; k < n_pass; ++k) {
     float* slot = s.slots + k * SF;
     float sig1 = 1.f, sig2 = 1.f;
-    if (sn) {
+    if (sn()) {
       sig1 = spectral_sigma(s.W1, s.u1, s.v1, s.tvec, s.red, H, d, a.training != 0);
       // layer 2 is a [1, H] matrix: u2 scalar, v2 [H]
       float t = 0.f;
@@ -223,7 +233,7 @@ __global__ void __launch_bounds__(THREADS) gail_update_kernel(const GailUpdParam
   // ---- phase 2 (PUGAIL only): the clamp of training.py:102 needs the batch scalar before any gradient ------
   float pu_gate = 1.f;
   float loss_bce = 0.f, loss_gp = 0.f;
-  if (a.loss_function == IL_LOSS_PUGAIL) {
+  if (loss_function() == IL_LOSS_PUGAIL) {
     float sums[2] = {0.f, 0.f};  // sum w_p softplus(f_p), sum w_e softplus(f_e)
     for (int k = 0; k < 2; ++k) {
       const float* slot = s.slots + k * SF;
@@ -242,8 +252,8 @@ __global__ void __launch_bounds__(THREADS) gail_update_kernel(const GailUpdParam
       }
       sums[k] = bsum(part, s.red);
     }
-    const float inner = a.pos_class_prior * (sums[1] * invB) - sums[0] * invB;
-    pu_gate = inner >= -a.nonnegative_margin ? 1.f : 0.f;  // torch.clamp(min=) passes gradient where x >= min
+    const float inner = s.scal[3] * (sums[1] * invB) - sums[0] * invB;
+    pu_gate = inner >= -s.scal[4] ? 1.f : 0.f;  // torch.clamp(min=) passes gradient where x >= min
   }
 
   // ---- phase 3: forward + backward per pass, projected through that pass's spectral norm --------------------
@@ -270,15 +280,15 @@ __global__ void __launch_bounds__(THREADS) gail_update_kernel(const GailUpdParam
         for (int b = tid; b < nb; b += THREADS) {
           const float f = s.GX[b], w = s.CO[b], sg = sigmoidf(f);
           float df;
-          if (a.loss_function == IL_LOSS_MIXUP) {  // training.py:112
+          if (loss_function() == IL_LOSS_MIXUP) {  // training.py:112
             const float e = s.DF[b];
             df = w * (sg - e) * invB;
             loss_part += e * w * softplusf(-f) + (1.f - e) * w * softplusf(f);
-          } else if (a.loss_function == IL_LOSS_BCE) {  // training.py:98-99
+          } else if (loss_function() == IL_LOSS_BCE) {  // training.py:98-99
             df = kind == PASS_EXPERT ? w * (sg - 1.f) * invB : w * sg * invB;
             loss_part += kind == PASS_EXPERT ? w * softplusf(-f) : w * softplusf(f);
           } else {  // PUGAIL, training.py:101-102
-            const float pr = a.pos_class_prior;
+            const float pr = s.scal[3];
             df = kind == PASS_EXPERT ? pr * w * (sg - 1.f) * invB + pu_gate * pr * w * sg * invB : -pu_gate * w * sg * invB;
             loss_part += kind == PASS_EXPERT ? pr * w * softplusf(-f) + pu_gate * pr * w * softplusf(f) : -pu_gate * w * softplusf(f);
           }
@@ -384,7 +394,7 @@ __global__ void __launch_bounds__(THREADS) gail_update_kernel(const GailUpdParam
     }
     // ---- spectral-norm backward: dL/dW = (G - <G, W_eff> u v^T) / sigma (SURVEY §8a a12), accumulate over passes
     float inner1 = 0.f, inner2 = 0.f;
-    if (sn) {
+    if (sn()) {
 #pragma unroll
       for (int i = 0; i < NE; ++i) {
         const int e = tid + i * THREADS;
@@ -399,11 +409,11 @@ __global__ void __launch_bounds__(THREADS) gail_update_kernel(const GailUpdParam
       const int e = tid + i * THREADS;
       if (e < H * d) {
         const int h = e / d, j = e % d;
-        s.G1[e] += sn ? (g1k[i] - inner1 * slot[h] * slot[H + j]) / sig1 : g1k[i];
+        s.G1[e] += sn() ? (g1k[i] - inner1 * slot[h] * slot[H + j]) / sig1 : g1k[i];
       }
     }
     for (int h = tid; h < H; h += THREADS) {
-      s.G2[h] += sn ? (s.G2k[h] - inner2 * u2k * slot[H + d + h]) / sig2 : s.G2k[h];
+      s.G2[h] += sn() ? (s.G2k[h] - inner2 * u2k * slot[H + d + h]) / sig2 : s.G2k[h];
       s.gb1[h] += s.gb1k[h];
     }
     gb2k = bsum(gb2k, s.red);
@@ -440,7 +450,7 @@ __global__ void __launch_bounds__(THREADS) gail_update_kernel(const GailUpdParam
   for (int i = tid; i < H * d; i += THREADS) adam(p.off_w1 + i, s.G1[i]);
   for (int h = tid; h < H; h += THREADS) { adam(p.off_b1 + h, s.gb1[h]); adam(p.off_w2 + h, s.G2[h]); }
   if (tid == 0) adam(p.off_b2, gb2);
-  if (sn) {  // persist the power-iteration state (in-place buffers of the parametrization)
+  if (sn()) {  // persist the power-iteration state (in-place buffers of the parametrization)
     for (int h = tid; h < H; h += THREADS) { a.disc.u[(int64_t)r * a.disc.u_stride + h] = s.u1[h]; a.disc.v[(int64_t)r * a.disc.v_stride + d + h] = s.v2[h]; }
     for (int j = tid; j < d; j += THREADS) a.disc.v[(int64_t)r * a.disc.v_stride + j] = s.v1[j];
     if (tid == 0) a.disc.u[(int64_t)r * a.disc.u_stride + H] = u2;
@@ -599,7 +609,7 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
   const int r = blockIdx.x, tid = threadIdx.x;
   const int H = g.H, d = g.d, B = g.B, DP = g.DP, LDZ = g.LDZ;
   float* prm = a.disc.g.params + (int64_t)r * a.disc.g.stride;
-  const bool sn = a.disc.u != nullptr;
+  const bool sn_r = a.disc.u != nullptr && (!a.disc.spectral_norm_r || a.disc.spectral_norm_r[r] != 0);  // a replica at 0 never touches its u / v slots
   const float* pol = a.policy.rows + (int64_t)r * a.policy.replica_stride;
   const float* exp_ = a.expert.rows + (int64_t)r * a.expert.replica_stride;
   const float* eps_gp = a.eps_gp ? a.eps_gp + (int64_t)r * B : nullptr;
@@ -612,17 +622,27 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
   for (int i = tid; i < H * d; i += THREADS) { s.W1[i] = prm[p.off_w1 + i]; s.G1[i] = 0.f; }
   for (int h = tid; h < H; h += THREADS) {
     s.b1[h] = prm[p.off_b1 + h]; s.w2[h] = prm[p.off_w2 + h]; s.G2[h] = 0.f; s.gb1[h] = 0.f;
-    if (sn) { s.u1[h] = a.disc.u[(int64_t)r * a.disc.u_stride + h]; s.v2[h] = a.disc.v[(int64_t)r * a.disc.v_stride + d + h]; }
+    if (sn_r) { s.u1[h] = a.disc.u[(int64_t)r * a.disc.u_stride + h]; s.v2[h] = a.disc.v[(int64_t)r * a.disc.v_stride + d + h]; }
   }
-  if (sn) for (int j = tid; j < d; j += THREADS) s.v1[j] = a.disc.v[(int64_t)r * a.disc.v_stride + j];
+  if (sn_r) for (int j = tid; j < d; j += THREADS) s.v1[j] = a.disc.v[(int64_t)r * a.disc.v_stride + j];
   const float b2 = prm[p.off_b2];
-  float u2 = sn ? a.disc.u[(int64_t)r * a.disc.u_stride + H] : 1.f;
+  float u2 = sn_r ? a.disc.u[(int64_t)r * a.disc.u_stride + H] : 1.f;
+  // the per-replica choices (sweeps) live in shared memory and are re-read where used: the register budget of the tiled variants has no room
+  // for them (scal[0:2] is the AdamW scratch at the end)
+  if (tid == 0) {
+    s.scal[2] = __int_as_float(a.loss_function_r ? a.loss_function_r[r] : a.loss_function);
+    s.scal[3] = a.pos_class_prior_r ? a.pos_class_prior_r[r] : a.pos_class_prior;
+    s.scal[4] = a.nonnegative_margin_r ? a.nonnegative_margin_r[r] : a.nonnegative_margin;
+    s.scal[5] = sn_r ? 1.f : 0.f;
+  }
   __syncthreads();
+  auto loss_function = [&] { return __float_as_int(s.scal[2]); };
+  auto sn = [&] { return s.scal[5] != 0.f; };
 
   int kinds[3], n_pass = 0;
   const float* pass_eps[3] = {nullptr, nullptr, nullptr};
   int gp_pass = -1;
-  if (a.loss_function == IL_LOSS_MIXUP) { kinds[n_pass] = PASS_MIX; pass_eps[n_pass++] = eps_mix; }
+  if (loss_function() == IL_LOSS_MIXUP) { kinds[n_pass] = PASS_MIX; pass_eps[n_pass++] = eps_mix; }
   else { kinds[n_pass++] = PASS_POLICY; kinds[n_pass++] = PASS_EXPERT; }
   if (grad_penalty > 0.f) { gp_pass = n_pass; kinds[n_pass] = PASS_MIX; pass_eps[n_pass++] = eps_gp; }
 
@@ -631,7 +651,7 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
   for (int k = 0; k < n_pass; ++k) {
     float* slot = s.slots + k * SF;
     float sig1 = 1.f, sig2 = 1.f;
-    if (sn) {
+    if (sn()) {
       sig1 = spectral_sigma(s.W1, s.u1, s.v1, s.tvec, s.red, H, d, a.training != 0);
       float t = 0.f;
       if (a.training) {
@@ -666,7 +686,7 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
   };
   // ---- phase 2 (PUGAIL): batch scalar of the clamp ---------------------------------------------------------------------------------
   float pu_gate = 1.f, loss_bce = 0.f, loss_gp = 0.f;
-  if (a.loss_function == IL_LOSS_PUGAIL) {
+  if (loss_function() == IL_LOSS_PUGAIL) {
     float sums[2] = {0.f, 0.f};
     for (int k = 0; k < 2; ++k) {
       set_effective(s.slots + k * SF);
@@ -683,7 +703,7 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
       }
       sums[k] = bsum(part, s.red);
     }
-    pu_gate = (a.pos_class_prior * (sums[1] * invB) - sums[0] * invB) >= -a.nonnegative_margin ? 1.f : 0.f;
+    pu_gate = (s.scal[3] * (sums[1] * invB) - sums[0] * invB) >= -s.scal[4] ? 1.f : 0.f;
   }
 
   // ---- phase 3: forward + backward per pass ---------------------------------------------------------------------------------------
@@ -740,15 +760,15 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
           float df = 0.f;
           if (b < nb) {
             const float f = s.F[b], w = s.CO[b], sg = sigmoidf(f);
-            if (a.loss_function == IL_LOSS_MIXUP) {
+            if (loss_function() == IL_LOSS_MIXUP) {
               const float e = s.DF[b];
               df = w * (sg - e) * invB;
               loss_part += e * w * softplusf(-f) + (1.f - e) * w * softplusf(f);
-            } else if (a.loss_function == IL_LOSS_BCE) {
+            } else if (loss_function() == IL_LOSS_BCE) {
               df = kind == PASS_EXPERT ? w * (sg - 1.f) * invB : w * sg * invB;
               loss_part += kind == PASS_EXPERT ? w * softplusf(-f) : w * softplusf(f);
             } else {
-              const float pr = a.pos_class_prior;
+              const float pr = s.scal[3];
               df = kind == PASS_EXPERT ? pr * w * (sg - 1.f) * invB + pu_gate * pr * w * sg * invB : -pu_gate * w * sg * invB;
               loss_part += kind == PASS_EXPERT ? pr * w * softplusf(-f) + pu_gate * pr * w * softplusf(f) : -pu_gate * w * softplusf(f);
             }
@@ -875,7 +895,7 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
     __syncthreads();
     // ---- spectral-norm backward: dL/dW = (G - <G, W_eff> u v^T) / sigma, accumulated over the passes
     float inner1 = 0.f, inner2 = 0.f;
-    if (sn) {
+    if (sn()) {
       for (int e = tid; e < H * d; e += THREADS) inner1 = fmaf(s.G1k[(e / d) * DP + e % d], s.W1e[(e / d) * DP + e % d], inner1);
       inner1 = bsum(inner1, s.red);
       for (int h = tid; h < H; h += THREADS) inner2 = fmaf(s.G2k[h], s.w2e[h], inner2);
@@ -884,10 +904,10 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
     for (int e = tid; e < H * d; e += THREADS) {
       const int h = e / d, j = e % d;
       const float gk = s.G1k[h * DP + j];
-      s.G1[e] += sn ? (gk - inner1 * slot[h] * slot[H + j]) / sig1 : gk;
+      s.G1[e] += sn() ? (gk - inner1 * slot[h] * slot[H + j]) / sig1 : gk;
     }
     for (int h = tid; h < H; h += THREADS) {
-      s.G2[h] += sn ? (s.G2k[h] - inner2 * u2k * slot[H + d + h]) / sig2 : s.G2k[h];
+      s.G2[h] += sn() ? (s.G2k[h] - inner2 * u2k * slot[H + d + h]) / sig2 : s.G2k[h];
       s.gb1[h] += s.gb1k[h];
     }
     gb2k = bsum(gb2k, s.red);
@@ -924,7 +944,7 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
   for (int i = tid; i < H * d; i += THREADS) adam(p.off_w1 + i, s.G1[i]);
   for (int h = tid; h < H; h += THREADS) { adam(p.off_b1 + h, s.gb1[h]); adam(p.off_w2 + h, s.G2[h]); }
   if (tid == 0) adam(p.off_b2, gb2);
-  if (sn) {
+  if (sn()) {
     for (int h = tid; h < H; h += THREADS) { a.disc.u[(int64_t)r * a.disc.u_stride + h] = s.u1[h]; a.disc.v[(int64_t)r * a.disc.v_stride + d + h] = s.v2[h]; }
     for (int j = tid; j < d; j += THREADS) a.disc.v[(int64_t)r * a.disc.v_stride + j] = s.v1[j];
     if (tid == 0) a.disc.u[(int64_t)r * a.disc.u_stride + H] = u2;
@@ -938,7 +958,8 @@ __global__ void __launch_bounds__(THREADS) gail_reward_kernel(const GailRewParam
   gail_carve(g, sm, &s);
   const int r = blockIdx.x, tid = threadIdx.x, H = g.H, d = g.d, B = g.B;
   const float* prm = p.disc.g.params + (int64_t)r * p.disc.g.stride;
-  const bool sn = p.disc.u != nullptr;
+  const bool sn = p.disc.u != nullptr && (!p.disc.spectral_norm_r || p.disc.spectral_norm_r[r] != 0);
+  const int reward_function = p.disc.reward_function_r ? p.disc.reward_function_r[r] : p.disc.reward_function;
   for (int i = tid; i < H * d; i += THREADS) s.W1[i] = prm[p.off_w1 + i];
   for (int h = tid; h < H; h += THREADS) {
     s.b1[h] = prm[p.off_b1 + h]; s.w2[h] = prm[p.off_w2 + h];
@@ -968,8 +989,8 @@ __global__ void __launch_bounds__(THREADS) gail_reward_kernel(const GailRewParam
       if (p.logits) p.logits[(int64_t)r * B + b0 + b] = f;
       if (p.reward) {  // models.py:177-180
         const float D = sigmoidf(f);
-        float hh = p.disc.reward_function == IL_REWARD_GAIL ? -log1pf(-D + 1e-6f) : logf(D + 1e-6f) - log1pf(-D + 1e-6f);
-        if (p.disc.reward_function == IL_REWARD_FAIRL) hh = expf(hh) * -hh;
+        float hh = reward_function == IL_REWARD_GAIL ? -log1pf(-D + 1e-6f) : logf(D + 1e-6f) - log1pf(-D + 1e-6f);
+        if (reward_function == IL_REWARD_FAIRL) hh = expf(hh) * -hh;
         p.reward[(int64_t)r * p.reward_rs + (int64_t)(b0 + b) * p.reward_ld] = hh;
       }
     }
@@ -995,7 +1016,8 @@ __global__ void __launch_bounds__(THREADS, 3) gail_reward_tiled_kernel(const Gai
   float *X = take(g.RB * DP), *Z = take(g.RB * g.LDZ), *F = take(g.RB), *CO = take(g.RB), *DF = take(g.RB), *red = take(32);
   (void)spare;
   const float* prm = p.disc.g.params + (int64_t)r * p.disc.g.stride;
-  const bool sn = p.disc.u != nullptr;
+  const bool sn = p.disc.u != nullptr && (!p.disc.spectral_norm_r || p.disc.spectral_norm_r[r] != 0);
+  const int reward_function = p.disc.reward_function_r ? p.disc.reward_function_r[r] : p.disc.reward_function;
   for (int i = tid; i < H * d; i += THREADS) W1[i] = prm[p.off_w1 + i];
   for (int h = tid; h < H; h += THREADS) {
     b1[h] = prm[p.off_b1 + h]; w2[h] = prm[p.off_w2 + h];
@@ -1029,8 +1051,8 @@ __global__ void __launch_bounds__(THREADS, 3) gail_reward_tiled_kernel(const Gai
       if (p.logits) p.logits[(int64_t)r * B + b0 + b] = f;
       if (p.reward) {  // models.py:177-180
         const float D = sigmoidf(f);
-        float hh = p.disc.reward_function == IL_REWARD_GAIL ? -log1pf(-D + 1e-6f) : logf(D + 1e-6f) - log1pf(-D + 1e-6f);
-        if (p.disc.reward_function == IL_REWARD_FAIRL) hh = expf(hh) * -hh;
+        float hh = reward_function == IL_REWARD_GAIL ? -log1pf(-D + 1e-6f) : logf(D + 1e-6f) - log1pf(-D + 1e-6f);
+        if (reward_function == IL_REWARD_FAIRL) hh = expf(hh) * -hh;
         p.reward[(int64_t)r * p.reward_rs + (int64_t)(b0 + b) * p.reward_ld] = hh;
       }
     }
@@ -1050,6 +1072,7 @@ int gail_setup(const il_gail* disc, const il_batch* batch, GailDims* g, int64_t*
   IL_CHECK(H <= THREADS, "%s: hidden size %d exceeds the kernel limit %d", what, H, THREADS);
   IL_CHECK((disc->u == nullptr) == (disc->v == nullptr), "%s: spectral-norm buffers must both be set or both be null", what);
   if (disc->u) IL_CHECK(disc->u_stride >= H + 1 && disc->v_stride >= d + H, "%s: spectral-norm buffer strides too small", what);
+  IL_CHECK(!disc->spectral_norm_r || disc->u, "%s: spectral_norm_r needs the u / v buffers of every replica", what);
   int RB = 64;
   for (;;) {
     *g = gail_dims(batch->S, batch->A, H, batch->B, disc->state_only, RB);
@@ -1076,7 +1099,8 @@ extern "C" int il_gail_update(il_handle* h, const il_gail_update_args* a, void* 
   IL_CHECK(a->loss_function >= 0 && a->loss_function <= 2, "il_gail_update: bad loss function %d", a->loss_function);
   IL_CHECK(!((a->grad_penalty > 0.f || a->grad_penalty_r) && !a->eps_gp), "il_gail_update: grad_penalty > 0 (or grad_penalty_r) needs eps_gp");
   IL_CHECK(!(a->opt.lr_r || a->opt.weight_decay_r) || a->opt.replica_floats == a->disc.g.stride, "il_gail_update: opt.replica_floats must be the discriminator stride");
-  IL_CHECK(!(a->loss_function == IL_LOSS_MIXUP && !a->eps_mix), "il_gail_update: Mixup needs eps_mix");
+  // with loss_function_r the scalar is unused and the caller passes eps_mix when any replica is Mixup (the host cannot read the array)
+  IL_CHECK(!(!a->loss_function_r && a->loss_function == IL_LOSS_MIXUP && !a->eps_mix), "il_gail_update: Mixup needs eps_mix");
   GailUpdParams p;
   p.a = *a;
   int64_t smem, off[4];

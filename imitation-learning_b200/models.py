@@ -59,6 +59,17 @@ class _RNG:
     _lib.check(_lib.lib().il_counter_add(_lib.handle(), ctr.data_ptr(), (out.numel() + 3) // 4, _lib.stream()))
     return out
 
+  def beta(self, shape, alpha_r: Tensor, device, stream_id: int = 2, out: Optional[Tensor] = None) -> Tensor:
+    """[R, ...] Beta(alpha_r[r], alpha_r[r]) draws (il_fill_beta); alpha_r is an [R] float32 device tensor. Where alpha is 1 the values are
+    those `uniform` draws with the same stream id and counter, and the counter advances as for `uniform`."""
+    out = torch.empty(shape, device=device, dtype=torch.float32) if out is None else out
+    R = alpha_r.numel()
+    assert out.numel() % R == 0 and alpha_r.dtype == torch.float32 and alpha_r.is_cuda
+    ctr = self._ctr(device)
+    _lib.check(_lib.lib().il_fill_beta(_lib.handle(), out.data_ptr(), R, out.numel() // R, alpha_r.data_ptr(), self.seed, stream_id, ctr.data_ptr(), _lib.stream()))
+    _lib.check(_lib.lib().il_counter_add(_lib.handle(), ctr.data_ptr(), (out.numel() + 3) // 4, _lib.stream()))
+    return out
+
 
 default_rng = _RNG(0)
 
@@ -319,24 +330,41 @@ def _spectral_norm_init(weight: Tensor) -> Tuple[Tensor, Tensor]:
   return u, v
 
 
+def _per_replica_choice(x, R: int) -> list:
+  """R values of a choice given as one value or one value per replica."""
+  if isinstance(x, (str, bool, int, float)): return [x] * R
+  x = list(x.tolist() if torch.is_tensor(x) else x)
+  assert len(x) == R, f'{len(x)} per-replica values for {R} replicas'
+  return x
+
+
 class GAILDiscriminator(_Module):
   """:152-180. Accelerated configuration: the depth-1 relu `g` network of conf/algorithm/GAIL.yaml (no reward
   shaping / log-policy subtraction), with or without spectral norm."""
 
-  def __init__(self, state_size: int, action_size: int, imitation_cfg, discount, replicas: int = 1, rng: Optional[ReplicaRNG] = None, device=None):
+  def __init__(self, state_size: int, action_size: int, imitation_cfg, discount, replicas: int = 1, rng: Optional[ReplicaRNG] = None, device=None,
+               reward_function=None, spectral_norm=None):
+    """reward_function / spectral_norm: None = the config's value; otherwise one value, or one value per replica (hyper-parameter sweeps of the
+    fused discriminator: replica r is initialised, trained and rewarded as a single run with its own values)."""
     model_cfg = imitation_cfg.discriminator
     self.state_only = bool(imitation_cfg.state_only)
     # reward-shaping discount (models.py:174): a float, or one value per replica (an [R] float32 device tensor, hyper-parameter sweeps)
     self.discount = discount if isinstance(discount, (int, float)) else \
         torch.as_tensor(discount, dtype=torch.float32).to(torch.device('cuda') if device is None else torch.device(device)).reshape(replicas).contiguous()
-    self.reward_shaping, self.subtract_log_policy, self.reward_function = bool(model_cfg.reward_shaping), bool(model_cfg.subtract_log_policy), model_cfg.reward_function
+    self.reward_shaping, self.subtract_log_policy = bool(model_cfg.reward_shaping), bool(model_cfg.subtract_log_policy)
     self.state_size, self.action_size, self.replicas = state_size, action_size, replicas
-    self.spectral_norm = bool(imitation_cfg.spectral_norm)
+    rf = model_cfg.reward_function if reward_function is None else reward_function
+    sn = imitation_cfg.spectral_norm if spectral_norm is None else spectral_norm
+    rf_list, sn_list = _per_replica_choice(rf, replicas), [bool(x) for x in _per_replica_choice(sn, replicas)]
+    self.reward_function = rf_list[0]
+    self.spectral_norm = any(sn_list)  # u / v are allocated for every replica when any replica uses spectral norm
+    self.spectral_norm_r, self._reward_function_r, self._spectral_norm_r = None, None, None
     # the default configuration (GAIL.yaml:10-17: one relu hidden layer, no shaping, no log-policy term) runs in the fused one-CTA-per-replica
     # kernel (csrc/gail.cu); every other configuration of models.py:157-175 runs as the replica-batched GEMM program of csrc/gail_general.cu
     self.general = self.reward_shaping or self.subtract_log_policy or model_cfg.depth != 1 or model_cfg.activation != 'relu'
     self._ws = None
     if self.general:
+      if len(set(rf_list)) > 1 or len(set(sn_list)) > 1: raise ValueError('per-replica reward_function / spectral_norm need the fused discriminator (depth 1, relu, no shaping or log-policy term)')
       self._init_general(model_cfg, rng, device)
       return
     d, H = (state_size if self.state_only else state_size + action_size), model_cfg.hidden_size
@@ -348,21 +376,38 @@ class GAILDiscriminator(_Module):
     for r in range(replicas):
       with (rng.replica(r) if rng is not None else _null_ctx()):
         params, us, vs = [], [], []
-        for l in range(2):  # _create_fcnn order (:52-59,:62-67): Linear, orthogonal_, zero bias, then spectral_norm
+        for l in range(2):  # _create_fcnn order (:52-59,:62-67): Linear, orthogonal_, zero bias, then spectral_norm (this replica's flag)
           layer = torch.nn.Linear(dims[l], dims[l + 1])
           torch.nn.init.orthogonal_(layer.weight, gain=torch.nn.init.calculate_gain('relu') if l == 0 else 1)
           torch.nn.init.constant_(layer.bias, 0)
           w = layer.weight.detach()
-          if self.spectral_norm:
+          if sn_list[r]:
             u_, v_ = _spectral_norm_init(w)
             us.append(u_)
             vs.append(v_)
           params += [w, layer.bias.detach()]
         self.mlp.load_params(r, 0, params)
-        if self.spectral_norm:
+        if sn_list[r]:
           self.u[r].copy_(torch.cat(us))
           self.v[r].copy_(torch.cat(vs))
+    self.set_choices(rf_list, sn_list)
     self.training = True
+
+  def set_choices(self, reward_function, spectral_norm):
+    """Per-replica reward function / spectral-norm flag of the fused discriminator (one value or R values; R equal values are the uniform path).
+    A replica without spectral norm never reads or writes its u / v rows. Trainer(fast_init=True) sets them after replicating replica 0."""
+    R = self.replicas
+    rf_list, sn_list = _per_replica_choice(reward_function, R), [bool(x) for x in _per_replica_choice(spectral_norm, R)]
+    for x in rf_list: assert x in _lib.REWARD, f'reward_function {x!r} not in {sorted(_lib.REWARD)}'
+    assert not any(sn_list) or self.u is not None, 'spectral norm needs the u / v buffers (construct with spectral_norm on for some replica)'
+    self.reward_function, self.spectral_norm = rf_list[0], any(sn_list)
+    self._reward_function_r = torch.tensor([_lib.REWARD[x] for x in rf_list], dtype=torch.int32, device=self.device) if len(set(rf_list)) > 1 else None
+    if len(set(sn_list)) > 1:
+      self.spectral_norm_r = sn_list
+      self._spectral_norm_r = torch.tensor(sn_list, dtype=torch.int32, device=self.device)
+    else:
+      self.spectral_norm_r, self._spectral_norm_r = None, None
+      if self.u is not None and not sn_list[0]: self.u, self.v = None, None
 
   # ---- general configuration (models.py:157-162): flat [R, g | h] parameter buffer, per-net spectral-norm vectors ----------------
   def _init_general(self, model_cfg, rng, device):
@@ -467,13 +512,19 @@ class GAILDiscriminator(_Module):
     if self.spectral_norm:
       g.u, g.v, g.u_stride, g.v_stride = self.u.data_ptr(), self.v.data_ptr(), self.u.stride(0), self.v.stride(0)
     g.state_only, g.reward_function = int(self.state_only), _lib.REWARD[self.reward_function]
+    g.reward_function_r, g.spectral_norm_r = _lib.ptr(self._reward_function_r), _lib.ptr(self._spectral_norm_r)
     return g
 
-  def _state_items(self):
+  def state_dict(self, spectral_norm: Optional[bool] = None) -> Dict[str, Tensor]:
+    """Reference key names. spectral_norm: the layout (parametrizations.weight.original / _u / _v, or weight) — by default that of a module
+    with spectral norm on when any replica uses it; with per-replica flags, pass a replica block's own flag and slice that block."""
+    return {k: (v[0] if v.size(0) == 1 else v).detach().clone() for k, v in self._state_items(spectral_norm)}
+
+  def _state_items(self, spectral_norm: Optional[bool] = None):
     if self.general: return self._general_state_items()
     v = self.mlp.layer_views()[0]
     d, H = self.mlp.dims[0], self.mlp.dims[1]
-    if not self.spectral_norm:
+    if not (self.spectral_norm if spectral_norm is None else spectral_norm):
       return [(f'g.{2 * l}.{n}', v[2 * l + i]) for l in range(2) for i, n in enumerate(('weight', 'bias'))]
     return [('g.0.bias', v[1]), ('g.0.parametrizations.weight.original', v[0]), ('g.0.parametrizations.weight.0._u', self.u[:, :H]), ('g.0.parametrizations.weight.0._v', self.v[:, :d]),
             ('g.2.bias', v[3]), ('g.2.parametrizations.weight.original', v[2]), ('g.2.parametrizations.weight.0._u', self.u[:, H:H + 1]),

@@ -6,7 +6,7 @@ counts, RNG counters, the `step` counter) resident on the device — so both seq
 graphs and replayed without host involvement. Replica r is a reference-equivalent run with seed `cfg.seed + r`.
 
 `Trainer(per_replica={key: R values})` gives the replicas their own values of the shape-preserving hyper-parameters
-(config.VECTORISED); `main` runs a multirun sweep (`-m key=a,b,...`) as groups of such Trainers, one replica block per job.
+(config.VECTORISED, and for GAIL the discriminator choices of config.PER_REPLICA_DISCRIMINATOR); `main` runs a multirun sweep (`-m key=a,b,...`) as groups of such Trainers, one replica block per job.
 """
 from __future__ import annotations
 
@@ -61,7 +61,7 @@ def check_config(cfg: Config):
 class Trainer:
   def __init__(self, cfg: Config, replicas: Optional[int] = None, seed_offset: int = 0, fast_init: bool = False, device=None,
                per_replica: Optional[Dict[str, Sequence[float]]] = None):
-    """per_replica: dotted config key (config.VECTORISED) -> R values, replica r training with value r; a key whose values are all equal
+    """per_replica: dotted config key (config.vectorised_keys) -> R values, replica r training with value r; a key whose values are all equal
     runs as that scalar. None: every replica uses the config's values."""
     R = int(cfg.get('replicas', 1) if replicas is None else replicas)
     self.per_replica: Dict[str, List[float]] = {}
@@ -91,20 +91,36 @@ class Trainer:
     nrep = 1 if fast_init else R
     self.actor, self.critic = SoftActor(S, A, cfg.reinforcement.actor, replicas=nrep, rng=rng, device=dev), TwinCritic(S, A, cfg.reinforcement.critic, replicas=nrep, rng=rng, device=dev)
     self.discriminator = None
-    if self.algorithm == 'GAIL': self.discriminator = GAILDiscriminator(S, A, cfg.imitation, cfg.reinforcement.discount, replicas=nrep, rng=rng, device=dev)
+    pr = self.per_replica
+    # per-replica discriminator choices (GAIL sweeps): replica r is initialised with its own spectral-norm flag (fast_init: replica 0's draws with
+    # spectral norm on when any replica uses it, the flags set after replication)
+    rf, sn = pr.get('imitation.discriminator.reward_function'), pr.get('imitation.spectral_norm')
+    if self.algorithm == 'GAIL':
+      self.discriminator = GAILDiscriminator(S, A, cfg.imitation, cfg.reinforcement.discount, replicas=nrep, rng=rng, device=dev, reward_function=None if fast_init else rf,
+                                             spectral_norm=(any(sn) if fast_init else sn) if sn is not None else None)
     elif self.algorithm == 'DRIL': self.discriminator = SoftActor(S, A, cfg.imitation.discriminator, replicas=nrep, rng=rng, device=dev)  # train.py:74
     elif self.algorithm == 'RED': self.discriminator = REDDiscriminator(S, A, cfg.imitation, replicas=nrep, rng=rng, device=dev)  # train.py:82
-    if fast_init and R > 1: self._replicate()
+    if fast_init and R > 1:
+      self._replicate()
+      if self.algorithm == 'GAIL' and (rf is not None or sn is not None):
+        self.discriminator.set_choices(cfg.imitation.discriminator.reward_function if rf is None else rf, cfg.imitation.spectral_norm if sn is None else sn)
     self.log_alpha = torch.zeros(R, device=dev)
     self.target_critic, self.entropy_target = create_target_network(self.critic), cfg.reinforcement.target_temperature * A
     # per-replica values: float64 lists for the optimisers (Python floats in the reference), float32 device tensors for the kernels, each
     # rounded once from the double the scalar path computes
-    pr, f32 = self.per_replica, lambda vals: torch.tensor(vals, dtype=torch.float32, device=dev)
+    f32 = lambda vals: torch.tensor(vals, dtype=torch.float32, device=dev)
     if 'reinforcement.target_temperature' in pr: self.entropy_target = f32([float(t) * A for t in pr['reinforcement.target_temperature']])
     self.discount = f32(pr['reinforcement.discount']) if 'reinforcement.discount' in pr else cfg.reinforcement.discount
     self.polyak_factor = f32(pr['reinforcement.polyak_factor']) if 'reinforcement.polyak_factor' in pr else cfg.reinforcement.polyak_factor
-    self.imitation_cfg = Config(dict(cfg.imitation, **{k.split('.')[1]: f32(pr[k]) for k in ('imitation.grad_penalty', 'imitation.entropy_bonus') if k in pr}))
+    self.imitation_cfg = Config(dict(cfg.imitation, **{k.split('.')[1]: f32(pr[k]) for k in ('imitation.grad_penalty', 'imitation.entropy_bonus', 'imitation.mixup_alpha',
+                                                                                             'imitation.pos_class_prior', 'imitation.nonnegative_margin') if k in pr}))
+    if 'imitation.loss_function' in pr: self.imitation_cfg.loss_function = list(pr['imitation.loss_function'])  # one name per replica
     self._grad_penalty_on = max(pr.get('imitation.grad_penalty', [cfg.imitation.get('grad_penalty', 0)])) > 0  # GAIL only (GAIL.yaml)
+    # the Mixup noise (training.py:106) is drawn for every replica when any replica uses Mixup: U(0, 1) when every alpha is 1, Beta(alpha_r, alpha_r)
+    # otherwise (equal to the uniform draw where alpha_r is 1)
+    self._mixup_on = self.algorithm == 'GAIL' and 'Mixup' in pr.get('imitation.loss_function', [cfg.imitation.get('loss_function')])
+    alphas = pr.get('imitation.mixup_alpha', [float(cfg.imitation.get('mixup_alpha', 1))] * R)
+    self.mixup_alpha = None if all(a == 1.0 for a in alphas) else f32(alphas)
     if self.algorithm == 'GAIL' and isinstance(self.discount, Tensor): self.discriminator.discount = self.discount  # reward shaping (models.py:174)
     hp = lambda k: pr.get(k, get_key(cfg, k))
     lr, wd = hp('training.learning_rate'), hp('training.weight_decay')
@@ -237,9 +253,10 @@ class Trainer:
       from .training import adversarial_imitation_update
       if self._grad_penalty_on and not self.inject: self.rng.uniform(None, self.device, stream_id=5, out=self.eps_gp)
       eps_mix = None
-      if cfg.imitation.loss_function == 'Mixup':  # training.py:106: Beta(a, a) draws; a == 1 (all published configs) is U(0, 1)
-        if float(cfg.imitation.mixup_alpha) != 1.0: raise NotImplementedError('mixup_alpha != 1 needs Beta draws; only mixup_alpha = 1 (the reference default) is on the graph-captured path')
-        if not self.inject: self.rng.uniform(None, self.device, stream_id=8, out=self.eps_mix)
+      if self._mixup_on:  # training.py:106: Beta(a, a) draws; a == 1 (all published configs) is U(0, 1)
+        if not self.inject:
+          if self.mixup_alpha is None: self.rng.uniform(None, self.device, stream_id=8, out=self.eps_mix)
+          else: self.rng.beta(None, self.mixup_alpha, self.device, stream_id=8, out=self.eps_mix)
         eps_mix = self.eps_mix
       self.discriminator.train()  # train.py:178-180
       adversarial_imitation_update(self.actor, self.discriminator, self.batch, self.expert_batch, self.discriminator_optimiser, self.imitation_cfg, eps_gp=self.eps_gp,
@@ -467,7 +484,10 @@ def _train(cfg: Config, blocks, per_replica: Optional[Dict[str, Sequence[float]]
     if rank == 0:  # train.py:237-239
       sd = trainer.state_dicts()
       torch.save(dict(actor=cut(sd['actor'], b), critic=cut(sd['critic'], b), log_alpha=part(sd['log_alpha'], b)), f'{b[0]}agent.pth')
-      if cfg.algorithm in ('DRIL', 'GAIL', 'RED'): torch.save(cut(trainer.discriminator.state_dict(), b), f'{b[0]}discriminator.pth')  # train.py:238
+      if cfg.algorithm in ('DRIL', 'GAIL', 'RED'):  # train.py:238; a job of a spectral-norm sweep writes the layout of its own flag
+        d = trainer.discriminator
+        sd = d.state_dict(spectral_norm=d.spectral_norm_r[b[2]]) if getattr(d, 'spectral_norm_r', None) is not None and b[2] is not None else d.state_dict()
+        torch.save(cut(sd, b), f'{b[0]}discriminator.pth')
       torch.save(m, f'{b[0]}metrics.pth')
   return [float(np.mean(sc)) if sc else float('nan') for sc in scores]
 

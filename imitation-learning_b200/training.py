@@ -2,7 +2,7 @@
 C-ABI entry point that runs the whole update for all replicas on the current CUDA stream.
 
 The scalar hyper-parameters that leave every shape unchanged (discount, entropy_target, polyak_factor, grad_penalty,
-entropy_bonus) are a float (every replica) or an [R] tensor (one value per replica, for hyper-parameter sweeps). Keep such a
+entropy_bonus, mixup_alpha, pos_class_prior, nonnegative_margin) are a float (every replica) or an [R] tensor (one value per replica, for hyper-parameter sweeps). Keep such a
 tensor on the device and alive for as long as a CUDA graph that captured the call is replayed."""
 from __future__ import annotations
 
@@ -37,6 +37,15 @@ def _per_replica(x, R: int, device) -> Tuple[float, Optional[Tensor]]:
   t = torch.as_tensor(x, dtype=torch.float32).to(device).reshape(-1).contiguous()
   assert t.numel() == R, f'per-replica hyper-parameter has {t.numel()} values for {R} replicas'
   return 0.0, t
+
+
+def _choice_codes(owner, key: str, values, table) -> Tensor:
+  """[R] int32 device tensor of table[v] for per-replica string choices, made once per distinct list and kept by `owner` (a captured CUDA graph
+  keeps reading it)."""
+  cache = owner.__dict__.setdefault('_choice_cache', {})
+  k = (key, tuple(values))
+  if k not in cache: cache[k] = torch.tensor([table[v] for v in values], dtype=torch.int32, device=owner.device)
+  return cache[k]
 
 
 def _as_batch(t: Union[TransitionBatch, Dict[str, Tensor]], device) -> Tuple[TransitionBatch, Optional[Tensor]]:
@@ -83,29 +92,40 @@ def sac_update(actor: SoftActor, critic: TwinCritic, log_alpha: Tensor, target_c
 
 def adversarial_imitation_update(actor: SoftActor, discriminator: GAILDiscriminator, transitions, expert_transitions, discriminator_optimiser: Adam, imitation_cfg,
                                  eps_gp: Optional[Tensor] = None, eps_mix: Optional[Tensor] = None, out_losses: Optional[Tensor] = None):
-  """training.py:85-134. `eps_gp` injects the U(0,1) draw of :118 and `eps_mix` the Beta draw of :106."""
+  """training.py:85-134. `eps_gp` injects the U(0,1) draw of :118 and `eps_mix` the Beta draw of :106.
+
+  imitation_cfg.loss_function is a name or one name per replica; mixup_alpha, pos_class_prior and nonnegative_margin are floats or [R] values
+  (per-replica loss function, prior and margin need the fused discriminator). Without `eps_mix`, a scalar mixup_alpha draws as in the
+  reference (U(0, 1) on the device at 1, torch's Beta otherwise) and per-replica values draw Beta(alpha_r, alpha_r) on the device."""
   R, device = discriminator.replicas, discriminator.device
   pol, _ = _as_batch(transitions, device)
   exp, _ = _as_batch(expert_transitions, device)
   B = pol.B
-  loss_function = imitation_cfg.loss_function
+  losses = [imitation_cfg.loss_function] * R if isinstance(imitation_cfg.loss_function, str) else list(imitation_cfg.loss_function)
+  assert len(losses) == R and all(x in _lib.LOSS for x in losses), f'loss_function: one of {sorted(_lib.LOSS)} or R = {R} of them'
+  loss_function = losses[0] if len(set(losses)) == 1 else None  # None: per replica
   (grad_penalty, grad_penalty_r), (entropy_bonus, entropy_bonus_r) = _per_replica(imitation_cfg.grad_penalty, R, device), _per_replica(imitation_cfg.entropy_bonus, R, device)
+  (pos_class_prior, pos_class_prior_r), (nonnegative_margin, nonnegative_margin_r) = (_per_replica(getattr(imitation_cfg, k), R, device) for k in ('pos_class_prior', 'nonnegative_margin'))
   # per-replica grad_penalty: the gradient-penalty pass runs (replicas at 0 skip their contribution inside it)
   if (grad_penalty > 0 or grad_penalty_r is not None) and eps_gp is None: eps_gp = default_rng.uniform((R, B), device, stream_id=21)
-  if loss_function == 'Mixup' and eps_mix is None:
-    alpha = float(imitation_cfg.mixup_alpha)  # training.py:106
-    if alpha == 1.0: eps_mix = default_rng.uniform((R, B), device, stream_id=22)  # Beta(1, 1) = U(0, 1): every published config uses mixup_alpha 1
+  if 'Mixup' in losses and eps_mix is None:
+    alpha, alpha_r = _per_replica(imitation_cfg.mixup_alpha, R, device)  # training.py:106
+    if alpha_r is not None: eps_mix = default_rng.beta((R, B), alpha_r, device, stream_id=22)
+    elif alpha == 1.0: eps_mix = default_rng.uniform((R, B), device, stream_id=22)  # Beta(1, 1) = U(0, 1): every published config uses mixup_alpha 1
     else: eps_mix = torch.distributions.Beta(torch.full((R, B), alpha, device=device), torch.full((R, B), alpha, device=device)).sample()
   as_dev = lambda t: None if t is None else torch.as_tensor(t, dtype=torch.float32).to(device).reshape(R, B).contiguous()
   eps_gp, eps_mix = as_dev(eps_gp), as_dev(eps_mix)
   hyper = (grad_penalty, grad_penalty_r, entropy_bonus, entropy_bonus_r)
   if discriminator.general:
+    if loss_function is None or pos_class_prior_r is not None or nonnegative_margin_r is not None:
+      raise ValueError('per-replica loss_function / pos_class_prior / nonnegative_margin need the fused discriminator (depth 1, relu, no shaping or log-policy term)')
     return _general_adversarial_update(actor, discriminator, pol, exp, discriminator_optimiser, imitation_cfg, hyper, eps_gp, eps_mix, out_losses)
   a = _lib.GailUpdateArgs()
   a.disc, a.opt, a.policy, a.expert = discriminator.c_struct(), discriminator_optimiser.c_struct(), pol.c_struct(), exp.c_struct()
-  a.eps_gp, a.eps_mix, a.R, a.loss_function, a.training = _lib.ptr(eps_gp), _lib.ptr(eps_mix), R, _lib.LOSS[loss_function], int(discriminator.training)
+  a.eps_gp, a.eps_mix, a.R, a.loss_function, a.training = _lib.ptr(eps_gp), _lib.ptr(eps_mix), R, _lib.LOSS[losses[0]], int(discriminator.training)
+  if loss_function is None: a.loss_function_r = _choice_codes(discriminator, 'loss_function', losses, _lib.LOSS).data_ptr()
   a.grad_penalty, a.grad_penalty_r, a.entropy_bonus, a.entropy_bonus_r = grad_penalty, _lib.ptr(grad_penalty_r), entropy_bonus, _lib.ptr(entropy_bonus_r)
-  a.pos_class_prior, a.nonnegative_margin = float(imitation_cfg.pos_class_prior), float(imitation_cfg.nonnegative_margin)
+  a.pos_class_prior, a.pos_class_prior_r, a.nonnegative_margin, a.nonnegative_margin_r = pos_class_prior, _lib.ptr(pos_class_prior_r), nonnegative_margin, _lib.ptr(nonnegative_margin_r)
   a.out_losses = _lib.ptr(out_losses)
   _lib.check(_lib.lib().il_gail_update(_lib.handle(), C.byref(a), _lib.stream()))
 

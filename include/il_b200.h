@@ -115,6 +115,14 @@ int il_debug_gemm(il_handle* h, int M, int N, int K, int G, const float* A, int6
 int il_fill_normal(il_handle* h, float* out, int64_t n, uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream);
 int il_fill_uniform(il_handle* h, float* out, int64_t n, uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream);
 int il_counter_add(il_handle* h, uint64_t* counter, uint64_t inc, void* stream);
+/* [R, n_per_replica] Beta(alpha_r[r], alpha_r[r]) draws (training.py:106 with a per-replica mixup_alpha); alpha_r is an [R] device array.
+ * Element i uses the Philox counter (*counter + i / 4), lane i % 4, like il_fill_uniform: where alpha == 1 the value is bitwise the
+ * il_fill_uniform value, and the caller advances the counter by ceil(R * n_per_replica / 4) as for il_fill_uniform. Other alpha: X / (X + Y),
+ * X, Y ~ Gamma(alpha) (Marsaglia-Tsang; alpha < 1 as Gamma(alpha + 1) U^(1/alpha), in log space), with the rejection draws taken from the
+ * same counter under stream ids tagged in their high word, at most 16 attempts per gamma (then the deterministic value d = shape - 1/3,
+ * the draw at normal 0). alpha must be > 0 (other values give NaN). An element's value depends only on (seed, stream_id, *counter, i, its replica's alpha). */
+int il_fill_beta(il_handle* h, float* out, int R, int64_t n_per_replica, const float* alpha_r, uint64_t seed, uint64_t stream_id, const uint64_t* counter,
+                 void* stream);
 
 /* ---- SoftActor (models.py:84-102) --------------------------------------------------------------------- */
 /* forward + tanh-Gaussian head for n states per replica. eps == NULL: greedy (tanh(mean), models.py:101-102).
@@ -260,6 +268,11 @@ typedef struct il_gail {
   int32_t u_stride, v_stride;
   int32_t state_only;               /* imitation.state_only (models.py:156) */
   int32_t reward_function;          /* IL_REWARD_* */
+  /* [R] per-replica values (hyper-parameter sweeps), read by il_gail_update and il_gail_reward; NULL = the scalar / the u != NULL test.
+   * spectral_norm_r (0 / 1) needs u and v for every replica; a replica at 0 never reads or writes its u / v slots and takes the branches
+   * of a run without spectral norm. */
+  const int32_t* reward_function_r; /* IL_REWARD_* */
+  const int32_t* spectral_norm_r;
 } il_gail;
 typedef struct il_gail_update_args {
   il_gail  disc;
@@ -279,6 +292,11 @@ typedef struct il_gail_update_args {
    * passing eps_gp (the caller passes it when any replica's value is > 0); a replica whose value is 0 skips it as in a uniform run. */
   const float* grad_penalty_r;
   const float* entropy_bonus_r;
+  /* [R] per-replica loss function (IL_LOSS_*), PUGAIL prior and margin; NULL = the scalar. With loss_function_r the caller passes eps_mix
+   * when any replica is Mixup; a Mixup replica runs one loss pass, a BCE / PUGAIL replica two. */
+  const int32_t* loss_function_r;
+  const float* pos_class_prior_r;
+  const float* nonnegative_margin_r;
 } il_gail_update_args;
 int64_t il_gail_workspace_bytes(const il_gail_update_args* a);
 /* adversarial_imitation_update (training.py:85-134) incl. the train()/eval() power-iteration semantics. */
