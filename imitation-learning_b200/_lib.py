@@ -15,6 +15,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'csrc', 'libil_b200.so')
 MAX_LAYERS = 6
+MAX_WIDTH_CLASSES = 8  # IL_MAX_WIDTH_CLASSES: distinct discriminator widths of one il_gail
 ACT = {'relu': 0, 'tanh': 1, 'sigmoid': 2}
 REWARD = {'AIRL': 0, 'GAIL': 1, 'FAIRL': 2}
 LOSS = {'BCE': 0, 'Mixup': 1, 'PUGAIL': 2}
@@ -54,7 +55,8 @@ class BcArgs(C.Structure):
 
 class Gail(C.Structure):
   _fields_ = [('g', Mlp), ('u', vp), ('v', vp), ('u_stride', C.c_int32), ('v_stride', C.c_int32), ('state_only', C.c_int32), ('reward_function', C.c_int32),
-              ('reward_function_r', vp), ('spectral_norm_r', vp)]
+              ('reward_function_r', vp), ('spectral_norm_r', vp), ('n_width_classes', C.c_int32), ('width_class_H', C.c_int32 * MAX_WIDTH_CLASSES),
+              ('width_class_begin', C.c_int32 * MAX_WIDTH_CLASSES), ('_pad', C.c_int32), ('replica_order', vp)]
 
 
 class GailUpdateArgs(C.Structure):

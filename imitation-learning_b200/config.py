@@ -13,6 +13,8 @@ from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import yaml
 
+from ._lib import MAX_WIDTH_CLASSES
+
 CONF_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'conf')
 
 
@@ -94,6 +96,9 @@ VECTORISED = ('training.learning_rate', 'training.weight_decay', 'reinforcement.
 # replica branches on them). The general discriminator (csrc/gail_general.cu) takes only the Mixup alpha per replica.
 PER_REPLICA_DISCRIMINATOR = ('imitation.loss_function', 'imitation.discriminator.reward_function', 'imitation.spectral_norm', 'imitation.mixup_alpha',
                              'imitation.pos_class_prior', 'imitation.nonnegative_margin')
+# The fused GAIL discriminator's hidden size: a per-replica shape (each replica keeps a single run's layout inside the stride of the widest; one
+# launch per width class), with at most MAX_WIDTH_CLASSES distinct widths in one program. The general discriminator groups on it.
+PER_REPLICA_WIDTH = ('imitation.discriminator.hidden_size', )
 # Keys an algorithm never reads: jobs that differ only in them are the same run (GAILDiscriminator never passes its dropout to _create_fcnn,
 # models.py:157-162), so they neither split groups nor become per-replica values.
 UNUSED_KEYS = {'GAIL': ('imitation.discriminator.input_dropout', 'imitation.discriminator.dropout')}
@@ -180,7 +185,7 @@ def vectorised_keys(cfg: Config) -> Tuple[str, ...]:
   gail = cfg.get('algorithm') == 'GAIL'
   general = gail and bool(d.get('reward_shaping') or d.get('subtract_log_policy') or d.get('depth', 1) != 1 or d.get('activation', 'relu') != 'relu')
   keys = tuple(k for k in VECTORISED if not (general and k == 'imitation.grad_penalty'))
-  if gail: keys += ('imitation.mixup_alpha', ) if general else PER_REPLICA_DISCRIMINATOR
+  if gail: keys += ('imitation.mixup_alpha', ) if general else PER_REPLICA_DISCRIMINATOR + PER_REPLICA_WIDTH
   return keys
 
 
@@ -206,6 +211,7 @@ def group_jobs(jobs: List[SweepJob], conf_dir: str = CONF_DIR) -> List[SweepGrou
     vec = vectorised_keys(cfgs[0])
     for k in swept:
       if k in vec: g.per_job[k] = [get_key(c, k) for c in cfgs]
+    for k in PER_REPLICA_WIDTH: _check_width_classes(k, g.per_job.get(k, []))
   return list(groups.values())
 
 
@@ -222,8 +228,16 @@ def set_key(cfg: Dict[str, Any], dotted: str, value: Any):
   node[parts[-1]] = value
 
 
+def _check_width_classes(k: str, vals: Sequence[Any]):
+  n = len(set(vals))
+  if n > MAX_WIDTH_CLASSES: raise SweepError(f'{k}: {n} distinct widths in one program; the fused discriminator takes at most {MAX_WIDTH_CLASSES}')
+
+
 def _per_replica_value(k: str, x: Any) -> Any:
-  """A per-replica value as the config holds it: a name of _CHOICES[k], a bool for spectral_norm, a float otherwise."""
+  """A per-replica value as the config holds it: a name of _CHOICES[k], a bool for spectral_norm, a positive int for a width, a float otherwise."""
+  if k in PER_REPLICA_WIDTH:
+    if isinstance(x, bool) or not isinstance(x, int) or x <= 0: raise SweepError(f'{k}={x!r}: not a positive integer')
+    return x
   if k in _CHOICES:
     if x not in _CHOICES[k]: raise SweepError(f'{k}={x!r}: not one of {", ".join(_CHOICES[k])}')  # train.py:42,44
     return x
@@ -256,6 +270,7 @@ def split_per_replica(cfg: Config, per_replica: Optional[Dict[str, Sequence[Any]
     if k not in allowed: raise SweepError(f'{k} cannot take per-replica values in this configuration (per-replica keys: {", ".join(allowed)})')
     vals = [_per_replica_value(k, x) for x in vals]
     if len(vals) != R: raise SweepError(f'{k}: {len(vals)} values for {R} replicas')
+    if k in PER_REPLICA_WIDTH: _check_width_classes(k, vals)
     if all(x == vals[0] for x in vals): set_key(cfg, k, vals[0])
     else: arrays[k] = vals
   if cfg.get('algorithm') == 'GAIL': _check_gail_replicas(cfg, arrays, R)

@@ -42,10 +42,12 @@ __host__ inline GailDims gail_dims(int S, int A, int H, int B, int state_only, i
   return g;
 }
 
+// `order` (NULL = identity): CTA b runs replica order[b] (one launch per width class: that class's slice of il_gail.replica_order)
 struct GailUpdParams {
   il_gail_update_args a;
   GailDims g;
   int64_t off_w1, off_b1, off_w2, off_b2;
+  const int32_t* order;
 };
 struct GailRewParams {
   il_gail disc;
@@ -54,6 +56,7 @@ struct GailRewParams {
   int64_t off_w1, off_b1, off_w2, off_b2;
   float* reward; int64_t reward_rs; int reward_ld;
   float* logits;
+  const int32_t* order;
 };
 
 __device__ __forceinline__ float bsum(float v, float* red) { return block_sum(v, red); }
@@ -159,7 +162,7 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_kernel(const GailUpdPa
   GailSmem s;
   gail_carve(g, sm, &s);
   const il_gail_update_args& a = p.a;
-  const int r = blockIdx.x, tid = threadIdx.x;
+  const int r = p.order ? p.order[blockIdx.x] : blockIdx.x, tid = threadIdx.x;
   const int H = g.H, d = g.d, B = g.B;
   float* prm = a.disc.g.params + (int64_t)r * a.disc.g.stride;
   const bool sn_r = a.disc.u != nullptr && (!a.disc.spectral_norm_r || a.disc.spectral_norm_r[r] != 0);  // a replica at 0 never touches its u / v slots
@@ -188,6 +191,7 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_kernel(const GailUpdPa
     s.scal[3] = a.pos_class_prior_r ? a.pos_class_prior_r[r] : a.pos_class_prior;
     s.scal[4] = a.nonnegative_margin_r ? a.nonnegative_margin_r[r] : a.nonnegative_margin;
     s.scal[5] = sn_r ? 1.f : 0.f;
+    s.scal[6] = __int_as_float(r);
   }
   __syncthreads();
   auto loss_function = [&] { return __float_as_int(s.scal[2]); };
@@ -422,10 +426,13 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_kernel(const GailUpdPa
     if (is_gp) loss_gp = loss_part * invB; else loss_bce += loss_part * invB;
     __syncthreads();
   }
-  if (tid == 0 && a.out_losses) { a.out_losses[r * 2 + 0] = loss_bce; a.out_losses[r * 2 + 1] = loss_gp; }
+  // the replica index (order[blockIdx.x] in a width-class launch) and the pointers derived from it are re-derived from shared memory here:
+  // kept live from the start in registers they cost the tiled variants spills
+  const int rr = __float_as_int(s.scal[6]);
+  if (tid == 0 && a.out_losses) { a.out_losses[rr * 2 + 0] = loss_bce; a.out_losses[rr * 2 + 1] = loss_gp; }
 
   // ---- AdamW (train.py:84; torch _single_tensor_adam) -----------------------------------------------------------
-  const double lr = a.opt.lr_r ? a.opt.lr_r[r] : a.opt.lr, wd = a.opt.weight_decay_r ? a.opt.weight_decay_r[r] : a.opt.weight_decay;
+  const double lr = a.opt.lr_r ? a.opt.lr_r[rr] : a.opt.lr, wd = a.opt.weight_decay_r ? a.opt.weight_decay_r[rr] : a.opt.weight_decay;
   if (tid == 0) {
     const double t = (double)*a.opt.step;
     s.scal[0] = (float)(lr / (1.0 - pow(a.opt.beta1, t)));
@@ -436,8 +443,9 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_kernel(const GailUpdPa
   const float decay = (float)(1.0 - lr * wd), w1 = (float)(1.0 - a.opt.beta1), w2c = (float)(1.0 - a.opt.beta2), beta2 = (float)a.opt.beta2,
               eps = (float)a.opt.eps;
   const bool has_wd = wd != 0.0;
-  float* am = a.opt.m + (int64_t)r * a.disc.g.stride;
-  float* avv = a.opt.v + (int64_t)r * a.disc.g.stride;
+  prm = a.disc.g.params + (int64_t)rr * a.disc.g.stride;
+  float* am = a.opt.m + (int64_t)rr * a.disc.g.stride;
+  float* avv = a.opt.v + (int64_t)rr * a.disc.g.stride;
   auto adam = [&](int64_t off, float grad) {
     float pi = prm[off], mi = am[off], vi = avv[off];
     if (has_wd) pi = __fmul_rn(pi, decay);
@@ -451,9 +459,9 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_kernel(const GailUpdPa
   for (int h = tid; h < H; h += THREADS) { adam(p.off_b1 + h, s.gb1[h]); adam(p.off_w2 + h, s.G2[h]); }
   if (tid == 0) adam(p.off_b2, gb2);
   if (sn()) {  // persist the power-iteration state (in-place buffers of the parametrization)
-    for (int h = tid; h < H; h += THREADS) { a.disc.u[(int64_t)r * a.disc.u_stride + h] = s.u1[h]; a.disc.v[(int64_t)r * a.disc.v_stride + d + h] = s.v2[h]; }
-    for (int j = tid; j < d; j += THREADS) a.disc.v[(int64_t)r * a.disc.v_stride + j] = s.v1[j];
-    if (tid == 0) a.disc.u[(int64_t)r * a.disc.u_stride + H] = u2;
+    for (int h = tid; h < H; h += THREADS) { a.disc.u[(int64_t)rr * a.disc.u_stride + h] = s.u1[h]; a.disc.v[(int64_t)rr * a.disc.v_stride + d + h] = s.v2[h]; }
+    for (int j = tid; j < d; j += THREADS) a.disc.v[(int64_t)rr * a.disc.v_stride + j] = s.v1[j];
+    if (tid == 0) a.disc.u[(int64_t)rr * a.disc.u_stride + H] = u2;
   }
 }
 
@@ -484,6 +492,7 @@ struct GailTiledParams {
   il_gail_update_args a;
   TDims g;
   int64_t off_w1, off_b1, off_w2, off_b2;
+  const int32_t* order;
 };
 
 // Loads rows [b0, b0 + nb) into X [RB][DP] (zero padded columns / rows); CO = sample weight, DF = mixing epsilon.
@@ -606,7 +615,7 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
   TSmem s;
   tiled_carve(g, sm, &s);
   const il_gail_update_args& a = p.a;
-  const int r = blockIdx.x, tid = threadIdx.x;
+  const int r = p.order ? p.order[blockIdx.x] : blockIdx.x, tid = threadIdx.x;
   const int H = g.H, d = g.d, B = g.B, DP = g.DP, LDZ = g.LDZ;
   float* prm = a.disc.g.params + (int64_t)r * a.disc.g.stride;
   const bool sn_r = a.disc.u != nullptr && (!a.disc.spectral_norm_r || a.disc.spectral_norm_r[r] != 0);  // a replica at 0 never touches its u / v slots
@@ -634,6 +643,7 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
     s.scal[3] = a.pos_class_prior_r ? a.pos_class_prior_r[r] : a.pos_class_prior;
     s.scal[4] = a.nonnegative_margin_r ? a.nonnegative_margin_r[r] : a.nonnegative_margin;
     s.scal[5] = sn_r ? 1.f : 0.f;
+    s.scal[6] = __int_as_float(r);
   }
   __syncthreads();
   auto loss_function = [&] { return __float_as_int(s.scal[2]); };
@@ -916,10 +926,13 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
     if (is_gp) loss_gp = loss_part * invB; else loss_bce += loss_part * invB;
     __syncthreads();
   }
-  if (tid == 0 && a.out_losses) { a.out_losses[r * 2 + 0] = loss_bce; a.out_losses[r * 2 + 1] = loss_gp; }
+  // the replica index (order[blockIdx.x] in a width-class launch) and the pointers derived from it are re-derived from shared memory here:
+  // kept live from the start in registers they cost the tiled variants spills
+  const int rr = __float_as_int(s.scal[6]);
+  if (tid == 0 && a.out_losses) { a.out_losses[rr * 2 + 0] = loss_bce; a.out_losses[rr * 2 + 1] = loss_gp; }
 
   // ---- AdamW (train.py:84; torch _single_tensor_adam) -----------------------------------------------------------
-  const double lr = a.opt.lr_r ? a.opt.lr_r[r] : a.opt.lr, wd = a.opt.weight_decay_r ? a.opt.weight_decay_r[r] : a.opt.weight_decay;
+  const double lr = a.opt.lr_r ? a.opt.lr_r[rr] : a.opt.lr, wd = a.opt.weight_decay_r ? a.opt.weight_decay_r[rr] : a.opt.weight_decay;
   if (tid == 0) {
     const double t = (double)*a.opt.step;
     s.scal[0] = (float)(lr / (1.0 - pow(a.opt.beta1, t)));
@@ -930,8 +943,9 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
   const float decay = (float)(1.0 - lr * wd), w1c = (float)(1.0 - a.opt.beta1), w2c = (float)(1.0 - a.opt.beta2), beta2 = (float)a.opt.beta2,
               eps = (float)a.opt.eps;
   const bool has_wd = wd != 0.0;
-  float* am = a.opt.m + (int64_t)r * a.disc.g.stride;
-  float* avv = a.opt.v + (int64_t)r * a.disc.g.stride;
+  prm = a.disc.g.params + (int64_t)rr * a.disc.g.stride;
+  float* am = a.opt.m + (int64_t)rr * a.disc.g.stride;
+  float* avv = a.opt.v + (int64_t)rr * a.disc.g.stride;
   auto adam = [&](int64_t off, float grad) {
     float pi = prm[off], mi = am[off], vi = avv[off];
     if (has_wd) pi = __fmul_rn(pi, decay);
@@ -945,9 +959,9 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
   for (int h = tid; h < H; h += THREADS) { adam(p.off_b1 + h, s.gb1[h]); adam(p.off_w2 + h, s.G2[h]); }
   if (tid == 0) adam(p.off_b2, gb2);
   if (sn()) {
-    for (int h = tid; h < H; h += THREADS) { a.disc.u[(int64_t)r * a.disc.u_stride + h] = s.u1[h]; a.disc.v[(int64_t)r * a.disc.v_stride + d + h] = s.v2[h]; }
-    for (int j = tid; j < d; j += THREADS) a.disc.v[(int64_t)r * a.disc.v_stride + j] = s.v1[j];
-    if (tid == 0) a.disc.u[(int64_t)r * a.disc.u_stride + H] = u2;
+    for (int h = tid; h < H; h += THREADS) { a.disc.u[(int64_t)rr * a.disc.u_stride + h] = s.u1[h]; a.disc.v[(int64_t)rr * a.disc.v_stride + d + h] = s.v2[h]; }
+    for (int j = tid; j < d; j += THREADS) a.disc.v[(int64_t)rr * a.disc.v_stride + j] = s.v1[j];
+    if (tid == 0) a.disc.u[(int64_t)rr * a.disc.u_stride + H] = u2;
   }
 }
 
@@ -956,7 +970,7 @@ __global__ void __launch_bounds__(THREADS) gail_reward_kernel(const GailRewParam
   const GailDims g = p.g;
   GailSmem s;
   gail_carve(g, sm, &s);
-  const int r = blockIdx.x, tid = threadIdx.x, H = g.H, d = g.d, B = g.B;
+  const int r = p.order ? p.order[blockIdx.x] : blockIdx.x, tid = threadIdx.x, H = g.H, d = g.d, B = g.B;
   const float* prm = p.disc.g.params + (int64_t)r * p.disc.g.stride;
   const bool sn = p.disc.u != nullptr && (!p.disc.spectral_norm_r || p.disc.spectral_norm_r[r] != 0);
   const int reward_function = p.disc.reward_function_r ? p.disc.reward_function_r[r] : p.disc.reward_function;
@@ -1009,7 +1023,7 @@ __global__ void __launch_bounds__(THREADS, 3) gail_reward_tiled_kernel(const Gai
   extern __shared__ __align__(16) float sm[];
   const GailRewParams& p = tp.r;
   const TDims g = tp.g;
-  const int r = blockIdx.x, tid = threadIdx.x, H = g.H, d = g.d, B = g.B, DP = g.DP;
+  const int r = p.order ? p.order[blockIdx.x] : blockIdx.x, tid = threadIdx.x, H = g.H, d = g.d, B = g.B, DP = g.DP;
   int64_t o = 0;
   auto take = [&](int n) { float* q = sm + o; o += (n + 3) / 4 * 4; return q; };
   float *W1 = take(g.HD), *W1eT = take(DP * H), *b1 = take(H), *w2 = take(H), *w2e = take(H), *u1 = take(H), *v2 = take(H), *spare = take(H), *v1 = take(d), *tvec = take(H > d ? H : d);
@@ -1086,6 +1100,115 @@ int gail_setup(const il_gail* disc, const il_batch* batch, GailDims* g, int64_t*
   return 0;
 }
 
+// The width classes of a discriminator (il_gail.width_class_*): each is launched as a uniform run of its width over its slice of
+// replica_order. Without a table: one class of width g.dims[1] over the replicas in order (order = NULL, the kernels use blockIdx.x).
+struct WidthClass { int H, blocks; const int32_t* order; };
+
+int gail_width_classes(const il_gail* disc, int R, WidthClass* cls, int* n, const char* what) {
+  if (disc->n_width_classes == 0 || !disc->replica_order) {
+    cls[0].H = disc->g.dims[1]; cls[0].blocks = R; cls[0].order = nullptr;
+    *n = 1;
+    return 0;
+  }
+  const int nc = disc->n_width_classes;
+  IL_CHECK(nc >= 1 && nc <= IL_MAX_WIDTH_CLASSES, "%s: %d width classes (at most %d)", what, nc, IL_MAX_WIDTH_CLASSES);
+  IL_CHECK(disc->width_class_begin[0] == 0, "%s: the first width class must start at index 0 of replica_order", what);
+  for (int c = 0; c < nc; ++c) {
+    const int b = disc->width_class_begin[c], e = c + 1 < nc ? disc->width_class_begin[c + 1] : R;
+    IL_CHECK(b < e && e <= R, "%s: width class ranges must increase and end at R = %d (class %d: [%d, %d))", what, R, c, b, e);
+    const int H = disc->width_class_H[c];
+    IL_CHECK(H >= 1 && H <= disc->g.dims[1], "%s: width class %d has width %d outside [1, %d] (g.dims[1] is the widest)", what, c, H, disc->g.dims[1]);
+    cls[c].H = H; cls[c].blocks = e - b; cls[c].order = disc->replica_order + b;
+  }
+  *n = nc;
+  return 0;
+}
+
+// The launch il_gail_update makes for one width class: the kernel, shared memory and parameters a uniform run of that width picks.
+struct UpdPlan {
+  int kernel;  // 0..2: gail_update_tiled_kernel<1, 2, 4>; 3..6: gail_update_kernel<4, 16, 32, 64>
+  int blocks;
+  int64_t smem;
+  GailUpdParams p;
+  GailTiledParams tp;
+};
+
+int gail_update_plan(il_handle* h, const il_gail_update_args* a, const WidthClass& wc, UpdPlan* pl) {
+  il_gail disc = a->disc;
+  disc.g.dims[1] = wc.H;
+  GailUpdParams& p = pl->p;
+  p.a = *a;
+  int64_t smem, off[4];
+  IL_TRY(gail_setup(&disc, &a->policy, &p.g, &smem, off, "il_gail_update"));
+  p.off_w1 = off[0]; p.off_b1 = off[1]; p.off_w2 = off[2]; p.off_b2 = off[3];
+  p.order = wc.order;
+  pl->blocks = wc.blocks;
+  const int tiled_tiles = (p.g.H / 4) * ((p.g.d + 3) / 4);
+  if (h->gail_tiled && p.g.d <= 32 && (p.g.H == 32 || p.g.H == 64 || p.g.H == 128) && a->policy.B % 4 == 0 && tiled_tiles <= 256 && p.g.row % 4 == 0) {
+    GailTiledParams& tp = pl->tp;
+    tp.a = *a;
+    TDims& t = tp.g;
+    t.S = p.g.S; t.A = p.g.A; t.d = p.g.d; t.DP = (p.g.d + 3) / 4 * 4; t.H = p.g.H; t.B = p.g.B; t.row = p.g.row; t.LDZ = p.g.H + 4; t.HD = (p.g.H * p.g.d + 3) / 4 * 4;
+    t.RB = a->policy.B < 128 ? (a->policy.B + 15) / 16 * 16 : 128;  // multiple of 16: the tile loops (H / 4 x RB / 4 tiles) have warp-uniform trip counts
+    tp.off_w1 = off[0]; tp.off_b1 = off[1]; tp.off_w2 = off[2]; tp.off_b2 = off[3];
+    tp.order = wc.order;
+    int64_t tsm = tiled_carve(t, nullptr, nullptr);
+    while (tsm > 110 * 1024 && t.RB > 32) {  // wider nets: shorter row chunks keep two CTAs per SM
+      t.RB /= 2;
+      tsm = tiled_carve(t, nullptr, nullptr);
+    }
+    IL_CHECK(tsm <= 110 * 1024, "il_gail_update: tiled kernel shared memory %lld", (long long)tsm);
+    pl->kernel = tiled_tiles <= 64 ? 0 : (tiled_tiles <= 128 ? 1 : 2);
+    pl->smem = tsm;
+    return 0;
+  }
+  const int ne = (p.g.H * p.g.d + THREADS - 1) / THREADS;
+  pl->kernel = ne <= 4 ? 3 : (ne <= 16 ? 4 : (ne <= 32 ? 5 : 6));
+  pl->smem = smem;
+  return 0;
+}
+
+int gail_update_launch(il_handle* h, const UpdPlan& pl, cudaStream_t st) {
+  switch (pl.kernel) {
+    case 0: IL_LAUNCH(h, gail_update_tiled_kernel<1>, pl.blocks, THREADS, (size_t)pl.smem, st, pl.tp); break;
+    case 1: IL_LAUNCH(h, gail_update_tiled_kernel<2>, pl.blocks, THREADS, (size_t)pl.smem, st, pl.tp); break;
+    case 2: IL_LAUNCH(h, gail_update_tiled_kernel<4>, pl.blocks, THREADS, (size_t)pl.smem, st, pl.tp); break;
+    case 3: IL_LAUNCH(h, gail_update_kernel<4>, pl.blocks, THREADS, (size_t)pl.smem, st, pl.p); break;
+    case 4: IL_LAUNCH(h, gail_update_kernel<16>, pl.blocks, THREADS, (size_t)pl.smem, st, pl.p); break;
+    case 5: IL_LAUNCH(h, gail_update_kernel<32>, pl.blocks, THREADS, (size_t)pl.smem, st, pl.p); break;
+    default: IL_LAUNCH(h, gail_update_kernel<64>, pl.blocks, THREADS, (size_t)pl.smem, st, pl.p); break;
+  }
+  return 0;
+}
+
+// The reward launch for one width class (tiled forward when a uniform run of that width takes it).
+int gail_reward_launch(il_handle* h, const il_gail* disc, const WidthClass& wc, const il_batch* batch, float* reward, int64_t reward_rs, int reward_ld, float* logits,
+                       cudaStream_t st) {
+  il_gail dc = *disc;
+  dc.g.dims[1] = wc.H;
+  GailRewParams p;
+  p.disc = *disc; p.batch = *batch;
+  int64_t smem, off[4];
+  IL_TRY(gail_setup(&dc, batch, &p.g, &smem, off, "il_gail_reward"));
+  p.off_w1 = off[0]; p.off_b1 = off[1]; p.off_w2 = off[2]; p.off_b2 = off[3];
+  p.reward = reward; p.reward_rs = reward_rs; p.reward_ld = reward_ld; p.logits = logits;
+  p.order = wc.order;
+  if (h->gail_tiled && p.g.d <= 32 && (p.g.H == 32 || p.g.H == 64 || p.g.H == 128) && p.g.row % 4 == 0) {
+    GailRewTiledParams tp;
+    tp.r = p;
+    TDims& t = tp.g;
+    t.S = p.g.S; t.A = p.g.A; t.d = p.g.d; t.DP = (p.g.d + 3) / 4 * 4; t.H = p.g.H; t.B = p.g.B; t.row = p.g.row; t.LDZ = p.g.H + 4; t.HD = (p.g.H * p.g.d + 3) / 4 * 4;
+    t.RB = batch->B < 64 ? (batch->B + 15) / 16 * 16 : 64;
+    const int64_t tsm = reward_tiled_floats(t) * 4;
+    if (tsm <= 72 * 1024) {
+      IL_LAUNCH(h, gail_reward_tiled_kernel, wc.blocks, THREADS, (size_t)tsm, st, tp);
+      return 0;
+    }
+  }
+  IL_LAUNCH(h, gail_reward_kernel, wc.blocks, THREADS, (size_t)smem, st, p);
+  return 0;
+}
+
 }  // namespace
 
 extern "C" int64_t il_gail_workspace_bytes(const il_gail_update_args*) { return 0; }
@@ -1101,64 +1224,34 @@ extern "C" int il_gail_update(il_handle* h, const il_gail_update_args* a, void* 
   IL_CHECK(!(a->opt.lr_r || a->opt.weight_decay_r) || a->opt.replica_floats == a->disc.g.stride, "il_gail_update: opt.replica_floats must be the discriminator stride");
   // with loss_function_r the scalar is unused and the caller passes eps_mix when any replica is Mixup (the host cannot read the array)
   IL_CHECK(!(!a->loss_function_r && a->loss_function == IL_LOSS_MIXUP && !a->eps_mix), "il_gail_update: Mixup needs eps_mix");
-  GailUpdParams p;
-  p.a = *a;
-  int64_t smem, off[4];
-  IL_TRY(gail_setup(&a->disc, &a->policy, &p.g, &smem, off, "il_gail_update"));
-  p.off_w1 = off[0]; p.off_b1 = off[1]; p.off_w2 = off[2]; p.off_b2 = off[3];
-  cudaStream_t st = (cudaStream_t)stream;
-  IL_LAUNCH(h, gail_tick_kernel, 1, 1, 0, st, a->opt.step);
-  const int tiled_tiles = (p.g.H / 4) * ((p.g.d + 3) / 4);
-  if (h->gail_tiled && p.g.d <= 32 && (p.g.H == 32 || p.g.H == 64 || p.g.H == 128) && a->policy.B % 4 == 0 && tiled_tiles <= 256 && p.g.row % 4 == 0) {
-    GailTiledParams tp;
-    tp.a = *a;
-    TDims& t = tp.g;
-    t.S = p.g.S; t.A = p.g.A; t.d = p.g.d; t.DP = (p.g.d + 3) / 4 * 4; t.H = p.g.H; t.B = p.g.B; t.row = p.g.row; t.LDZ = p.g.H + 4; t.HD = (p.g.H * p.g.d + 3) / 4 * 4;
-    t.RB = a->policy.B < 128 ? (a->policy.B + 15) / 16 * 16 : 128;  // multiple of 16: the tile loops (H / 4 x RB / 4 tiles) have warp-uniform trip counts
-    tp.off_w1 = off[0]; tp.off_b1 = off[1]; tp.off_w2 = off[2]; tp.off_b2 = off[3];
-    int64_t tsm = tiled_carve(t, nullptr, nullptr);
-    while (tsm > 110 * 1024 && t.RB > 32) {  // wider nets: shorter row chunks keep two CTAs per SM
-      t.RB /= 2;
-      tsm = tiled_carve(t, nullptr, nullptr);
-    }
-    IL_CHECK(tsm <= 110 * 1024, "il_gail_update: tiled kernel shared memory %lld", (long long)tsm);
-    if (tiled_tiles <= 64) IL_LAUNCH(h, gail_update_tiled_kernel<1>, a->R, THREADS, (size_t)tsm, st, tp);
-    else if (tiled_tiles <= 128) IL_LAUNCH(h, gail_update_tiled_kernel<2>, a->R, THREADS, (size_t)tsm, st, tp);
-    else IL_LAUNCH(h, gail_update_tiled_kernel<4>, a->R, THREADS, (size_t)tsm, st, tp);
-    return 0;
+  WidthClass cls[IL_MAX_WIDTH_CLASSES];
+  int nc = 0;
+  IL_TRY(gail_width_classes(&a->disc, a->R, cls, &nc, "il_gail_update"));
+  UpdPlan plans[IL_MAX_WIDTH_CLASSES];
+  if (cls[0].order) {  // width classes: the widest layout's checks (u / v strides), then every class's own
+    GailDims g;
+    int64_t smem, off[4];
+    IL_TRY(gail_setup(&a->disc, &a->policy, &g, &smem, off, "il_gail_update"));
   }
-  const int ne = (p.g.H * p.g.d + THREADS - 1) / THREADS;
-#define GAIL_LAUNCH(NE) IL_LAUNCH(h, gail_update_kernel<NE>, a->R, THREADS, (size_t)smem, st, p)
-  if (ne <= 4) GAIL_LAUNCH(4);
-  else if (ne <= 16) GAIL_LAUNCH(16);
-  else if (ne <= 32) GAIL_LAUNCH(32);
-  else GAIL_LAUNCH(64);
-#undef GAIL_LAUNCH
+  for (int c = 0; c < nc; ++c) IL_TRY(gail_update_plan(h, a, cls[c], &plans[c]));
+  cudaStream_t st = (cudaStream_t)stream;
+  IL_LAUNCH(h, gail_tick_kernel, 1, 1, 0, st, a->opt.step);  // one optimiser step per call, whatever the number of classes
+  for (int c = 0; c < nc; ++c) IL_TRY(gail_update_launch(h, plans[c], st));
   return 0;
 }
 
 extern "C" int il_gail_reward(il_handle* h, const il_gail* disc, int R, const il_batch* batch, float* reward, int64_t reward_rs, int reward_ld, float* logits, void* stream) {
   IL_CHECK(h && disc && batch && batch->rows && R > 0, "il_gail_reward: bad argument");
   IL_CHECK(batch->row == row_layout(batch->S, batch->A).len, "il_gail_reward: bad row length");
-  GailRewParams p;
-  p.disc = *disc; p.batch = *batch;
-  int64_t smem, off[4];
-  IL_TRY(gail_setup(disc, batch, &p.g, &smem, off, "il_gail_reward"));
-  p.off_w1 = off[0]; p.off_b1 = off[1]; p.off_w2 = off[2]; p.off_b2 = off[3];
-  p.reward = reward; p.reward_rs = reward_rs; p.reward_ld = reward_ld; p.logits = logits;
-  if (h->gail_tiled && p.g.d <= 32 && (p.g.H == 32 || p.g.H == 64 || p.g.H == 128) && p.g.row % 4 == 0) {
-    GailRewTiledParams tp;
-    tp.r = p;
-    TDims& t = tp.g;
-    t.S = p.g.S; t.A = p.g.A; t.d = p.g.d; t.DP = (p.g.d + 3) / 4 * 4; t.H = p.g.H; t.B = p.g.B; t.row = p.g.row; t.LDZ = p.g.H + 4; t.HD = (p.g.H * p.g.d + 3) / 4 * 4;
-    t.RB = batch->B < 64 ? (batch->B + 15) / 16 * 16 : 64;
-    const int64_t tsm = reward_tiled_floats(t) * 4;
-    if (tsm <= 72 * 1024) {
-      IL_LAUNCH(h, gail_reward_tiled_kernel, R, THREADS, (size_t)tsm, (cudaStream_t)stream, tp);
-      return 0;
-    }
+  WidthClass cls[IL_MAX_WIDTH_CLASSES];
+  int nc = 0;
+  IL_TRY(gail_width_classes(disc, R, cls, &nc, "il_gail_reward"));
+  if (cls[0].order) {
+    GailDims g;
+    int64_t smem, off[4];
+    IL_TRY(gail_setup(disc, batch, &g, &smem, off, "il_gail_reward"));
   }
-  IL_LAUNCH(h, gail_reward_kernel, R, THREADS, (size_t)smem, (cudaStream_t)stream, p);
+  for (int c = 0; c < nc; ++c) IL_TRY(gail_reward_launch(h, disc, cls[c], batch, reward, reward_rs, reward_ld, logits, (cudaStream_t)stream));
   return 0;
 }
 

@@ -343,9 +343,11 @@ class GAILDiscriminator(_Module):
   shaping / log-policy subtraction), with or without spectral norm."""
 
   def __init__(self, state_size: int, action_size: int, imitation_cfg, discount, replicas: int = 1, rng: Optional[ReplicaRNG] = None, device=None,
-               reward_function=None, spectral_norm=None):
-    """reward_function / spectral_norm: None = the config's value; otherwise one value, or one value per replica (hyper-parameter sweeps of the
-    fused discriminator: replica r is initialised, trained and rewarded as a single run with its own values)."""
+               reward_function=None, spectral_norm=None, hidden_size=None):
+    """reward_function / spectral_norm / hidden_size: None = the config's value; otherwise one value, or one value per replica (hyper-parameter
+    sweeps of the fused discriminator: replica r is initialised, trained and rewarded as a single run with its own values). With per-replica
+    widths the flat buffer keeps the stride of the widest replica; replica r's block starts with the layout of a single width-H_r run and the
+    rest of it stays zero."""
     model_cfg = imitation_cfg.discriminator
     self.state_only = bool(imitation_cfg.state_only)
     # reward-shaping discount (models.py:174): a float, or one value per replica (an [R] float32 device tensor, hyper-parameter sweeps)
@@ -356,28 +358,33 @@ class GAILDiscriminator(_Module):
     rf = model_cfg.reward_function if reward_function is None else reward_function
     sn = imitation_cfg.spectral_norm if spectral_norm is None else spectral_norm
     rf_list, sn_list = _per_replica_choice(rf, replicas), [bool(x) for x in _per_replica_choice(sn, replicas)]
+    h_list = [int(x) for x in _per_replica_choice(model_cfg.hidden_size if hidden_size is None else hidden_size, replicas)]
     self.reward_function = rf_list[0]
     self.spectral_norm = any(sn_list)  # u / v are allocated for every replica when any replica uses spectral norm
     self.spectral_norm_r, self._reward_function_r, self._spectral_norm_r = None, None, None
+    self.hidden_size_r, self._width_classes, self._replica_order = None, [], None
     # the default configuration (GAIL.yaml:10-17: one relu hidden layer, no shaping, no log-policy term) runs in the fused one-CTA-per-replica
     # kernel (csrc/gail.cu); every other configuration of models.py:157-175 runs as the replica-batched GEMM program of csrc/gail_general.cu
     self.general = self.reward_shaping or self.subtract_log_policy or model_cfg.depth != 1 or model_cfg.activation != 'relu'
     self._ws = None
     if self.general:
-      if len(set(rf_list)) > 1 or len(set(sn_list)) > 1: raise ValueError('per-replica reward_function / spectral_norm need the fused discriminator (depth 1, relu, no shaping or log-policy term)')
-      self._init_general(model_cfg, rng, device)
+      if len(set(rf_list)) > 1 or len(set(sn_list)) > 1 or len(set(h_list)) > 1:
+        raise ValueError('per-replica reward_function / spectral_norm / hidden_size need the fused discriminator (depth 1, relu, no shaping or log-policy term)')
+      self._init_general(model_cfg, rng, device, h_list[0])
       return
-    d, H = (state_size if self.state_only else state_size + action_size), model_cfg.hidden_size
+    d, H = (state_size if self.state_only else state_size + action_size), max(h_list)
     dims = [d, H, 1]
     self.mlp = ReplicaMLP(dims, 'relu', replicas, 1, device)
     self.device = self.mlp.device
     self.u = torch.zeros(replicas, H + 1, device=self.device) if self.spectral_norm else None  # layer0 u [H], layer1 u [1]
     self.v = torch.zeros(replicas, d + H, device=self.device) if self.spectral_norm else None  # layer0 v [d], layer1 v [H]
+    self._set_widths(h_list)
     for r in range(replicas):
+      dims_r = [d, h_list[r], 1]  # this replica's own width
       with (rng.replica(r) if rng is not None else _null_ctx()):
         params, us, vs = [], [], []
         for l in range(2):  # _create_fcnn order (:52-59,:62-67): Linear, orthogonal_, zero bias, then spectral_norm (this replica's flag)
-          layer = torch.nn.Linear(dims[l], dims[l + 1])
+          layer = torch.nn.Linear(dims_r[l], dims_r[l + 1])
           torch.nn.init.orthogonal_(layer.weight, gain=torch.nn.init.calculate_gain('relu') if l == 0 else 1)
           torch.nn.init.constant_(layer.bias, 0)
           w = layer.weight.detach()
@@ -386,12 +393,32 @@ class GAILDiscriminator(_Module):
             us.append(u_)
             vs.append(v_)
           params += [w, layer.bias.detach()]
-        self.mlp.load_params(r, 0, params)
-        if sn_list[r]:
-          self.u[r].copy_(torch.cat(us))
-          self.v[r].copy_(torch.cat(vs))
+        for view, x in zip(self._width_views(h_list[r]), params): view[r].copy_(x.to(self.device, torch.float32))
+        if sn_list[r]:  # [u0 (H_r) | u1 (1)] and [v0 (d) | v1 (H_r)] as a prefix of the widest rows
+          self.u[r, :h_list[r] + 1].copy_(torch.cat(us))
+          self.v[r, :d + h_list[r]].copy_(torch.cat(vs))
     self.set_choices(rf_list, sn_list)
     self.training = True
+
+  def _set_widths(self, h_list):
+    """The width classes of the fused kernels (il_gail.width_class_*): distinct widths in increasing order, and replica_order, the replicas grouped
+    by class (made once: a captured CUDA graph keeps reading it). R equal widths are the uniform path."""
+    if len(set(h_list)) == 1: return
+    classes = sorted(set(h_list))
+    if len(classes) > _lib.MAX_WIDTH_CLASSES: raise ValueError(f'{len(classes)} distinct discriminator widths; the fused kernels take at most {_lib.MAX_WIDTH_CLASSES}')
+    order, self._width_classes = [], []
+    for H in classes:
+      self._width_classes.append((H, len(order)))
+      order += [r for r, h in enumerate(h_list) if h == H]
+    self.hidden_size_r = list(h_list)
+    self._replica_order = torch.tensor(order, dtype=torch.int32, device=self.device)
+
+  def _width_views(self, H: int) -> List[Tensor]:
+    """[W0 [R, H, d], b0 [R, H], W1 [R, 1, H], b1 [R, 1]] at the offsets of a single width-H net (il_mlp_param_offsets({d, H, 1})), for every replica."""
+    d, R, f = self.mlp.dims[0], self.replicas, self.mlp.flat
+    assert H <= self.mlp.dims[1], f'width {H} exceeds the widest replica ({self.mlp.dims[1]})'
+    w, b, _ = _lib.py_mlp_offsets([d, H, 1])
+    return [f[:, w[0]:w[0] + H * d].view(R, H, d), f[:, b[0]:b[0] + H], f[:, w[1]:w[1] + H].view(R, 1, H), f[:, b[1]:b[1] + 1]]
 
   def set_choices(self, reward_function, spectral_norm):
     """Per-replica reward function / spectral-norm flag of the fused discriminator (one value or R values; R equal values are the uniform path).
@@ -410,9 +437,9 @@ class GAILDiscriminator(_Module):
       if self.u is not None and not sn_list[0]: self.u, self.v = None, None
 
   # ---- general configuration (models.py:157-162): flat [R, g | h] parameter buffer, per-net spectral-norm vectors ----------------
-  def _init_general(self, model_cfg, rng, device):
+  def _init_general(self, model_cfg, rng, device, H):
     R, S, A = self.replicas, self.state_size, self.action_size
-    din, H, depth, act = (S if self.state_only else S + A), model_cfg.hidden_size, model_cfg.depth, model_cfg.activation
+    din, depth, act = (S if self.state_only else S + A), model_cfg.depth, model_cfg.activation
     self.activation = act
     self.g_dims = [din, 1] if self.reward_shaping else [din] + [H] * depth + [1]
     self.h_dims = ([S] + [H] * depth + [1]) if self.reward_shaping else None
@@ -513,17 +540,36 @@ class GAILDiscriminator(_Module):
       g.u, g.v, g.u_stride, g.v_stride = self.u.data_ptr(), self.v.data_ptr(), self.u.stride(0), self.v.stride(0)
     g.state_only, g.reward_function = int(self.state_only), _lib.REWARD[self.reward_function]
     g.reward_function_r, g.spectral_norm_r = _lib.ptr(self._reward_function_r), _lib.ptr(self._spectral_norm_r)
+    if self.hidden_size_r is not None:
+      g.n_width_classes, g.replica_order = len(self._width_classes), self._replica_order.data_ptr()
+      for c, (H, begin) in enumerate(self._width_classes): g.width_class_H[c], g.width_class_begin[c] = H, begin
     return g
 
-  def state_dict(self, spectral_norm: Optional[bool] = None) -> Dict[str, Tensor]:
+  def state_dict(self, spectral_norm: Optional[bool] = None, hidden_size: Optional[int] = None) -> Dict[str, Tensor]:
     """Reference key names. spectral_norm: the layout (parametrizations.weight.original / _u / _v, or weight) — by default that of a module
-    with spectral norm on when any replica uses it; with per-replica flags, pass a replica block's own flag and slice that block."""
-    return {k: (v[0] if v.size(0) == 1 else v).detach().clone() for k, v in self._state_items(spectral_norm)}
+    with spectral norm on when any replica uses it; with per-replica flags, pass a replica block's own flag and slice that block. hidden_size:
+    the shapes of a single run of that width (a replica block's own width, then slice that block); required with per-replica widths."""
+    return {k: (v[0] if v.size(0) == 1 else v).detach().clone() for k, v in self._state_items(spectral_norm, hidden_size)}
 
-  def _state_items(self, spectral_norm: Optional[bool] = None):
+  def load_state_dict(self, sd: Dict[str, Tensor], spectral_norm: Optional[bool] = None, hidden_size: Optional[int] = None):
+    """The inverse of state_dict. With per-replica widths, pass hidden_size: only the replicas of that width are written (from one replica's
+    tensors, or one per replica of that width)."""
+    rows = None
+    if self.hidden_size_r is not None:
+      if hidden_size is None: raise ValueError('per-replica discriminator widths: pass hidden_size (the width of the replicas to load)')
+      rows = torch.tensor([r for r, h in enumerate(self.hidden_size_r) if h == hidden_size], dtype=torch.int64, device=self.device)
+    for k, v in self._state_items(spectral_norm, hidden_size):
+      src = torch.as_tensor(sd[k]).to(v.device, torch.float32)
+      dst = v if rows is None else v[rows]
+      dst.copy_(src.reshape(dst.shape) if src.numel() == dst.numel() else src.unsqueeze(0).expand_as(dst))
+      if rows is not None: v[rows] = dst
+
+  def _state_items(self, spectral_norm: Optional[bool] = None, hidden_size: Optional[int] = None):
     if self.general: return self._general_state_items()
-    v = self.mlp.layer_views()[0]
-    d, H = self.mlp.dims[0], self.mlp.dims[1]
+    if hidden_size is None and self.hidden_size_r is not None:
+      raise ValueError('per-replica discriminator widths have no common layout: pass hidden_size (a replica block\'s width) and slice that block')
+    d, H = self.mlp.dims[0], self.mlp.dims[1] if hidden_size is None else int(hidden_size)
+    v = self._width_views(H)
     if not (self.spectral_norm if spectral_norm is None else spectral_norm):
       return [(f'g.{2 * l}.{n}', v[2 * l + i]) for l in range(2) for i, n in enumerate(('weight', 'bias'))]
     return [('g.0.bias', v[1]), ('g.0.parametrizations.weight.original', v[0]), ('g.0.parametrizations.weight.0._u', self.u[:, :H]), ('g.0.parametrizations.weight.0._v', self.v[:, :d]),

@@ -27,6 +27,14 @@ class ReplicaRNG:
       g.manual_seed(seed + r)
       self.states.append(g.get_state())
 
+  @classmethod
+  def repeated(cls, state: Tensor, replicas: int) -> 'ReplicaRNG':
+    """Every replica starts from the same CPU RNG state: replica r draws what a single run constructed from `state` draws (Trainer(fast_init=True)
+    with per-replica discriminator widths)."""
+    rng = cls(0, 0)
+    rng.states = [state.clone() for _ in range(replicas)]
+    return rng
+
   @contextlib.contextmanager
   def replica(self, r: int):
     saved = torch.get_rng_state()

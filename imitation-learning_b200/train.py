@@ -6,7 +6,7 @@ counts, RNG counters, the `step` counter) resident on the device — so both seq
 graphs and replayed without host involvement. Replica r is a reference-equivalent run with seed `cfg.seed + r`.
 
 `Trainer(per_replica={key: R values})` gives the replicas their own values of the shape-preserving hyper-parameters
-(config.VECTORISED, and for GAIL the discriminator choices of config.PER_REPLICA_DISCRIMINATOR); `main` runs a multirun sweep (`-m key=a,b,...`) as groups of such Trainers, one replica block per job.
+(config.VECTORISED, and for GAIL the discriminator choices of config.PER_REPLICA_DISCRIMINATOR and its hidden size, config.PER_REPLICA_WIDTH); `main` runs a multirun sweep (`-m key=a,b,...`) as groups of such Trainers, one replica block per job.
 """
 from __future__ import annotations
 
@@ -92,12 +92,16 @@ class Trainer:
     self.actor, self.critic = SoftActor(S, A, cfg.reinforcement.actor, replicas=nrep, rng=rng, device=dev), TwinCritic(S, A, cfg.reinforcement.critic, replicas=nrep, rng=rng, device=dev)
     self.discriminator = None
     pr = self.per_replica
-    # per-replica discriminator choices (GAIL sweeps): replica r is initialised with its own spectral-norm flag (fast_init: replica 0's draws with
-    # spectral norm on when any replica uses it, the flags set after replication)
-    rf, sn = pr.get('imitation.discriminator.reward_function'), pr.get('imitation.spectral_norm')
+    # per-replica discriminator choices (GAIL sweeps): replica r is initialised with its own spectral-norm flag and width (fast_init: replica 0's
+    # draws with spectral norm on when any replica uses it, the flags set after replication; with per-replica widths, each replica draws from
+    # replica 0's stream at its own width, so a width class starts where a fast_init run of that width starts)
+    rf, sn, hw = pr.get('imitation.discriminator.reward_function'), pr.get('imitation.spectral_norm'), pr.get('imitation.discriminator.hidden_size')
     if self.algorithm == 'GAIL':
-      self.discriminator = GAILDiscriminator(S, A, cfg.imitation, cfg.reinforcement.discount, replicas=nrep, rng=rng, device=dev, reward_function=None if fast_init else rf,
-                                             spectral_norm=(any(sn) if fast_init else sn) if sn is not None else None)
+      d_rng, d_rep = rng, nrep
+      if fast_init and hw is not None: d_rng, d_rep = ReplicaRNG.repeated(torch.get_rng_state(), R), R
+      self.discriminator = GAILDiscriminator(S, A, cfg.imitation, cfg.reinforcement.discount, replicas=d_rep, rng=d_rng, device=dev, reward_function=None if fast_init else rf,
+                                             spectral_norm=(any(sn) if fast_init else sn) if sn is not None else None, hidden_size=hw)
+      if d_rng is not rng: torch.set_rng_state(d_rng.states[0])  # the global stream goes on as after a fast_init run of replica 0's width
     elif self.algorithm == 'DRIL': self.discriminator = SoftActor(S, A, cfg.imitation.discriminator, replicas=nrep, rng=rng, device=dev)  # train.py:74
     elif self.algorithm == 'RED': self.discriminator = REDDiscriminator(S, A, cfg.imitation, replicas=nrep, rng=rng, device=dev)  # train.py:82
     if fast_init and R > 1:
@@ -484,9 +488,11 @@ def _train(cfg: Config, blocks, per_replica: Optional[Dict[str, Sequence[float]]
     if rank == 0:  # train.py:237-239
       sd = trainer.state_dicts()
       torch.save(dict(actor=cut(sd['actor'], b), critic=cut(sd['critic'], b), log_alpha=part(sd['log_alpha'], b)), f'{b[0]}agent.pth')
-      if cfg.algorithm in ('DRIL', 'GAIL', 'RED'):  # train.py:238; a job of a spectral-norm sweep writes the layout of its own flag
-        d = trainer.discriminator
-        sd = d.state_dict(spectral_norm=d.spectral_norm_r[b[2]]) if getattr(d, 'spectral_norm_r', None) is not None and b[2] is not None else d.state_dict()
+      if cfg.algorithm in ('DRIL', 'GAIL', 'RED'):  # train.py:238; a job of a spectral-norm / width sweep writes the layout of its own flag and width
+        d, kw = trainer.discriminator, {}
+        if b[2] is not None and getattr(d, 'spectral_norm_r', None) is not None: kw['spectral_norm'] = d.spectral_norm_r[b[2]]
+        if b[2] is not None and getattr(d, 'hidden_size_r', None) is not None: kw['hidden_size'] = d.hidden_size_r[b[2]]
+        sd = d.state_dict(**kw)
         torch.save(cut(sd, b), f'{b[0]}discriminator.pth')
       torch.save(m, f'{b[0]}metrics.pth')
   return [float(np.mean(sc)) if sc else float('nan') for sc in scores]

@@ -26,6 +26,7 @@ extern "C" {
 #endif
 
 #define IL_MAX_LAYERS 6
+#define IL_MAX_WIDTH_CLASSES 8           /* distinct discriminator widths of one il_gail (width sweeps) */
 
 enum { IL_ACT_RELU = 0, IL_ACT_TANH = 1, IL_ACT_SIGMOID = 2 };          /* models.py:17 ACTIVATION_FUNCTIONS */
 enum { IL_REWARD_AIRL = 0, IL_REWARD_GAIL = 1, IL_REWARD_FAIRL = 2 };    /* models.py:179-180 */
@@ -273,6 +274,18 @@ typedef struct il_gail {
    * of a run without spectral norm. */
   const int32_t* reward_function_r; /* IL_REWARD_* */
   const int32_t* spectral_norm_r;
+  /* Per-replica hidden sizes (width sweeps). Replica r has width H_r <= g.dims[1] (the widest). Its block of the [R, g.stride] buffer (and of
+   * the AdamW m / v) starts with the layout of a single width-H_r net, il_mlp_param_offsets({d, H_r, 1}); the rest of the block is zero and
+   * never read or written. Its u / v rows hold [u0 (H_r) | u1 (1)] and [v0 (d) | v1 (H_r)] as a prefix of the widest strides.
+   * Width class c (of n_width_classes <= IL_MAX_WIDTH_CLASSES) has width width_class_H[c] and the replicas
+   * replica_order[width_class_begin[c] .. width_class_begin[c + 1]) (the last class ends at R); replica_order ([R], device) lists every
+   * replica once. Each class runs as the launch a uniform run of its width makes. n_width_classes = 0 or replica_order = NULL: every
+   * replica has width g.dims[1]. */
+  int32_t n_width_classes;
+  int32_t width_class_H[IL_MAX_WIDTH_CLASSES];
+  int32_t width_class_begin[IL_MAX_WIDTH_CLASSES];
+  int32_t _pad;
+  const int32_t* replica_order;
 } il_gail;
 typedef struct il_gail_update_args {
   il_gail  disc;
