@@ -6,20 +6,31 @@
 //                      accuracy (error ~2^-21 per product, the dropped lo*lo term) at 3 MMAs per product ("3xTF32").
 //     IL_GEMM_TF32   : hi*hi only (10-bit mantissa operands).
 //
-// Structure: one CTA of two warpgroups per 128 x 256 output tile; warpgroup w owns rows [64 w, 64 w + 64) as the 128
-// fp32 accumulator registers per thread of wgmma.mma_async m64n256k8.tf32. wgmma reads 32-bit operands from shared memory
-// in K-major layout only, and every operand needs the hi/lo split (a CUDA-core pass) anyway, so the operands go global ->
-// registers -> shared memory: all 256 threads load the raw fp32 chunks of k-block i + 1 (16 floats of k) while the
-// wgmmas of k-block i run, split them and store the hi and lo tiles into the other of two shared-memory stages in the
-// canonical K-major SWIZZLE_64B layout. Operands stored [K, rows] in global memory are transposed on the way: a thread
-// loads a 4 (k) x 4 (rows) block with four coalesced 128-bit loads and stores four 16-byte k-chunks, in a per-thread
-// rotated order that keeps the shared-memory stores conflict-free.
+// Structure: persistent CTAs of two warpgroups, one per SM, each walking the 128 x 256 output tiles blockIdx.x,
+// blockIdx.x + gridDim.x, ... (the two M-tiles of a group run in the same wave, so the second read of B hits L2).
+// Warpgroup w owns rows [64 w, 64 w + 64) of the tile as the 128 fp32 accumulator registers per thread of
+// wgmma.mma_async m64n256k8.tf32. wgmma reads 32-bit operands from shared memory in K-major layout only, and every
+// operand needs the hi/lo split (a CUDA-core pass) anyway, so each k-block (16 floats of k) takes three steps, all
+// running at once on different k-blocks of the CTA's continuous k-block stream (it runs on across tile boundaries):
+//   1. copy: cp.async 16-byte copies of the raw fp32 chunks global -> a RAW_STAGES-deep shared-memory ring, no
+//      registers held; k-blocks q + 2 .. q + 1 + RAW_STAGES are in flight while k-block q is multiplied;
+//   2. split: each thread reads back exactly the chunks it copied (so cp.async.wait_group is all the visibility it
+//      needs), splits them and stores the hi and lo tiles into one of three hi/lo stages in the canonical K-major
+//      SWIZZLE_64B layout. Operands stored [K, rows] in global memory are transposed on the way: a thread splits a
+//      4 (k) x 4 (rows) block and stores four 16-byte k-chunks, in a per-thread rotated order that keeps the
+//      shared-memory stores conflict-free;
+//   3. multiply: the 6 (3xTF32) or 2 (TF32) wgmmas of the k-block per warpgroup.
+// Per k-block q: issue the wgmmas of q, split q + 1, issue the copy of q + 1 + RAW_STAGES, wgmma.wait_group 1 (the
+// wgmmas of q - 1 are done) and one CTA barrier. The wgmmas of q keep running across that barrier, and with three hi/lo
+// stages the split of q + 1 only overwrites the stage of q - 2, so the tensor pipe does not drain inside a tile.
 // The epilogue works on the accumulator fragments in registers (bias / activation / activation-derivative mask /
 // fused final linear layer, reduced over the four lanes that share a row) and stores 8-byte pairs; the four lanes of a
-// row fill one 32-byte sector.
+// row fill one 32-byte sector. The copies of the next tile's first k-blocks are in flight while it runs.
 // TMA is not used because the tensor core cannot consume the raw tile: the split pass has to see every element.
-// The pipeline is the simplest correct one — two stages, wgmma.wait_group 0 and one CTA barrier per k-block, one CTA per SM — and
-// its depth has not been tuned on an H100.
+// The k loop never writes the accumulators outside wgmma (they are zeroed before it and read after it), so ptxas adds no
+// wgmma wait of its own and the loop's only wait is wait_group 1.
+// Measured on an H100 80GB HBM3 (SXM, 700 W, 1980 MHz): 3xTF32 256 x 256 x 256 with G = 2048 takes 0.88-0.91 ms per
+// layout (0.48 ms floor at data-sheet rates; the two-stage loop this replaced took 1.04-1.10 ms). See DESIGN.md §3.
 #include "common.cuh"
 #include <cstdio>
 #include <cstdlib>
@@ -30,24 +41,36 @@ constexpr int BM = 128, BN = 256, BK = 16;        // tile: 128 x 256 outputs; k-
 constexpr int THREADS = 256;                      // two warpgroups
 constexpr int A_BYTES = BM * BK * 4, B_BYTES = BN * BK * 4;          // 8 KB / 16 KB per k-block (hi or lo copy)
 constexpr int A_HI = 0, A_LO = A_BYTES, B_HI = 2 * A_BYTES, B_LO = 2 * A_BYTES + B_BYTES;
-constexpr int STAGE_BYTES = 2 * (A_BYTES + B_BYTES);                 // 48 KB
-constexpr int N_STAGES = 2;
+constexpr int STAGE_BYTES = 2 * (A_BYTES + B_BYTES);                 // 48 KB hi/lo stage
+constexpr int N_STAGES = 3;                                          // hi/lo stages: split q + 1 while the wgmmas of q (and the tail of q - 1) read the other two
+constexpr int RAW_STAGES = 3;                                        // raw ring: k-blocks in flight global -> shared memory
 constexpr int HEAD_MAX = 8;                                          // fused head: up to 8 output units (N = 1 critic, 2A <= 8 actor)
 constexpr int HEAD_BYTES = (BN + HEAD_MAX * BN) * 4;                 // bias [256] + head weights [8][256]
 // FUSE: the A operand is not loaded but COMPUTED — the previous (first) MLP layer relu(X W1^T + b1) with K0 <= 16 input
 // columns, evaluated chunk by chunk straight into the swizzled operand tile — so the first hidden activation never
-// round-trips HBM. W1 [256][16] (zero padded), b1 [256] and the tile's input rows [128][16] are staged once per CTA.
+// round-trips HBM. W1 [256][16] (zero padded), b1 [256] and the tile's input rows [128][16] are staged once per tile.
 constexpr int L1_MAXK = 16, L1_ROWS = 256;
 constexpr int L1_W_BYTES = L1_ROWS * L1_MAXK * 4, L1_B_BYTES = L1_ROWS * 4, L1_X_BYTES = BM * L1_MAXK * 4;
-constexpr int HEAD_OFF = N_STAGES * STAGE_BYTES, L1_OFF = HEAD_OFF + HEAD_BYTES;
-constexpr int smem_bytes(bool fuse) { return 1024 + L1_OFF + (fuse ? L1_W_BYTES + L1_B_BYTES + L1_X_BYTES : 0); }  // the first-layer staging only where it is used
+// raw ring slot: A (8 KB, absent with FUSE, which computes A) then B (16 KB)
+constexpr int raw_a_bytes(bool fuse) { return fuse ? 0 : A_BYTES; }
+constexpr int raw_bytes(bool fuse) { return raw_a_bytes(fuse) + B_BYTES; }
+constexpr int RAW_OFF = N_STAGES * STAGE_BYTES;
+constexpr int head_off(bool fuse) { return RAW_OFF + RAW_STAGES * raw_bytes(fuse); }
+constexpr int l1_off(bool fuse) { return head_off(fuse) + HEAD_BYTES; }
+constexpr int smem_bytes(bool fuse) { return 1024 + l1_off(fuse) + (fuse ? L1_W_BYTES + L1_B_BYTES + L1_X_BYTES : 0); }  // the first-layer staging only where it is used
+static_assert(smem_bytes(false) <= 227 * 1024 && smem_bytes(true) <= 227 * 1024, "tc_gemm: shared memory over the 227 KB per-CTA limit");
 
 // ---- PTX wrappers ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void cp_async16(uint32_t dst, const float* src) { asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory"); }
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 // D (64 x 256, fp32, 128 registers per thread) += A (64 x 8, K-major in shared memory) * B (8 x 256, K-major in shared memory)
 __device__ __forceinline__ void wgmma_tf32(float (&d)[128], uint64_t a_desc, uint64_t b_desc) {
   asm volatile(
@@ -95,7 +118,6 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
   asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
   return v;
 }
-__device__ __forceinline__ uint4 ldg128(const float* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
 __device__ __forceinline__ uint32_t hi_of(uint32_t x) { return x & 0xFFFFE000u; }
 __device__ __forceinline__ uint32_t lo_of(uint32_t x) { return __float_as_uint(__uint_as_float(x) - __uint_as_float(x & 0xFFFFE000u)); }
 // one 16-byte chunk (4 consecutive k of one row) into the hi tile and, for 3xTF32, the lo tile at the same offset
@@ -139,58 +161,59 @@ template <int EPI, bool FUSE = false>
 __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  float* head_s = reinterpret_cast<float*>(smem + HEAD_OFF);  // [BN] bias then [HEAD_MAX][BN] head weights
-  const uint32_t stage0 = smem_u32(smem);
-  const uint32_t w1s = stage0 + L1_OFF, b1s = w1s + L1_W_BYTES, xs = b1s + L1_B_BYTES;
+  float* head_s = reinterpret_cast<float*>(smem + head_off(FUSE));  // [BN] bias then [HEAD_MAX][BN] head weights
+  const uint32_t stage0 = smem_u32(smem), raw0 = stage0 + RAW_OFF;
+  const uint32_t w1s = stage0 + l1_off(FUSE), b1s = w1s + L1_W_BYTES, xs = b1s + L1_B_BYTES;
+  constexpr uint32_t RAW_A = 0, RAW_B = raw_a_bytes(FUSE), RAW_BYTES = raw_bytes(FUSE);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
   const GemmArgs& g = p.g;
-  const int nkb = g.K / BK;
-  const int tile = blockIdx.x, grp = tile / p.tiles_m, m0 = (tile % p.tiles_m) * BM;
+  const int nkb = g.K / BK, tiles_m = p.tiles_m;
+  const int my_tiles = (g.G * tiles_m - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;  // tiles blockIdx.x + i gridDim.x
+  const int nq = my_tiles * nkb;                                                                // this CTA's k-block stream
   const bool a_km = FUSE || g.a_kmajor != 0, b_km = g.b_kmajor != 0, split = p.split != 0;
 
-  // ---- per-thread addressing of one k-block ----
+  // ---- per-thread chunks of one k-block ----
   // stored [rows, K]: 16-byte chunk fc of rows fr + 64 j (A: j < 2, B: j < 4)
   // stored [K, rows]: 4 x 4 blocks, rows 4 c4 .. 4 c4 + 3 at k = 4 kg .. 4 kg + 3 (A: 128 blocks on the first warpgroup, B: 256 blocks)
+  // A thread's chunk j sits at (j THREADS + tid) * 16 of its operand's region in the raw slot: the copies and the reads back
+  // of a warp are 512 contiguous bytes.
   const int fr = tid >> 2, fc = tid & 3;
   const int a_c4 = tid & 31, a_kg = (tid >> 5) & 3, b_c4 = tid & 63, b_kg = tid >> 6;
-  const float* a_ptr = nullptr;
-  if (!FUSE) {
-    const float* A = g.A + (int64_t)(grp / g.a_gdiv) * g.a_gs;
-    a_ptr = a_km ? A + (int64_t)(m0 + fr) * g.lda + fc * 4 : A + (int64_t)(a_kg * 4) * g.lda + m0 + a_c4 * 4;
-  }
-  const float* Bg = g.B + (int64_t)(grp / g.b_gdiv) * g.b_gs;
-  const float* b_ptr = b_km ? Bg + (int64_t)fr * g.ldb + fc * 4 : Bg + (int64_t)(b_kg * 4) * g.ldb + b_c4 * 4;
-  const int64_t a_kstep = a_km ? BK : (int64_t)BK * g.lda, b_kstep = b_km ? BK : (int64_t)BK * g.ldb;  // floats per k-block
   const uint32_t km_off = sw64(fr, fc);  // rows fr + 64 j: + j * 4096 bytes (64 rows = 8 atoms)
+  auto tile_of = [&](int i) { return (int)blockIdx.x + i * (int)gridDim.x; };
 
-  uint4 ra[4], rb[4];
-  auto load_kb = [&]() {  // raw chunks of the next k-block into registers
-    if (!FUSE) {
-      if (a_km) {
-        ra[0] = ldg128(a_ptr);
-        ra[1] = ldg128(a_ptr + (int64_t)64 * g.lda);
-      } else if (wg == 0) {
+  auto copy_kb = [&](int q) {  // k-block q of the stream: raw chunks global -> raw slot q % RAW_STAGES; always one commit group
+    if (q < nq) {
+      const int t = tile_of(q / nkb), kb = q % nkb, grp = t / tiles_m, m0 = (t % tiles_m) * BM;
+      const uint32_t raw = raw0 + (uint32_t)(q % RAW_STAGES) * RAW_BYTES + (uint32_t)tid * 16u;
+      if (!FUSE) {
+        const float* A = g.A + (int64_t)(grp / g.a_gdiv) * g.a_gs;
+        if (a_km) {
+          const float* src = A + (int64_t)(m0 + fr) * g.lda + kb * BK + fc * 4;
+          cp_async16(raw + RAW_A, src);
+          cp_async16(raw + RAW_A + THREADS * 16, src + (int64_t)64 * g.lda);
+        } else if (wg == 0) {
+          const float* src = A + (int64_t)(kb * BK + a_kg * 4) * g.lda + m0 + a_c4 * 4;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) ra[k] = ldg128(a_ptr + (int64_t)k * g.lda);
+          for (int k = 0; k < 4; ++k) cp_async16(raw + RAW_A + k * (THREADS / 2) * 16, src + (int64_t)k * g.lda);
+        }
       }
-      a_ptr += a_kstep;
-    }
-    if (b_km) {
+      const float* Bg = g.B + (int64_t)(grp / g.b_gdiv) * g.b_gs;
+      const float* src = b_km ? Bg + (int64_t)fr * g.ldb + kb * BK + fc * 4 : Bg + (int64_t)(kb * BK + b_kg * 4) * g.ldb + b_c4 * 4;
+      const int64_t step = b_km ? (int64_t)64 * g.ldb : (int64_t)g.ldb;  // next chunk j: 64 rows further / the next k
 #pragma unroll
-      for (int j = 0; j < 4; ++j) rb[j] = ldg128(b_ptr + (int64_t)(64 * j) * g.ldb);
-    } else {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) rb[k] = ldg128(b_ptr + (int64_t)k * g.ldb);
+      for (int j = 0; j < 4; ++j) cp_async16(raw + RAW_B + j * THREADS * 16, src + j * step);
     }
-    b_ptr += b_kstep;
+    cp_async_commit();
   };
-  float* hstore = nullptr;
-  if (FUSE && p.l1.store) hstore = p.l1.store + (int64_t)grp * p.l1.store_gs + (int64_t)(m0 + fr) * g.K + fc * 4;
-  auto store_kb = [&](int kb, uint32_t st) {  // split + store the registers (FUSE: compute the A chunks of k-block kb) into stage `st`
+
+  auto split_kb = [&](int q) {  // k-block q: split the raw chunks this thread copied (FUSE: compute the A chunks) into hi/lo stage q % N_STAGES
+    const uint32_t st = stage0 + (uint32_t)(q % N_STAGES) * STAGE_BYTES;
+    const uint32_t raw = raw0 + (uint32_t)(q % RAW_STAGES) * RAW_BYTES + (uint32_t)tid * 16u;
     if (FUSE) {
       // A chunk values: relu(b1[k] + sum_j x[j] W1[k][j]) for k = 16 kb + 4 fc + {0..3}, rows fr and fr + 64
-      const int k0 = kb * BK + fc * 4;
+      const int kb = q % nkb, k0 = kb * BK + fc * 4;
       const uint4 bq = lds128(b1s + (uint32_t)k0 * 4u);
       float c0[4] = {__uint_as_float(bq.x), __uint_as_float(bq.y), __uint_as_float(bq.z), __uint_as_float(bq.w)};
       float c1[4] = {c0[0], c0[1], c0[2], c0[3]};
@@ -200,12 +223,12 @@ __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
         if (c4 < np) {
           const uint4 x0 = lds128(xs + sw64(fr, c4)), x1 = lds128(xs + sw64(fr + 64, c4));
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const uint4 w = lds128(w1s + (uint32_t)((k0 + q) * 64 + ((c4 ^ fc) << 4)));  // W1 row k: chunk c4 at c4 ^ ((k >> 2) & 3)
-            c0[q] = fmaf(__uint_as_float(x0.x), __uint_as_float(w.x), c0[q]); c1[q] = fmaf(__uint_as_float(x1.x), __uint_as_float(w.x), c1[q]);
-            c0[q] = fmaf(__uint_as_float(x0.y), __uint_as_float(w.y), c0[q]); c1[q] = fmaf(__uint_as_float(x1.y), __uint_as_float(w.y), c1[q]);
-            c0[q] = fmaf(__uint_as_float(x0.z), __uint_as_float(w.z), c0[q]); c1[q] = fmaf(__uint_as_float(x1.z), __uint_as_float(w.z), c1[q]);
-            c0[q] = fmaf(__uint_as_float(x0.w), __uint_as_float(w.w), c0[q]); c1[q] = fmaf(__uint_as_float(x1.w), __uint_as_float(w.w), c1[q]);
+          for (int qq = 0; qq < 4; ++qq) {
+            const uint4 w = lds128(w1s + (uint32_t)((k0 + qq) * 64 + ((c4 ^ fc) << 4)));  // W1 row k: chunk c4 at c4 ^ ((k >> 2) & 3)
+            c0[qq] = fmaf(__uint_as_float(x0.x), __uint_as_float(w.x), c0[qq]); c1[qq] = fmaf(__uint_as_float(x1.x), __uint_as_float(w.x), c1[qq]);
+            c0[qq] = fmaf(__uint_as_float(x0.y), __uint_as_float(w.y), c0[qq]); c1[qq] = fmaf(__uint_as_float(x1.y), __uint_as_float(w.y), c1[qq]);
+            c0[qq] = fmaf(__uint_as_float(x0.z), __uint_as_float(w.z), c0[qq]); c1[qq] = fmaf(__uint_as_float(x1.z), __uint_as_float(w.z), c1[qq]);
+            c0[qq] = fmaf(__uint_as_float(x0.w), __uint_as_float(w.w), c0[qq]); c1[qq] = fmaf(__uint_as_float(x1.w), __uint_as_float(w.w), c1[qq]);
           }
         }
       }
@@ -213,42 +236,40 @@ __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
       const uint4 a1 = make_uint4(__float_as_uint(fmaxf(c1[0], 0.f)), __float_as_uint(fmaxf(c1[1], 0.f)), __float_as_uint(fmaxf(c1[2], 0.f)), __float_as_uint(fmaxf(c1[3], 0.f)));
       store_chunk(st + A_HI, st + A_LO, km_off, a0, split);
       store_chunk(st + A_HI, st + A_LO, km_off + 4096u, a1, split);
-      if (hstore) {  // the first hidden activation, for the backward pass
-        *reinterpret_cast<uint4*>(hstore) = a0;
-        *reinterpret_cast<uint4*>(hstore + (int64_t)64 * g.K) = a1;
-        hstore += BK;
+      if (p.l1.store) {  // the first hidden activation, for the backward pass
+        const int t = tile_of(q / nkb);
+        float* hs = p.l1.store + (int64_t)(t / tiles_m) * p.l1.store_gs + (int64_t)((t % tiles_m) * BM + fr) * g.K + k0;
+        *reinterpret_cast<uint4*>(hs) = a0;
+        *reinterpret_cast<uint4*>(hs + (int64_t)64 * g.K) = a1;
       }
     } else if (a_km) {
-      store_chunk(st + A_HI, st + A_LO, km_off, ra[0], split);
-      store_chunk(st + A_HI, st + A_LO, km_off + 4096u, ra[1], split);
+      store_chunk(st + A_HI, st + A_LO, km_off, lds128(raw + RAW_A), split);
+      store_chunk(st + A_HI, st + A_LO, km_off + 4096u, lds128(raw + RAW_A + THREADS * 16), split);
     } else if (wg == 0) {
-      store_block_t(st + A_HI, st + A_LO, a_c4, a_kg, ra, split);
+      uint4 v[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) v[k] = lds128(raw + RAW_A + k * (THREADS / 2) * 16);
+      store_block_t(st + A_HI, st + A_LO, a_c4, a_kg, v, split);
     }
     if (b_km) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) store_chunk(st + B_HI, st + B_LO, km_off + (uint32_t)j * 4096u, rb[j], split);
+      for (int j = 0; j < 4; ++j) store_chunk(st + B_HI, st + B_LO, km_off + (uint32_t)j * 4096u, lds128(raw + RAW_B + j * THREADS * 16), split);
     } else {
-      store_block_t(st + B_HI, st + B_LO, b_c4, b_kg, rb, split);
+      uint4 v[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) v[k] = lds128(raw + RAW_B + k * THREADS * 16);
+      store_block_t(st + B_HI, st + B_LO, b_c4, b_kg, v, split);
     }
   };
 
-  // ---- per-CTA staging: fused-head bias / weights, first-layer parameters and input rows ----
-  if (EPI == 4 || EPI == 6) {
-    const float* wsrc = p.head_w + (int64_t)grp * p.head_gs;
-    if (EPI == 4) {
-      const float* bsrc = g.bias + (int64_t)grp * g.bias_gs;
-      for (int i = tid; i < BN; i += THREADS) head_s[i] = __ldg(bsrc + i);
-    }
-    for (int i = tid; i < p.head_n * BN; i += THREADS) head_s[BN + i] = __ldg(wsrc + (int64_t)(i / BN) * p.head_js + (int64_t)(i % BN) * p.head_ns);
-  }
-  if (FUSE) {
-    const int xk = p.l1.x_k;
+  auto stage_l1 = [&](int t) {  // FUSE: first-layer parameters and input rows of tile t (its split must not have started)
+    const int grp = t / tiles_m, m0 = (t % tiles_m) * BM, xk = p.l1.x_k;
     const float* w1 = p.l1.w1 + (int64_t)grp * p.l1.gs;
     const float* b1 = p.l1.b1 + (int64_t)grp * p.l1.gs;
     const float* x = p.l1.x + (int64_t)(grp / p.l1.x_gdiv) * p.l1.x_gs + (int64_t)m0 * p.l1.x_ld;
-    float* w1f = reinterpret_cast<float*>(smem + L1_OFF);
-    float* b1f = reinterpret_cast<float*>(smem + L1_OFF + L1_W_BYTES);
-    float* xf = reinterpret_cast<float*>(smem + L1_OFF + L1_W_BYTES + L1_B_BYTES);
+    float* w1f = reinterpret_cast<float*>(smem + l1_off(FUSE));
+    float* b1f = reinterpret_cast<float*>(smem + l1_off(FUSE) + L1_W_BYTES);
+    float* xf = reinterpret_cast<float*>(smem + l1_off(FUSE) + L1_W_BYTES + L1_B_BYTES);
     for (int i = tid; i < L1_ROWS * L1_MAXK; i += THREADS) {  // zero-padded to [256][16]
       const int k = i / L1_MAXK, j = i % L1_MAXK;
       w1f[k * L1_MAXK + ((((j >> 2) ^ ((k >> 2) & 3)) << 2) | (j & 3))] = (k < g.K && j < xk) ? __ldg(w1 + (int64_t)k * xk + j) : 0.f;
@@ -258,130 +279,156 @@ __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
       const int r = i / L1_MAXK, j = i % L1_MAXK;
       xf[(sw64(r, j >> 2) >> 2) + (j & 3)] = j < xk ? __ldg(x + (int64_t)r * p.l1.x_ld + j) : 0.f;
     }
+  };
+
+  // ---- prologue: fill the raw ring, split k-block 0 ----
+#pragma unroll 1
+  for (int q = 0; q < RAW_STAGES; ++q) copy_kb(q);
+  if (FUSE) {
+    stage_l1(tile_of(0));
     __syncthreads();
   }
-
-  float acc[128];
-#pragma unroll
-  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-
-  // ---- main loop: the loads and the split pass of k-block kb + 1 overlap the wgmmas of k-block kb ----
-  load_kb();
-  store_kb(0, stage0);
+  cp_async_wait<RAW_STAGES - 1>();
+  split_kb(0);
+  copy_kb(RAW_STAGES);
   fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
   __syncthreads();
   const uint64_t a_desc0 = make_desc(stage0 + (uint32_t)wg * 4096u), b_desc0 = make_desc(stage0);  // this warpgroup's 64 rows of A
-#pragma unroll 1
-  for (int kb = 0; kb < nkb; ++kb) {
-    const uint32_t cur = (uint32_t)(kb & 1) * STAGE_BYTES, nxt = STAGE_BYTES - cur;
-    const bool more = kb + 1 < nkb;
-    if (more) load_kb();
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < BK / 8; ++kk) {  // per MMA (K = 8 tf32): 32 bytes further inside the swizzled 64-byte rows
-      const uint32_t o = cur + kk * 32;
-      const uint64_t ah = a_desc0 + ((o + A_HI) >> 4), al = a_desc0 + ((o + A_LO) >> 4), bh = b_desc0 + ((o + B_HI) >> 4), bl = b_desc0 + ((o + B_LO) >> 4);
-      if (split) {
-        wgmma_tf32(acc, al, bh);
-        wgmma_tf32(acc, ah, bl);
-      }
-      wgmma_tf32(acc, ah, bh);
-    }
-    wgmma_commit();
-    if (more) store_kb(kb + 1, stage0 + nxt);  // that stage was last read by the wgmmas of k-block kb - 1, complete in both warpgroups before the barrier below
-    wgmma_wait_all();
-    fence_proxy_async();
-    __syncthreads();
-  }
 
-  // ---- epilogue on the accumulator fragments: acc[4 i + {0, 1}] = row r0, columns 8 i + 2 (lane % 4) + {0, 1}; acc[4 i + {2, 3}] = row r0 + 8 ----
-  const int r0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), cl = (lane & 3) * 2;
-  float* C = g.C + (int64_t)grp * g.c_gs + (int64_t)r0 * g.ldc + cl;
-  const int64_t c8 = (int64_t)8 * g.ldc;
-  const float* bias = (EPI == 1 || (EPI == 3 && g.bias)) ? g.bias + (int64_t)grp * g.bias_gs + cl : nullptr;
-  const float* mask = (EPI == 2 || (EPI == 3 && g.mask)) ? g.mask + (int64_t)grp * g.mask_gs + (int64_t)r0 * g.ldmask + cl : nullptr;
-  const int64_t m8 = (int64_t)8 * g.ldmask;
-  const uint32_t* mbits = (EPI == 5 || EPI == 6) ? g.mask_bits + (int64_t)grp * g.mask_bits_gs + (int64_t)r0 * (BN / 32) : nullptr;
-  float h0[HEAD_MAX], h1[HEAD_MAX];
+  // ---- tiles blockIdx.x + i gridDim.x; the k-block stream q = i nkb + kb runs on across them ----
+  // The k loop never writes the accumulators outside wgmma (they are zeroed before it and read after it), so nothing in
+  // it makes ptxas wait for the wgmmas in flight: those of k-block q run on across the barrier of step q.
+  float acc[128];
+#pragma unroll 1
+  for (int i = 0, q = 0; i < my_tiles; ++i) {
 #pragma unroll
-  for (int j = 0; j < HEAD_MAX; ++j) h0[j] = h1[j] = 0.f;
-  uint32_t word0 = 0, word1 = 0;  // sign-bit words of the two rows: read (EPI 5 / 6) or built (EPI 4) 32 columns at a time
+    for (int j = 0; j < 128; ++j) acc[j] = 0.f;
+#pragma unroll 1
+    for (int kb = 0; kb < nkb; ++kb, ++q) {  // step q multiplies k-block q, splits q + 1 and copies q + 1 + RAW_STAGES
+      const uint32_t cur = (uint32_t)(q % N_STAGES) * STAGE_BYTES;
+      wgmma_fence();
 #pragma unroll
-  for (int i = 0; i < BN / 8; ++i) {
-    float v00 = acc[4 * i], v01 = acc[4 * i + 1], v10 = acc[4 * i + 2], v11 = acc[4 * i + 3];
-    const int col = 8 * i, bit = (i & 3) * 8 + cl;  // column of v*0 is col + cl; its bit inside the 32-column word
-    if (EPI == 5 || EPI == 6) {  // ReLU derivative from the sign-bit words the forward kernel wrote
-      if ((i & 3) == 0) { word0 = __ldg(mbits + (i >> 2)); word1 = __ldg(mbits + 8 * (BN / 32) + (i >> 2)); }
-      v00 = (word0 >> bit) & 1u ? v00 : 0.f; v01 = (word0 >> (bit + 1)) & 1u ? v01 : 0.f;
-      v10 = (word1 >> bit) & 1u ? v10 : 0.f; v11 = (word1 >> (bit + 1)) & 1u ? v11 : 0.f;
+      for (int kk = 0; kk < BK / 8; ++kk) {  // per MMA (K = 8 tf32): 32 bytes further inside the swizzled 64-byte rows
+        const uint32_t o = cur + kk * 32;
+        const uint64_t ah = a_desc0 + ((o + A_HI) >> 4), al = a_desc0 + ((o + A_LO) >> 4), bh = b_desc0 + ((o + B_HI) >> 4), bl = b_desc0 + ((o + B_LO) >> 4);
+        if (split) {
+          wgmma_tf32(acc, al, bh);
+          wgmma_tf32(acc, ah, bl);
+        }
+        wgmma_tf32(acc, ah, bh);
+      }
+      wgmma_commit();
+      if (q + 1 < nq) {
+        if (FUSE && kb == nkb - 1) {  // the next split starts the next tile: its first-layer staging (every split of this tile is done: barrier of step q - 1)
+          stage_l1(tile_of(i + 1));
+          __syncthreads();
+        }
+        cp_async_wait<RAW_STAGES - 1>();  // this thread's chunks of k-block q + 1
+        split_kb(q + 1);                  // into the stage the wgmmas of q - 2 read (done in both warpgroups: wait + barrier of step q - 1)
+      }
+      copy_kb(q + 1 + RAW_STAGES);        // into the raw slot this thread just read back
+      wgmma_wait<1>();                    // the wgmmas of q - 1 are done; those of q keep running across the barrier
+      fence_proxy_async();
+      __syncthreads();
     }
-    if (EPI == 4) {
-      const float2 b = *reinterpret_cast<const float2*>(head_s + col + cl);
-      v00 = fmaxf(v00 + b.x, 0.f); v01 = fmaxf(v01 + b.y, 0.f); v10 = fmaxf(v10 + b.x, 0.f); v11 = fmaxf(v11 + b.y, 0.f);
-      if (g.bits_out) {  // sign bits of the hidden outputs: all a dX-only backward pass needs of them (1/32 of the bytes)
-        if ((i & 3) == 0) word0 = word1 = 0;
-        word0 |= (v00 > 0.f ? 1u : 0u) << bit | (v01 > 0.f ? 1u : 0u) << (bit + 1);
-        word1 |= (v10 > 0.f ? 1u : 0u) << bit | (v11 > 0.f ? 1u : 0u) << (bit + 1);
-        if ((i & 3) == 3) {  // the four lanes of a row hold 8 bits each of the word
-          word0 |= __shfl_xor_sync(0xffffffffu, word0, 1); word0 |= __shfl_xor_sync(0xffffffffu, word0, 2);
-          word1 |= __shfl_xor_sync(0xffffffffu, word1, 1); word1 |= __shfl_xor_sync(0xffffffffu, word1, 2);
+
+    // ---- epilogue of tile i: acc[4 c + {0, 1}] = row r0, columns 8 c + 2 (lane % 4) + {0, 1}; acc[4 c + {2, 3}] = row r0 + 8 ----
+    const int t = tile_of(i), grp = t / tiles_m, m0 = (t % tiles_m) * BM;
+    if (EPI == 4 || EPI == 6) {  // this tile's fused-head bias / weights, staged while the last wgmmas finish (the previous tile's epilogue
+                                 // finished reading head_s before the barriers of this tile's k loop); BN == THREADS: element tid of each row
+      const float* wsrc = p.head_w + (int64_t)grp * p.head_gs;
+      if (EPI == 4) head_s[tid] = __ldg(g.bias + (int64_t)grp * g.bias_gs + tid);
+#pragma unroll
+      for (int j = 0; j < HEAD_MAX; ++j)
+        if (j < p.head_n) head_s[BN + j * BN + tid] = __ldg(wsrc + (int64_t)j * p.head_js + (int64_t)tid * p.head_ns);
+    }
+    wgmma_wait<0>();
+    if (EPI == 4 || EPI == 6) __syncthreads();
+    const int r0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), cl = (lane & 3) * 2;
+    float* C = g.C + (int64_t)grp * g.c_gs + (int64_t)r0 * g.ldc + cl;
+    const int64_t c8 = (int64_t)8 * g.ldc;
+    const float* bias = (EPI == 1 || (EPI == 3 && g.bias)) ? g.bias + (int64_t)grp * g.bias_gs + cl : nullptr;
+    const float* mask = (EPI == 2 || (EPI == 3 && g.mask)) ? g.mask + (int64_t)grp * g.mask_gs + (int64_t)r0 * g.ldmask + cl : nullptr;
+    const int64_t m8 = (int64_t)8 * g.ldmask;
+    const uint32_t* mbits = (EPI == 5 || EPI == 6) ? g.mask_bits + (int64_t)grp * g.mask_bits_gs + (int64_t)r0 * (BN / 32) : nullptr;
+    uint32_t word0 = 0, word1 = 0;  // sign-bit words of the two rows: read (EPI 5 / 6) or built (EPI 4) 32 columns at a time
+#pragma unroll
+    for (int c = 0; c < BN / 8; ++c) {
+      float v00 = acc[4 * c], v01 = acc[4 * c + 1], v10 = acc[4 * c + 2], v11 = acc[4 * c + 3];
+      const int col = 8 * c, bit = (c & 3) * 8 + cl;  // column of v*0 is col + cl; its bit inside the 32-column word
+      if (EPI == 5 || EPI == 6) {  // ReLU derivative from the sign-bit words the forward kernel wrote
+        if ((c & 3) == 0) { word0 = __ldg(mbits + (c >> 2)); word1 = __ldg(mbits + 8 * (BN / 32) + (c >> 2)); }
+        v00 = (word0 >> bit) & 1u ? v00 : 0.f; v01 = (word0 >> (bit + 1)) & 1u ? v01 : 0.f;
+        v10 = (word1 >> bit) & 1u ? v10 : 0.f; v11 = (word1 >> (bit + 1)) & 1u ? v11 : 0.f;
+      }
+      if (EPI == 4) {
+        const float2 b = *reinterpret_cast<const float2*>(head_s + col + cl);
+        v00 = fmaxf(v00 + b.x, 0.f); v01 = fmaxf(v01 + b.y, 0.f); v10 = fmaxf(v10 + b.x, 0.f); v11 = fmaxf(v11 + b.y, 0.f);
+        if (g.bits_out) {  // sign bits of the hidden outputs: all a dX-only backward pass needs of them (1/32 of the bytes)
+          if ((c & 3) == 0) word0 = word1 = 0;
+          word0 |= (v00 > 0.f ? 1u : 0u) << bit | (v01 > 0.f ? 1u : 0u) << (bit + 1);
+          word1 |= (v10 > 0.f ? 1u : 0u) << bit | (v11 > 0.f ? 1u : 0u) << (bit + 1);
+          if ((c & 3) == 3) {  // the four lanes of a row hold 8 bits each of the word
+            word0 |= __shfl_xor_sync(0xffffffffu, word0, 1); word0 |= __shfl_xor_sync(0xffffffffu, word0, 2);
+            word1 |= __shfl_xor_sync(0xffffffffu, word1, 1); word1 |= __shfl_xor_sync(0xffffffffu, word1, 2);
+            if ((lane & 3) == 0) {
+              uint32_t* bo = g.bits_out + (int64_t)grp * g.bits_out_gs + (int64_t)r0 * (BN / 32) + (c >> 2);
+              bo[0] = word0;
+              bo[8 * (BN / 32)] = word1;
+            }
+          }
+        }
+      }
+      if (EPI == 4 || EPI == 6) {  // the fragment the thin product below reads, in place
+        acc[4 * c] = v00; acc[4 * c + 1] = v01; acc[4 * c + 2] = v10; acc[4 * c + 3] = v11;
+        if (!p.store_c) continue;
+      }
+      if (EPI == 1) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
+        v00 = fmaxf(v00 + b.x, 0.f); v01 = fmaxf(v01 + b.y, 0.f); v10 = fmaxf(v10 + b.x, 0.f); v11 = fmaxf(v11 + b.y, 0.f);
+      } else if (EPI == 2) {
+        const float2 ma = __ldg(reinterpret_cast<const float2*>(mask + col)), mb = __ldg(reinterpret_cast<const float2*>(mask + m8 + col));
+        v00 = ma.x > 0.f ? v00 : 0.f; v01 = ma.y > 0.f ? v01 : 0.f; v10 = mb.x > 0.f ? v10 : 0.f; v11 = mb.y > 0.f ? v11 : 0.f;
+      } else if (EPI == 3) {
+        if (bias) {
+          const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
+          v00 += b.x; v01 += b.y; v10 += b.x; v11 += b.y;
+        }
+        if (g.act >= 0) { v00 = act_apply(v00, g.act); v01 = act_apply(v01, g.act); v10 = act_apply(v10, g.act); v11 = act_apply(v11, g.act); }
+        if (mask) {
+          const float2 ma = __ldg(reinterpret_cast<const float2*>(mask + col)), mb = __ldg(reinterpret_cast<const float2*>(mask + m8 + col));
+          v00 *= act_grad_from_output(ma.x, g.mask_act); v01 *= act_grad_from_output(ma.y, g.mask_act);
+          v10 *= act_grad_from_output(mb.x, g.mask_act); v11 *= act_grad_from_output(mb.y, g.mask_act);
+        }
+      }
+      *reinterpret_cast<float2*>(C + col) = make_float2(v00, v01);
+      *reinterpret_cast<float2*>(C + c8 + col) = make_float2(v10, v11);
+    }
+    if (EPI == 4 || EPI == 6) {  // the next (thin) product on the fragment, one head unit at a time: h[j] = sum_c v[c] * W[j][c]
+      float* ho = p.head_out + (int64_t)grp * p.head_out_gs + (int64_t)r0 * p.head_n;
+      const float* hb = p.head_b ? p.head_b + (int64_t)grp * p.head_gs : nullptr;
+#pragma unroll 1
+      for (int j = 0; j < HEAD_MAX; ++j) {
+        if (j < p.head_n) {
+          float s0 = 0.f, s1 = 0.f;  // the four lanes of a row each sum a quarter of the columns, in column order
+#pragma unroll
+          for (int c = 0; c < BN / 8; ++c) {
+            const float2 w = *reinterpret_cast<const float2*>(head_s + BN + j * BN + 8 * c + cl);
+            s0 = fmaf(acc[4 * c], w.x, s0); s0 = fmaf(acc[4 * c + 1], w.y, s0);
+            s1 = fmaf(acc[4 * c + 2], w.x, s1); s1 = fmaf(acc[4 * c + 3], w.y, s1);
+          }
+          s0 += __shfl_xor_sync(0xffffffffu, s0, 1); s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
+          s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
           if ((lane & 3) == 0) {
-            uint32_t* bo = g.bits_out + (int64_t)grp * g.bits_out_gs + (int64_t)r0 * (BN / 32) + (i >> 2);
-            bo[0] = word0;
-            bo[8 * (BN / 32)] = word1;
+            const float b = hb ? __ldg(hb + j) : 0.f;
+            ho[j] = s0 + b;
+            ho[(int64_t)8 * p.head_n + j] = s1 + b;
           }
         }
       }
     }
-    if (EPI == 4 || EPI == 6) {  // the next (thin) product on the fragment: h[j] += sum_c v[c] * W[j][c]
-#pragma unroll
-      for (int j = 0; j < HEAD_MAX; ++j) {
-        if (j < p.head_n) {
-          const float2 w = *reinterpret_cast<const float2*>(head_s + BN + j * BN + col + cl);
-          h0[j] = fmaf(v00, w.x, h0[j]); h0[j] = fmaf(v01, w.y, h0[j]);
-          h1[j] = fmaf(v10, w.x, h1[j]); h1[j] = fmaf(v11, w.y, h1[j]);
-        }
-      }
-      if (!p.store_c) continue;
-    }
-    if (EPI == 1) {
-      const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
-      v00 = fmaxf(v00 + b.x, 0.f); v01 = fmaxf(v01 + b.y, 0.f); v10 = fmaxf(v10 + b.x, 0.f); v11 = fmaxf(v11 + b.y, 0.f);
-    } else if (EPI == 2) {
-      const float2 ma = __ldg(reinterpret_cast<const float2*>(mask + col)), mb = __ldg(reinterpret_cast<const float2*>(mask + m8 + col));
-      v00 = ma.x > 0.f ? v00 : 0.f; v01 = ma.y > 0.f ? v01 : 0.f; v10 = mb.x > 0.f ? v10 : 0.f; v11 = mb.y > 0.f ? v11 : 0.f;
-    } else if (EPI == 3) {
-      if (bias) {
-        const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
-        v00 += b.x; v01 += b.y; v10 += b.x; v11 += b.y;
-      }
-      if (g.act >= 0) { v00 = act_apply(v00, g.act); v01 = act_apply(v01, g.act); v10 = act_apply(v10, g.act); v11 = act_apply(v11, g.act); }
-      if (mask) {
-        const float2 ma = __ldg(reinterpret_cast<const float2*>(mask + col)), mb = __ldg(reinterpret_cast<const float2*>(mask + m8 + col));
-        v00 *= act_grad_from_output(ma.x, g.mask_act); v01 *= act_grad_from_output(ma.y, g.mask_act);
-        v10 *= act_grad_from_output(mb.x, g.mask_act); v11 *= act_grad_from_output(mb.y, g.mask_act);
-      }
-    }
-    *reinterpret_cast<float2*>(C + col) = make_float2(v00, v01);
-    *reinterpret_cast<float2*>(C + c8 + col) = make_float2(v10, v11);
   }
-  if (EPI == 4 || EPI == 6) {  // the four lanes of a row each hold the partial sums of a quarter of the columns
-    float* ho = p.head_out + (int64_t)grp * p.head_out_gs + (int64_t)r0 * p.head_n;
-    const float* hb = p.head_b ? p.head_b + (int64_t)grp * p.head_gs : nullptr;
-#pragma unroll
-    for (int j = 0; j < HEAD_MAX; ++j) {
-      if (j < p.head_n) {
-        float s0 = h0[j], s1 = h1[j];
-        s0 += __shfl_xor_sync(0xffffffffu, s0, 1); s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-        if ((lane & 3) == 0) {
-          const float b = hb ? __ldg(hb + j) : 0.f;
-          ho[j] = s0 + b;
-          ho[(int64_t)8 * p.head_n + j] = s1 + b;
-        }
-      }
-    }
-  }
+  cp_async_wait<0>();  // the trailing (empty) commit groups
 }
 
 // bias gradient for the dW products routed to the tensor-core engine: out[g, n] = sum_b dY[g, b, n]
@@ -418,12 +465,14 @@ int tc_gemm_init() {
   return 0;
 }
 
-// one CTA per 128 x 256 tile; the tiles of a group are adjacent, so its B operand is read from HBM once and from L2 after that
+// persistent: one CTA per SM, striding over the 128 x 256 tiles. The tiles of a group are adjacent and a wave holds whole
+// groups (the grid is a multiple of tiles_m), so a group's B operand is read from HBM once and from L2 after that.
 template <int EPI, bool FUSE = false>
 static int tc_launch(il_handle* h, TcParams& p, cudaStream_t stream) {
   const GemmArgs& a = p.g;
   p.tiles_m = a.M / BM;
-  IL_LAUNCH(h, (tc_gemm_kernel<EPI, FUSE>), a.G * p.tiles_m, THREADS, smem_bytes(FUSE), stream, p);
+  const int tiles = a.G * p.tiles_m, wave = h->sm_count >= p.tiles_m ? h->sm_count / p.tiles_m * p.tiles_m : h->sm_count;
+  IL_LAUNCH(h, (tc_gemm_kernel<EPI, FUSE>), tiles < wave ? tiles : wave, THREADS, smem_bytes(FUSE), stream, p);
   return 0;
 }
 
