@@ -227,12 +227,13 @@ __global__ void __launch_bounds__(256, 2) gemm_grouped_kernel(const GemmArgs p) 
 
   if constexpr (!A_KMAJOR) {
     if (do_colsum) {  // bias gradient: colsum[m] = sum_k A[k, m], deterministic order
+      constexpr int ACTIVE = A_F4 < THREADS ? A_F4 : THREADS;  // threads that loaded A
+      static_assert(ACTIVE * 4 <= 2 * BK * LDAS, "colsum partials do not fit in As");
       float4* red = reinterpret_cast<float4*>(&As[0][0][0]);
-      red[tid] = csum;
+      if (tid < ACTIVE) red[tid] = csum;  // only these slots are read back; 256 float4 would overrun As for BM = 16
       __syncthreads();
       if (tid < BM && m0 + tid < M) {
-        constexpr int CH = BM / 4;                               // float4 chunks per k row
-        constexpr int ACTIVE = A_F4 < THREADS ? A_F4 : THREADS;  // threads that loaded A
+        constexpr int CH = BM / 4;  // float4 chunks per k row
         const int chunk = tid / 4, comp = tid % 4;
         float s = 0.f;
         for (int t = chunk; t < ACTIVE; t += CH) s += reinterpret_cast<const float*>(&red[t])[comp];
