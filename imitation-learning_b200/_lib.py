@@ -89,7 +89,7 @@ class RedUpdateArgs(C.Structure):
 
 class Pwil(C.Structure):
   _fields_ = [('atoms', vp), ('scale', vp), ('offset', vp), ('weights', vp), ('N', C.c_int32), ('d', C.c_int32), ('S', C.c_int32), ('A', C.c_int32), ('state_only', C.c_int32),
-              ('time_horizon', C.c_int32), ('reward_scale', C.c_float), ('reward_bandwidth', C.c_float)]
+              ('time_horizon', C.c_int32), ('reward_scale', C.c_float), ('reward_bandwidth', C.c_float), ('reward_scale_r', vp), ('reward_bandwidth_r', vp)]
 
 
 class Env(C.Structure):
@@ -153,7 +153,7 @@ SIGNATURES = {
   'il_replay_sample_indices': (C.c_int, [vp, P(Replay), C.c_int, C.c_int, vp, vp, u64, u64, vp, vp]),
   'il_replay_gather': (C.c_int, [vp, P(Replay), C.c_int, vp, P(Batch), vp]),
   'il_mix_expert_rows': (C.c_int, [vp, P(Batch), P(Batch), C.c_int, vp]),
-  'il_adril_relabel': (C.c_int, [vp, P(Batch), P(Batch), C.c_int, C.c_int, C.c_int, vp, vp, f32, vp, C.c_int, C.c_int, vp]),
+  'il_adril_relabel': (C.c_int, [vp, P(Batch), P(Batch), C.c_int, C.c_int, C.c_int, vp, vp, f32, vp, C.c_int, C.c_int, vp, vp, vp]),
   'il_gail_workspace_bytes': (i64, [P(GailUpdateArgs)]),
   'il_gail_update': (C.c_int, [vp, P(GailUpdateArgs), vp]),
   'il_gail_reward': (C.c_int, [vp, P(Gail), C.c_int, P(Batch), vp, i64, C.c_int, vp, vp]),

@@ -102,6 +102,13 @@ PER_REPLICA_WIDTH = ('imitation.discriminator.hidden_size', )
 # Keys an algorithm never reads: jobs that differ only in them are the same run (GAILDiscriminator never passes its dropout to _create_fcnn,
 # models.py:157-162), so they neither split groups nor become per-replica values.
 UNUSED_KEYS = {'GAIL': ('imitation.discriminator.input_dropout', 'imitation.discriminator.dropout')}
+# Other algorithms' own search-space keys that change no shape and no random draw: AdRIL's update frequency and balanced sampling
+# (adril_relabel_kernel reads them per replica), PWIL's reward scale and bandwidth scale (pwil_reward_kernel), DRIL's quantile cutoff (the
+# per-replica threshold q, computed once after pre-training). PWIL's scales are per replica only with imitation.mix_expert_data == 'none':
+# with mixed_batch / prefill_memory the relabelling walk of train.py:136-140 writes scale-dependent rewards into the expert memory, which all
+# replicas share, so there they stay grouping keys.
+PER_REPLICA_ALGORITHM = {'AdRIL': ('imitation.update_freq', 'imitation.balanced'), 'PWIL': ('imitation.reward_scale', 'imitation.reward_bandwidth_scale'),
+                         'DRIL': ('imitation.quantile_cutoff', )}
 _CHOICES = {'imitation.loss_function': ('BCE', 'Mixup', 'PUGAIL'), 'imitation.discriminator.reward_function': ('AIRL', 'FAIRL', 'GAIL')}
 _SWEEP_FUNCTIONS = re.compile(r'^(range|choice|interval|glob|sort|shuffle|tag)\s*\(')
 
@@ -178,14 +185,18 @@ def expand_sweep(argv: Sequence[str]) -> Tuple[bool, List[SweepJob]]:
 
 
 def vectorised_keys(cfg: Config) -> Tuple[str, ...]:
-  """VECTORISED minus the keys a path of this configuration cannot take per replica, plus the discriminator choices for GAIL: the general GAIL
-  discriminator (csrc/gail_general.cu) batches its gradient-penalty pass over replicas, so a replica with grad_penalty 0 would still take that
-  pass's power iteration, and it takes only mixup_alpha of PER_REPLICA_DISCRIMINATOR."""
+  """VECTORISED minus the keys a path of this configuration cannot take per replica, plus the discriminator choices for GAIL and the
+  algorithm's own keys of PER_REPLICA_ALGORITHM: the general GAIL discriminator (csrc/gail_general.cu) batches its gradient-penalty pass over
+  replicas, so a replica with grad_penalty 0 would still take that pass's power iteration, and it takes only mixup_alpha of
+  PER_REPLICA_DISCRIMINATOR; PWIL takes its scales per replica only without expert-data mixing (the expert memory's relabelled rewards
+  depend on them and are shared)."""
   d = cfg.imitation.get('discriminator') or {}
   gail = cfg.get('algorithm') == 'GAIL'
   general = gail and bool(d.get('reward_shaping') or d.get('subtract_log_policy') or d.get('depth', 1) != 1 or d.get('activation', 'relu') != 'relu')
   keys = tuple(k for k in VECTORISED if not (general and k == 'imitation.grad_penalty'))
   if gail: keys += ('imitation.mixup_alpha', ) if general else PER_REPLICA_DISCRIMINATOR + PER_REPLICA_WIDTH
+  alg = cfg.get('algorithm')
+  if alg in PER_REPLICA_ALGORITHM and not (alg == 'PWIL' and cfg.imitation.get('mix_expert_data', 'none') != 'none'): keys += PER_REPLICA_ALGORITHM[alg]
   return keys
 
 
@@ -248,6 +259,20 @@ def _per_replica_value(k: str, x: Any) -> Any:
   return float(x)
 
 
+def _algorithm_value(k: str, x: Any, r: int) -> Any:
+  """A value of PER_REPLICA_ALGORITHM for replica r, as the reference types or asserts it: update_freq an int >= 0 (train.py:37), balanced a
+  bool, quantile_cutoff in [0, 1] (train.py:39), the PWIL scales numbers."""
+  if k == 'imitation.update_freq':
+    if isinstance(x, bool) or not isinstance(x, int) or x < 0: raise SweepError(f'replica {r}: {k}={x!r}: not an integer >= 0')
+    return x
+  if k == 'imitation.balanced':
+    if not isinstance(x, bool): raise SweepError(f'replica {r}: {k}={x!r}: not true / false')
+    return x
+  if isinstance(x, bool) or not isinstance(x, (int, float)): raise SweepError(f'replica {r}: {k}={x!r}: not a number')
+  if k == 'imitation.quantile_cutoff' and not 0 <= x <= 1: raise SweepError(f'replica {r}: {k}={x!r}: not in [0, 1]')
+  return float(x)
+
+
 def _check_gail_replicas(cfg: Config, arrays: Dict[str, List[Any]], R: int):
   """The reference's GAIL asserts (train.py:42-47) for every replica: alpha > 0 for Mixup replicas, 0 <= prior <= 1 and margin >= 0 for PUGAIL ones."""
   val = lambda k, r: arrays[k][r] if k in arrays else get_key(cfg, k)
@@ -262,13 +287,14 @@ def _check_gail_replicas(cfg: Config, arrays: Dict[str, List[Any]], R: int):
 def split_per_replica(cfg: Config, per_replica: Optional[Dict[str, Sequence[Any]]], R: int) -> Tuple[Config, Dict[str, List[Any]]]:
   """(config, arrays) for Trainer(per_replica=...): a key whose R values are all equal becomes that scalar in a copy of the config (the
   uniform path, bit for bit); the others stay per-replica lists. Keys outside vectorised_keys(cfg) and values the reference's asserts refuse
-  (train.py:42-49, per replica for GAIL) are refused."""
+  (train.py:37-49, per replica) are refused."""
   cfg = copy.deepcopy(cfg)
   arrays = {}
   allowed = vectorised_keys(cfg)
   for k, vals in (per_replica or {}).items():
     if k not in allowed: raise SweepError(f'{k} cannot take per-replica values in this configuration (per-replica keys: {", ".join(allowed)})')
-    vals = [_per_replica_value(k, x) for x in vals]
+    per_alg = k in PER_REPLICA_ALGORITHM.get(cfg.get('algorithm'), ())
+    vals = [_algorithm_value(k, x, r) if per_alg else _per_replica_value(k, x) for r, x in enumerate(vals)]
     if len(vals) != R: raise SweepError(f'{k}: {len(vals)} values for {R} replicas')
     if k in PER_REPLICA_WIDTH: _check_width_classes(k, vals)
     if all(x == vals[0] for x in vals): set_key(cfg, k, vals[0])

@@ -169,14 +169,18 @@ __global__ void replay_transfer_state_kernel(il_replay dst, const float* __restr
 //   balanced: the whole batch is the expert batch on "expert" calls (flag[0] != 0) and the policy batch otherwise; the flag alternates per call.
 //   unbalanced: the first B / 2 rows become expert rows (mix_expert_agent_transitions).
 //   rewards: expert rows 1 / num_expert_trajectories (AdRIL) or 1 (SQIL); policy rows -1[round(step) > round(row step)] / max(num_trajectories, 1) or 0.
+// update_freq_r / balanced_r ([R], optional): replica r runs as a uniform call with its own values; NULL = the scalar for every replica.
 __global__ void adril_relabel_kernel(float* __restrict__ rows, int64_t rs, const float* __restrict__ ex, int64_t ex_rs, int R, int B, int row4, int off_reward, int off_step,
                                      int balanced, int update_freq, const int32_t* __restrict__ flag, const float* __restrict__ step_f, float step_offset,
-                                     const int32_t* __restrict__ num_traj, int traj_shared, int num_expert_traj) {
+                                     const int32_t* __restrict__ num_traj, int traj_shared, int num_expert_traj, const int32_t* __restrict__ update_freq_r,
+                                     const int32_t* __restrict__ balanced_r) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= (int64_t)R * B * row4) return;
   const int q = (int)(t % row4);
   const int64_t rb = t / row4;
   const int r = (int)(rb / B), b = (int)(rb % B);
+  if (update_freq_r) update_freq = update_freq_r[r];
+  if (balanced_r) balanced = balanced_r[r];
   const bool expert_row = balanced ? (flag[0] != 0) : (b < B / 2);
   float4* dst = reinterpret_cast<float4*>(rows + (int64_t)r * rs + (int64_t)b * row4 * 4) + q;
   float4 v = expert_row ? __ldg(reinterpret_cast<const float4*>(ex + (int64_t)r * ex_rs + (int64_t)b * row4 * 4) + q) : *dst;
@@ -264,8 +268,12 @@ extern "C" int il_replay_gather(il_handle* h, const il_replay* mem, int R, const
   return 0;
 }
 
+// With update_freq_r / balanced_r the scalars keep a host-known meaning (the host cannot read device arrays during graph capture): balanced = 1
+// when any replica is balanced, update_freq = the largest value. The alternation flag stays one device scalar: every replica of a program
+// calls the relabeller at the same steps, so the balanced replicas see the flag sequence of a uniform balanced run and the others never read it.
 extern "C" int il_adril_relabel(il_handle* h, const il_batch* batch, const il_batch* expert, int R, int balanced, int update_freq, int32_t* sample_expert_flag,
-                                const float* step_f, float step_offset, const int32_t* num_trajectories, int trajectories_shared, int num_expert_trajectories, void* stream) {
+                                const float* step_f, float step_offset, const int32_t* num_trajectories, int trajectories_shared, int num_expert_trajectories, void* stream,
+                                const int32_t* update_freq_r, const int32_t* balanced_r) {
   IL_CHECK(h && R > 0, "il_adril_relabel: bad argument");
   IL_TRY(check_batch(batch, "il_adril_relabel(batch)"));
   IL_TRY(check_batch(expert, "il_adril_relabel(expert)"));
@@ -276,7 +284,8 @@ extern "C" int il_adril_relabel(il_handle* h, const il_batch* batch, const il_ba
   const int row4 = batch->row / 4;
   const int64_t total = (int64_t)R * batch->B * row4;
   IL_LAUNCH(h, adril_relabel_kernel, (unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream, batch->rows, batch->replica_stride, expert->rows, expert->replica_stride, R, batch->B, row4,
-            L.reward, L.step, balanced, update_freq, sample_expert_flag, step_f, step_offset, num_trajectories, trajectories_shared, num_expert_trajectories);
+            L.reward, L.step, balanced, update_freq, sample_expert_flag, step_f, step_offset, num_trajectories, trajectories_shared, num_expert_trajectories, update_freq_r,
+            balanced_r);
   if (balanced) IL_LAUNCH(h, flag_toggle_kernel, 1, 1, 0, (cudaStream_t)stream, sample_expert_flag);
   return 0;
 }

@@ -232,13 +232,21 @@ class SoftActor(_Module):
     _lib.check(_lib.lib().il_dril_reward(_lib.handle(), lp.data_ptr(), R, B, self.ENSEMBLE, None, 0, None, 0, 0, var.data_ptr(), _lib.stream()))
     return self._squeeze(var)
 
-  def set_uncertainty_threshold(self, expert_state: Tensor, expert_action: Tensor, quantile_cutoff: float, masks=None):  # :110-111 (one-off set-up statistic)
+  def set_uncertainty_threshold(self, expert_state: Tensor, expert_action: Tensor, quantile_cutoff, masks=None):  # :110-111 (one-off set-up statistic)
+    """quantile_cutoff: a float, or one float per replica (sweeps). q[r] is the row r of the scalar call with replica r's cutoff: one
+    torch.quantile over all rows per distinct cutoff, its rows taken where the cutoff applies."""
     R = self.replicas
     es = torch.as_tensor(expert_state, dtype=torch.float32).to(self.device)
     ea = torch.as_tensor(expert_action, dtype=torch.float32).to(self.device)
     if es.dim() == 2: es, ea = es.unsqueeze(0).expand(R, -1, -1), ea.unsqueeze(0).expand(R, -1, -1)
     var = self._get_action_uncertainty(es, ea, masks=masks).reshape(R, -1)
-    self._q = torch.quantile(var, quantile_cutoff, dim=1).contiguous()
+    cutoffs = [float(c) for c in _per_replica_choice(quantile_cutoff, R)]
+    if len(set(cutoffs)) == 1: self._q = torch.quantile(var, cutoffs[0], dim=1).contiguous()
+    else:
+      self._q = torch.empty(R, device=self.device)
+      for c in sorted(set(cutoffs)):
+        rows = torch.tensor([r for r in range(R) if cutoffs[r] == c], dtype=torch.long, device=self.device)
+        self._q[rows] = torch.quantile(var, c, dim=1)[rows]
     self.q = float(self._q[0]) if R == 1 else self._q
 
   def predict_reward(self, state: Tensor, action: Tensor, masks=None, out: Optional[Tensor] = None) -> Tensor:  # :113-120
@@ -666,7 +674,10 @@ class GMMILDiscriminator:
 class PWILDiscriminator:
   """:216-249. The expert atoms are shared by all replicas; the remaining-weight vector is per replica."""
 
-  def __init__(self, state_size: int, action_size: int, imitation_cfg, expert_memory: ReplayMemory, time_horizon: int, replicas: int = 1, device=None):
+  def __init__(self, state_size: int, action_size: int, imitation_cfg, expert_memory: ReplayMemory, time_horizon: int, replicas: int = 1, device=None,
+               reward_scale=None, reward_bandwidth_scale=None):
+    """reward_scale / reward_bandwidth_scale: None = the config's value; otherwise one value, or one value per replica (sweeps: replica r's
+    reward is that of a single run with its own scales). R equal values are the uniform path."""
     self.state_only, self.replicas = bool(imitation_cfg.state_only), replicas
     self.state_size, self.action_size, self.time_horizon = state_size, action_size, time_horizon
     self.expert_memory = expert_memory
@@ -676,8 +687,13 @@ class PWILDiscriminator:
     inv_scale[inv_scale == 0] = 1
     self.data_scale, self.data_offset = (1 / inv_scale).contiguous(), offset.contiguous()
     self.atoms = (self.data_scale * (atoms + self.data_offset)).contiguous()  # :229
-    self.reward_scale = imitation_cfg.reward_scale
-    self.reward_bandwidth = imitation_cfg.reward_bandwidth_scale * time_horizon / sqrt(state_size if self.state_only else state_size + action_size)  # :222
+    scales = _per_replica_choice(imitation_cfg.reward_scale if reward_scale is None else reward_scale, replicas)
+    bw_scales = _per_replica_choice(imitation_cfg.reward_bandwidth_scale if reward_bandwidth_scale is None else reward_bandwidth_scale, replicas)
+    bandwidths = [b * time_horizon / sqrt(state_size if self.state_only else state_size + action_size) for b in bw_scales]  # :222
+    self.reward_scale, self.reward_bandwidth = scales[0], bandwidths[0]
+    # per-replica float32 [R] arrays (NULL in the struct when all replicas agree), each value rounded once from the scalar path's double
+    per = lambda vals: torch.tensor(vals, dtype=torch.float32, device=self.device) if len(set(vals)) > 1 else None
+    self.reward_scale_r, self.reward_bandwidth_r = per(scales), per(bandwidths)
     self.expert_weights = torch.empty(replicas, self.atoms.size(0), device=self.device)
     self.reset()
 
@@ -690,6 +706,7 @@ class PWILDiscriminator:
     p.atoms, p.scale, p.offset, p.weights = self.atoms.data_ptr(), self.data_scale.data_ptr(), self.data_offset.data_ptr(), self.expert_weights.data_ptr()
     p.N, p.d, p.S, p.A = self.atoms.size(0), self.atoms.size(1), self.state_size, self.action_size
     p.state_only, p.time_horizon, p.reward_scale, p.reward_bandwidth = int(self.state_only), self.time_horizon, self.reward_scale, self.reward_bandwidth
+    p.reward_scale_r, p.reward_bandwidth_r = _lib.ptr(self.reward_scale_r), _lib.ptr(self.reward_bandwidth_r)
     return p
 
   def reset(self, mask: Optional[Tensor] = None):  # :228-230
@@ -808,11 +825,22 @@ def mix_expert_agent_transitions(transitions: TransitionBatch, expert_transition
 
 class RewardRelabeller:
   """:293-318 — AdRIL (update_freq > 0) / SQIL (update_freq == 0): builds the training batch from expert and policy data and labels the
-  rewards; one kernel, with the balanced-sampling alternation flag kept on the device so the call can live inside a captured CUDA graph."""
+  rewards; one kernel, with the balanced-sampling alternation flag kept on the device so the call can live inside a captured CUDA graph.
 
-  def __init__(self, update_freq: int, balanced: bool, device=None):
-    self.update_freq, self.balanced = int(update_freq), bool(balanced)
+  update_freq / balanced: one value, or one value per replica (sweeps: replica r relabels as a single run with its own values; R equal
+  values are the uniform path). With per-replica values `update_freq` is the largest and `balanced` is whether any replica is balanced, the
+  host-known scalars of il_adril_relabel; `update_freq_r` / `balanced_r` hold the lists."""
+
+  def __init__(self, update_freq, balanced, device=None):
     self.device = torch.device('cuda') if device is None else torch.device(device)
+    as_list = lambda x: list(x) if isinstance(x, (list, tuple)) else [x]
+    uf, bal = [int(x) for x in as_list(update_freq)], [bool(x) for x in as_list(balanced)]
+    self.update_freq, self.balanced = max(uf), any(bal)
+    self.update_freq_r = uf if len(set(uf)) > 1 else None
+    self.balanced_r = bal if len(set(bal)) > 1 else None
+    i32 = lambda vals: torch.tensor(vals, dtype=torch.int32, device=self.device)
+    self._update_freq_r = None if self.update_freq_r is None else i32(self.update_freq_r)  # made once: a captured graph keeps reading them
+    self._balanced_r = None if self.balanced_r is None else i32([int(b) for b in self.balanced_r])
     self._flag = torch.ones(1, dtype=torch.int32, device=self.device)  # sample_expert = True (:295)
 
   @property
@@ -823,6 +851,8 @@ class RewardRelabeller:
     R, dev = transitions.R, self.device
     step_t = step if torch.is_tensor(step) else torch.full((R, ), float(step), device=dev)
     nt = num_trajectories if torch.is_tensor(num_trajectories) else torch.full((R, ), int(num_trajectories), dtype=torch.int32, device=dev)
+    for a in (self._update_freq_r, self._balanced_r): assert a is None or a.numel() == R, f'{a.numel()} per-replica values for {R} replicas'
     b, e = transitions.c_struct(), expert_transitions.c_struct()
     _lib.check(_lib.lib().il_adril_relabel(_lib.handle(), C.byref(b), C.byref(e), R, int(self.balanced), self.update_freq, self._flag.data_ptr(), step_t.data_ptr(), float(step_offset),
-                                           nt.data_ptr(), int(nt.numel() == 1), int(num_expert_trajectories), _lib.stream()))
+                                           nt.data_ptr(), int(nt.numel() == 1), int(num_expert_trajectories), _lib.stream(), _lib.ptr(self._update_freq_r),
+                                           _lib.ptr(self._balanced_r)))

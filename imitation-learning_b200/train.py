@@ -6,7 +6,8 @@ counts, RNG counters, the `step` counter) resident on the device — so both seq
 graphs and replayed without host involvement. Replica r is a reference-equivalent run with seed `cfg.seed + r`.
 
 `Trainer(per_replica={key: R values})` gives the replicas their own values of the shape-preserving hyper-parameters
-(config.VECTORISED, and for GAIL the discriminator choices of config.PER_REPLICA_DISCRIMINATOR and its hidden size, config.PER_REPLICA_WIDTH); `main` runs a multirun sweep (`-m key=a,b,...`) as groups of such Trainers, one replica block per job.
+(config.VECTORISED, for GAIL the discriminator choices of config.PER_REPLICA_DISCRIMINATOR and its hidden size, config.PER_REPLICA_WIDTH, and
+the AdRIL / PWIL / DRIL keys of config.PER_REPLICA_ALGORITHM); `main` runs a multirun sweep (`-m key=a,b,...`) as groups of such Trainers, one replica block per job.
 """
 from __future__ import annotations
 
@@ -32,8 +33,9 @@ from .optim import Adam, AdamW
 ACCELERATED = ['AdRIL', 'BC', 'DRIL', 'SAC', 'GAIL', 'GMMIL', 'PWIL', 'RED']
 
 
-def check_config(cfg: Config):
-  """train.py:28-48."""
+def check_config(cfg: Config, per_replica: Optional[Dict[str, Sequence]] = None):
+  """train.py:28-48; the AdRIL / DRIL asserts hold for every replica's value in `per_replica` (config.split_per_replica's arrays)."""
+  pr = per_replica or {}
   assert cfg.algorithm in ['AdRIL', 'BC', 'DRIL', 'GAIL', 'GMMIL', 'PWIL', 'RED', 'SAC']
   assert cfg.env in ENVS
   cfg.memory.size = min(cfg.steps, cfg.memory.size)
@@ -43,8 +45,8 @@ def check_config(cfg: Config):
   assert cfg.imitation.mix_expert_data in ['none', 'mixed_batch', 'prefill_memory']
   if cfg.algorithm == 'AdRIL':  # train.py:35-37
     assert cfg.imitation.mix_expert_data == 'mixed_batch'
-    assert cfg.imitation.update_freq >= 0
-  if cfg.algorithm == 'DRIL': assert 0 <= cfg.imitation.quantile_cutoff <= 1  # train.py:38-39
+    assert all(f >= 0 for f in pr.get('imitation.update_freq', [cfg.imitation.update_freq]))
+  if cfg.algorithm == 'DRIL': assert all(0 <= q <= 1 for q in pr.get('imitation.quantile_cutoff', [cfg.imitation.quantile_cutoff]))  # train.py:38-39
   if cfg.algorithm == 'GAIL':
     assert cfg.imitation.mix_expert_data != 'prefill_memory'
     assert cfg.imitation.discriminator.reward_function in ['AIRL', 'FAIRL', 'GAIL']
@@ -67,7 +69,7 @@ class Trainer:
     self.per_replica: Dict[str, List[float]] = {}
     if per_replica: cfg, self.per_replica = split_per_replica(cfg, per_replica, R)
     for k in ('imitation.grad_penalty', 'imitation.entropy_bonus'): assert min(self.per_replica.get(k, [0.0])) >= 0, k  # train.py:48-49
-    check_config(cfg)
+    check_config(cfg, self.per_replica)
     self.cfg = cfg
     self.R = R
     self.device = dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
@@ -143,12 +145,13 @@ class Trainer:
     if self.algorithm == 'GAIL':
       self.discriminator.eval()  # train.py:147
     elif self.algorithm == 'AdRIL':
-      self.discriminator = RewardRelabeller(cfg.imitation.update_freq, cfg.imitation.balanced, device=dev)  # train.py:72
+      self.discriminator = RewardRelabeller(hp('imitation.update_freq'), hp('imitation.balanced'), device=dev)  # train.py:72
       self._expert_trajectories = int(self.expert_memory.num_trajectories)  # constant: read once, outside any graph capture
     elif self.algorithm == 'GMMIL':
       self.discriminator = GMMILDiscriminator(S, A, cfg.imitation, replicas=R, device=dev)
     elif self.algorithm == 'PWIL':
-      self.discriminator = PWILDiscriminator(S, A, cfg.imitation, self.expert_memory, self.env.max_episode_steps, replicas=R, device=dev)
+      self.discriminator = PWILDiscriminator(S, A, cfg.imitation, self.expert_memory, self.env.max_episode_steps, replicas=R, device=dev,
+                                             reward_scale=hp('imitation.reward_scale'), reward_bandwidth_scale=hp('imitation.reward_bandwidth_scale'))
     if self.expert_memory is not None: self.expert_memory.seed = seed + 7919
     if self.algorithm == 'PWIL' and cfg.imitation.mix_expert_data != 'none': self._pwil_relabel_expert()  # train.py:136-140
     if self.algorithm in ('GMMIL', 'PWIL') and cfg.imitation.mix_expert_data == 'prefill_memory': self.memory.transfer_transitions(self.expert_memory)  # train.py:141,143
@@ -334,7 +337,8 @@ class Trainer:
       else: target_estimation_update(d, self.expert_batch, self.discriminator_optimiser, masks=m)
     em = self.expert_memory
     if self.algorithm == 'DRIL':
-      d.set_uncertainty_threshold(em.rows[0, :, :self.S], em.rows[0, :, self.S:self.S + self.A], cfg.imitation.quantile_cutoff, masks=threshold_masks)  # train.py:127
+      cutoff = self.per_replica.get('imitation.quantile_cutoff', cfg.imitation.quantile_cutoff)
+      d.set_uncertainty_threshold(em.rows[0, :, :self.S], em.rows[0, :, self.S:self.S + self.A], cutoff, masks=threshold_masks)  # train.py:127
     else:
       first = torch.arange(B, dtype=torch.int32, device=self.device).unsqueeze(0).expand(self.R, -1).contiguous() % n
       self.expert_memory.gather(first, out=self.expert_batch)

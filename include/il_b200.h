@@ -257,9 +257,15 @@ int il_mix_expert_rows(il_handle* h, const il_batch* batch, const il_batch* expe
 
 /* RewardRelabeller.resample_and_relabel (models.py:297-318): AdRIL (update_freq > 0) / SQIL (update_freq == 0) batch construction and reward
  * labels. balanced != 0: the batch becomes the expert batch on calls where *sample_expert_flag != 0 and stays the policy batch otherwise; the
- * flag (device scalar, initially 1) is toggled by the call. Otherwise the first B / 2 rows become expert rows. step = step_f[r] + step_offset. */
+ * flag (device scalar, initially 1) is toggled by the call. Otherwise the first B / 2 rows become expert rows. step = step_f[r] + step_offset.
+ * Per-replica values (sweeps): update_freq_r / balanced_r, int32 [R] device arrays, NULL = the scalar for every replica. Replica r then
+ * runs as a uniform call with update_freq_r[r] and balanced_r[r]. With the arrays the scalars stay host-known for the checks and the launches
+ * (graph capture): balanced = 1 when any replica is balanced (the flag is toggled and the expert batch must hold B rows), update_freq =
+ * the largest value (> 0: the step and trajectory counters are needed). The flag stays one scalar: every replica calls the relabeller at the
+ * same steps, so the balanced replicas alternate in lock-step and the others never read it. */
 int il_adril_relabel(il_handle* h, const il_batch* batch, const il_batch* expert, int R, int balanced, int update_freq, int32_t* sample_expert_flag,
-                     const float* step_f, float step_offset, const int32_t* num_trajectories, int trajectories_shared, int num_expert_trajectories, void* stream);
+                     const float* step_f, float step_offset, const int32_t* num_trajectories, int trajectories_shared, int num_expert_trajectories, void* stream,
+                     const int32_t* update_freq_r, const int32_t* balanced_r);
 
 /* ---- GAILDiscriminator (models.py:152-180), depth-1 `g` network, optional spectral norm ------------------- */
 typedef struct il_gail {
@@ -379,6 +385,11 @@ typedef struct il_pwil {
   int32_t  N, d, S, A;
   int32_t  state_only, time_horizon;
   float    reward_scale, reward_bandwidth;
+  /* Per-replica scales (sweeps): float32 [R] device arrays, NULL = the scalar fields for every replica. Each value is rounded once from
+   * the double the scalar path computes (reward_bandwidth_scale * time_horizon / sqrt(d), models.py:222); il_pwil_reward reads replica r's
+   * pair once per CTA, so its reward is bitwise that of a uniform call with these scalars. */
+  const float* reward_scale_r;
+  const float* reward_bandwidth_r;
 } il_pwil;
 int il_pwil_reset(il_handle* h, const il_pwil* p, int R, const int32_t* mask, void* stream);   /* models.py:228-230 */
 int il_pwil_reward(il_handle* h, const il_pwil* p, int R, const float* state, const float* action, float* reward,
