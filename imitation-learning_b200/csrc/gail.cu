@@ -1144,7 +1144,9 @@ int gail_update_plan(il_handle* h, const il_gail_update_args* a, const WidthClas
   p.order = wc.order;
   pl->blocks = wc.blocks;
   const int tiled_tiles = (p.g.H / 4) * ((p.g.d + 3) / 4);
-  if (h->gail_tiled && p.g.d <= 32 && (p.g.H == 32 || p.g.H == 64 || p.g.H == 128) && a->policy.B % 4 == 0 && tiled_tiles <= 256 && p.g.row % 4 == 0) {
+  bool tiled = h->gail_tiled && p.g.d <= 32 && (p.g.H == 32 || p.g.H == 64 || p.g.H == 128) && a->policy.B % 4 == 0 && tiled_tiles <= 256 && p.g.row % 4 == 0;
+  int64_t tsm = 0;
+  if (tiled) {
     GailTiledParams& tp = pl->tp;
     tp.a = *a;
     TDims& t = tp.g;
@@ -1152,12 +1154,14 @@ int gail_update_plan(il_handle* h, const il_gail_update_args* a, const WidthClas
     t.RB = a->policy.B < 128 ? (a->policy.B + 15) / 16 * 16 : 128;  // multiple of 16: the tile loops (H / 4 x RB / 4 tiles) have warp-uniform trip counts
     tp.off_w1 = off[0]; tp.off_b1 = off[1]; tp.off_w2 = off[2]; tp.off_b2 = off[3];
     tp.order = wc.order;
-    int64_t tsm = tiled_carve(t, nullptr, nullptr);
+    tsm = tiled_carve(t, nullptr, nullptr);
     while (tsm > 110 * 1024 && t.RB > 32) {  // wider nets: shorter row chunks keep two CTAs per SM
       t.RB /= 2;
       tsm = tiled_carve(t, nullptr, nullptr);
     }
-    IL_CHECK(tsm <= 110 * 1024, "il_gail_update: tiled kernel shared memory %lld", (long long)tsm);
+    tiled = tsm <= 110 * 1024;  // H = 128 with d = 29..32 needs more even at 32-row chunks: the untiled kernel runs it
+  }
+  if (tiled) {
     pl->kernel = tiled_tiles <= 64 ? 0 : (tiled_tiles <= 128 ? 1 : 2);
     pl->smem = tsm;
     return 0;
@@ -1221,6 +1225,8 @@ extern "C" int il_gail_update(il_handle* h, const il_gail_update_args* a, void* 
   IL_CHECK(a->opt.m && a->opt.v && a->opt.step, "il_gail_update: null optimiser state");
   IL_CHECK(a->loss_function >= 0 && a->loss_function <= 2, "il_gail_update: bad loss function %d", a->loss_function);
   IL_CHECK(!((a->grad_penalty > 0.f || a->grad_penalty_r) && !a->eps_gp), "il_gail_update: grad_penalty > 0 (or grad_penalty_r) needs eps_gp");
+  IL_CHECK(!((a->grad_penalty > 0.f || a->grad_penalty_r) && a->disc.state_only),
+           "il_gail_update: grad_penalty with a state-only discriminator is undefined in the reference (autograd.grad on the unused action, training.py:125)");
   IL_CHECK(!(a->opt.lr_r || a->opt.weight_decay_r) || a->opt.replica_floats == a->disc.g.stride, "il_gail_update: opt.replica_floats must be the discriminator stride");
   // with loss_function_r the scalar is unused and the caller passes eps_mix when any replica is Mixup (the host cannot read the array)
   IL_CHECK(!(!a->loss_function_r && a->loss_function == IL_LOSS_MIXUP && !a->eps_mix), "il_gail_update: Mixup needs eps_mix");
