@@ -6,31 +6,38 @@
 //                      accuracy (error ~2^-21 per product, the dropped lo*lo term) at 3 MMAs per product ("3xTF32").
 //     IL_GEMM_TF32   : hi*hi only (10-bit mantissa operands).
 //
-// Structure: persistent CTAs of two warpgroups, one per SM, each walking the 128 x 256 output tiles blockIdx.x,
-// blockIdx.x + gridDim.x, ... (the two M-tiles of a group run in the same wave, so the second read of B hits L2).
-// Warpgroup w owns rows [64 w, 64 w + 64) of the tile as the 128 fp32 accumulator registers per thread of
-// wgmma.mma_async m64n256k8.tf32. wgmma reads 32-bit operands from shared memory in K-major layout only, and every
-// operand needs the hi/lo split (a CUDA-core pass) anyway, so each k-block (16 floats of k) takes three steps, all
-// running at once on different k-blocks of the CTA's continuous k-block stream (it runs on across tile boundaries):
-//   1. copy: cp.async 16-byte copies of the raw fp32 chunks global -> a RAW_STAGES-deep shared-memory ring, no
-//      registers held; k-blocks q + 2 .. q + 1 + RAW_STAGES are in flight while k-block q is multiplied;
-//   2. split: each thread reads back exactly the chunks it copied (so cp.async.wait_group is all the visibility it
-//      needs), splits them and stores the hi and lo tiles into one of three hi/lo stages in the canonical K-major
-//      SWIZZLE_64B layout. Operands stored [K, rows] in global memory are transposed on the way: a thread splits a
-//      4 (k) x 4 (rows) block and stores four 16-byte k-chunks, in a per-thread rotated order that keeps the
-//      shared-memory stores conflict-free;
-//   3. multiply: the 6 (3xTF32) or 2 (TF32) wgmmas of the k-block per warpgroup.
-// Per k-block q: issue the wgmmas of q, split q + 1, issue the copy of q + 1 + RAW_STAGES, wgmma.wait_group 1 (the
-// wgmmas of q - 1 are done) and one CTA barrier. The wgmmas of q keep running across that barrier, and with three hi/lo
-// stages the split of q + 1 only overwrites the stage of q - 2, so the tensor pipe does not drain inside a tile.
+// Structure: persistent CTAs, one per SM, each walking the 128 x 256 output tiles blockIdx.x, blockIdx.x + gridDim.x, ...
+// (the two M-tiles of a group run in the same wave, so the second read of B hits L2). The CTA is warp-specialised:
+//   - warpgroup 0, the producer (56 registers per thread after setmaxnreg.dec; 72 with FUSE), copies and splits;
+//   - warpgroups 1 and 2, the consumers (224 registers after setmaxnreg.inc; 216 with FUSE), only multiply and run the
+//     epilogue. Consumer w owns rows [64 w, 64 w + 64) of the tile as the 128 fp32 accumulator registers per thread of
+//     wgmma.mma_async m64n256k8.tf32.
+// wgmma reads 32-bit operands from shared memory in K-major layout only, and every operand needs the hi/lo split (a
+// CUDA-core pass) anyway, so each k-block (16 floats of k) of the CTA's k-block stream (which runs on across tile
+// boundaries) goes through three steps, all running at once on different k-blocks:
+//   1. copy (producer): cp.async 16-byte copies of the raw fp32 chunks global -> a RAW_STAGES-deep shared-memory ring,
+//      no registers held. Each producer thread reads back exactly the chunks it copied, so cp.async.wait_group is all
+//      the visibility the raw ring needs: no mbarrier (cp.async.mbarrier.arrive) and no TMA, which could not feed the
+//      tensor core anyway because the split has to see every element;
+//   2. split (producer): the hi and lo tiles go into one of three hi/lo stages in the canonical K-major SWIZZLE_64B
+//      layout. Operands stored [K, rows] in global memory are transposed on the way: a thread splits a 4 (k) x 4 (rows)
+//      block and stores four 16-byte k-chunks, in a per-thread rotated order that keeps the shared-memory stores
+//      conflict-free. With FUSE the A chunks are computed (the first MLP layer) instead of copied;
+//   3. multiply (consumers): the 6 (3xTF32) or 2 (TF32) wgmmas of the k-block per consumer warpgroup.
+// The stages hand over through full / empty mbarrier pairs with phase bits; the k loop has no CTA barrier. The producer
+// waits for stage q % 3 to be empty, splits k-block q into it, fences the generic-proxy stores to the async proxy and
+// arrives on its full barrier. A consumer waits for the full barrier, issues the wgmmas of q, wgmma.wait_group 1 (the
+// wgmmas of q - 1 are done) and arrives on the empty barrier of q - 1's stage. The producer runs up to three k-blocks
+// ahead, so while the consumers run a tile's epilogue it splits the next tile's first k-blocks.
 // The epilogue works on the accumulator fragments in registers (bias / activation / activation-derivative mask /
 // fused final linear layer, reduced over the four lanes that share a row) and stores 8-byte pairs; the four lanes of a
-// row fill one 32-byte sector. The copies of the next tile's first k-blocks are in flight while it runs.
-// TMA is not used because the tensor core cannot consume the raw tile: the split pass has to see every element.
+// row fill one 32-byte sector. The fused-head bias and weights are staged by the consumers behind a named barrier of
+// their 256 threads.
 // The k loop never writes the accumulators outside wgmma (they are zeroed before it and read after it), so ptxas adds no
 // wgmma wait of its own and the loop's only wait is wait_group 1.
-// Measured on an H100 80GB HBM3 (SXM, 700 W, 1980 MHz): 3xTF32 256 x 256 x 256 with G = 2048 takes 0.88-0.91 ms per
-// layout (0.48 ms floor at data-sheet rates; the two-stage loop this replaced took 1.04-1.10 ms). See DESIGN.md §3.
+// Measured on an H100 80GB HBM3 (SXM, 700 W, 1980 MHz): 3xTF32 256 x 256 x 256 with G = 2048 takes 0.82-0.86 ms per
+// layout (0.48 ms floor at data-sheet rates; the single-role loop this replaced, with a CTA barrier per k-block, took
+// 0.88-0.91 ms). See DESIGN.md §3.
 #include "common.cuh"
 #include <cstdio>
 #include <cstdlib>
@@ -38,11 +45,20 @@
 namespace {
 
 constexpr int BM = 128, BN = 256, BK = 16;        // tile: 128 x 256 outputs; k-blocks of 16 floats (64-byte rows, SWIZZLE_64B)
-constexpr int THREADS = 256;                      // two warpgroups
+constexpr int PRODUCER_THREADS = 128, CONSUMER_THREADS = 256;      // warpgroup 0 copies and splits, warpgroups 1 and 2 multiply
+constexpr int THREADS = PRODUCER_THREADS + CONSUMER_THREADS;
+// setmaxnreg: the launch gives every thread 65536 / 384 = 168 registers (rounded down to 8); the producer hands back all
+// but 56 (72 with FUSE, whose first-layer evaluation spills below that) and the consumers take them: 128 x 56 + 256 x 224
+// = 128 x 72 + 256 x 216 = 384 x 168. These are the smallest producer counts without spills (ptxas -v).
+constexpr int LAUNCH_REGS = 168;
+constexpr int producer_regs(bool fuse) { return fuse ? 72 : 56; }
+constexpr int consumer_regs(bool fuse) { return (THREADS * LAUNCH_REGS - PRODUCER_THREADS * producer_regs(fuse)) / CONSUMER_THREADS; }
+static_assert(THREADS * LAUNCH_REGS <= 65536 && consumer_regs(false) % 8 == 0 && consumer_regs(true) % 8 == 0, "tc_gemm: setmaxnreg split");
+constexpr int CONSUMER_BAR = 1, PRODUCER_BAR = 2;                   // named barriers (0 is __syncthreads)
 constexpr int A_BYTES = BM * BK * 4, B_BYTES = BN * BK * 4;          // 8 KB / 16 KB per k-block (hi or lo copy)
 constexpr int A_HI = 0, A_LO = A_BYTES, B_HI = 2 * A_BYTES, B_LO = 2 * A_BYTES + B_BYTES;
 constexpr int STAGE_BYTES = 2 * (A_BYTES + B_BYTES);                 // 48 KB hi/lo stage
-constexpr int N_STAGES = 3;                                          // hi/lo stages: split q + 1 while the wgmmas of q (and the tail of q - 1) read the other two
+constexpr int N_STAGES = 3;                                          // hi/lo stages: the producer splits up to two k-blocks ahead of the wgmmas in flight
 constexpr int RAW_STAGES = 3;                                        // raw ring: k-blocks in flight global -> shared memory
 constexpr int HEAD_MAX = 8;                                          // fused head: up to 8 output units (N = 1 critic, 2A <= 8 actor)
 constexpr int HEAD_BYTES = (BN + HEAD_MAX * BN) * 4;                 // bias [256] + head weights [8][256]
@@ -57,6 +73,11 @@ constexpr int raw_bytes(bool fuse) { return raw_a_bytes(fuse) + B_BYTES; }
 constexpr int RAW_OFF = N_STAGES * STAGE_BYTES;
 constexpr int head_off(bool fuse) { return RAW_OFF + RAW_STAGES * raw_bytes(fuse); }
 constexpr int l1_off(bool fuse) { return head_off(fuse) + HEAD_BYTES; }
+// The full / empty mbarrier pairs of the hi/lo stages sit in the BAR_BYTES just below the 512-byte aligned base (SWIZZLE_64B
+// repeats every 512 bytes); with dynamic shared memory at least 16-byte aligned, barriers plus alignment take at most
+// BAR_BYTES + 496 <= 1024 bytes.
+constexpr int BAR_BYTES = 64;
+static_assert(2 * N_STAGES * 8 <= BAR_BYTES && BAR_BYTES + 512 - 16 <= 1024, "tc_gemm: mbarrier area");
 constexpr int smem_bytes(bool fuse) { return 1024 + l1_off(fuse) + (fuse ? L1_W_BYTES + L1_B_BYTES + L1_X_BYTES : 0); }  // the first-layer staging only where it is used
 static_assert(smem_bytes(false) <= 227 * 1024 && smem_bytes(true) <= 227 * 1024, "tc_gemm: shared memory over the 227 KB per-CTA limit");
 
@@ -71,6 +92,21 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const float* src) { asm
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
+// returns once the phase of parity `parity` has completed (the phase before the first counts as completed with parity 1)
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  asm volatile(
+      "{\n .reg .pred p;\n"
+      "WAIT:\n mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+      " @!p bra WAIT;\n}" ::"r"(bar), "r"(parity) : "memory");
+}
+template <int ID, int N>
+__device__ __forceinline__ void named_bar_sync() { asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(N) : "memory"); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 // D (64 x 256, fp32, 128 registers per thread) += A (64 x 8, K-major in shared memory) * B (8 x 256, K-major in shared memory)
 __device__ __forceinline__ void wgmma_tf32(float (&d)[128], uint64_t a_desc, uint64_t b_desc) {
   asm volatile(
@@ -160,9 +196,10 @@ struct TcParams {
 template <int EPI, bool FUSE = false>
 __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + BAR_BYTES + 511) & ~(uintptr_t)511);
   float* head_s = reinterpret_cast<float*>(smem + head_off(FUSE));  // [BN] bias then [HEAD_MAX][BN] head weights
   const uint32_t stage0 = smem_u32(smem), raw0 = stage0 + RAW_OFF;
+  const uint32_t full0 = stage0 - BAR_BYTES, empty0 = full0 + N_STAGES * 8;  // mbarriers of hi/lo stage s: full0 + 8 s, empty0 + 8 s
   const uint32_t w1s = stage0 + l1_off(FUSE), b1s = w1s + L1_W_BYTES, xs = b1s + L1_B_BYTES;
   constexpr uint32_t RAW_A = 0, RAW_B = raw_a_bytes(FUSE), RAW_BYTES = raw_bytes(FUSE);
 
@@ -171,141 +208,187 @@ __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
   const int nkb = g.K / BK, tiles_m = p.tiles_m;
   const int my_tiles = (g.G * tiles_m - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;  // tiles blockIdx.x + i gridDim.x
   const int nq = my_tiles * nkb;                                                                // this CTA's k-block stream
-  const bool a_km = FUSE || g.a_kmajor != 0, b_km = g.b_kmajor != 0, split = p.split != 0;
-
-  // ---- per-thread chunks of one k-block ----
-  // stored [rows, K]: 16-byte chunk fc of rows fr + 64 j (A: j < 2, B: j < 4)
-  // stored [K, rows]: 4 x 4 blocks, rows 4 c4 .. 4 c4 + 3 at k = 4 kg .. 4 kg + 3 (A: 128 blocks on the first warpgroup, B: 256 blocks)
-  // A thread's chunk j sits at (j THREADS + tid) * 16 of its operand's region in the raw slot: the copies and the reads back
-  // of a warp are 512 contiguous bytes.
-  const int fr = tid >> 2, fc = tid & 3;
-  const int a_c4 = tid & 31, a_kg = (tid >> 5) & 3, b_c4 = tid & 63, b_kg = tid >> 6;
-  const uint32_t km_off = sw64(fr, fc);  // rows fr + 64 j: + j * 4096 bytes (64 rows = 8 atoms)
   auto tile_of = [&](int i) { return (int)blockIdx.x + i * (int)gridDim.x; };
 
-  auto copy_kb = [&](int q) {  // k-block q of the stream: raw chunks global -> raw slot q % RAW_STAGES; always one commit group
-    if (q < nq) {
-      const int t = tile_of(q / nkb), kb = q % nkb, grp = t / tiles_m, m0 = (t % tiles_m) * BM;
-      const uint32_t raw = raw0 + (uint32_t)(q % RAW_STAGES) * RAW_BYTES + (uint32_t)tid * 16u;
-      if (!FUSE) {
-        const float* A = g.A + (int64_t)(grp / g.a_gdiv) * g.a_gs;
-        if (a_km) {
-          const float* src = A + (int64_t)(m0 + fr) * g.lda + kb * BK + fc * 4;
-          cp_async16(raw + RAW_A, src);
-          cp_async16(raw + RAW_A + THREADS * 16, src + (int64_t)64 * g.lda);
-        } else if (wg == 0) {
-          const float* src = A + (int64_t)(kb * BK + a_kg * 4) * g.lda + m0 + a_c4 * 4;
+  if (tid == 0) {
 #pragma unroll
-          for (int k = 0; k < 4; ++k) cp_async16(raw + RAW_A + k * (THREADS / 2) * 16, src + (int64_t)k * g.lda);
-        }
-      }
-      const float* Bg = g.B + (int64_t)(grp / g.b_gdiv) * g.b_gs;
-      const float* src = b_km ? Bg + (int64_t)fr * g.ldb + kb * BK + fc * 4 : Bg + (int64_t)(kb * BK + b_kg * 4) * g.ldb + b_c4 * 4;
-      const int64_t step = b_km ? (int64_t)64 * g.ldb : (int64_t)g.ldb;  // next chunk j: 64 rows further / the next k
-#pragma unroll
-      for (int j = 0; j < 4; ++j) cp_async16(raw + RAW_B + j * THREADS * 16, src + j * step);
+    for (int s = 0; s < N_STAGES; ++s) {
+      mbar_init(full0 + 8 * s, PRODUCER_THREADS);
+      mbar_init(empty0 + 8 * s, CONSUMER_THREADS);
     }
-    cp_async_commit();
-  };
-
-  auto split_kb = [&](int q) {  // k-block q: split the raw chunks this thread copied (FUSE: compute the A chunks) into hi/lo stage q % N_STAGES
-    const uint32_t st = stage0 + (uint32_t)(q % N_STAGES) * STAGE_BYTES;
-    const uint32_t raw = raw0 + (uint32_t)(q % RAW_STAGES) * RAW_BYTES + (uint32_t)tid * 16u;
-    if (FUSE) {
-      // A chunk values: relu(b1[k] + sum_j x[j] W1[k][j]) for k = 16 kb + 4 fc + {0..3}, rows fr and fr + 64
-      const int kb = q % nkb, k0 = kb * BK + fc * 4;
-      const uint4 bq = lds128(b1s + (uint32_t)k0 * 4u);
-      float c0[4] = {__uint_as_float(bq.x), __uint_as_float(bq.y), __uint_as_float(bq.z), __uint_as_float(bq.w)};
-      float c1[4] = {c0[0], c0[1], c0[2], c0[3]};
-      const int np = (p.l1.x_k + 3) >> 2;
-#pragma unroll
-      for (int c4 = 0; c4 < L1_MAXK / 4; ++c4) {
-        if (c4 < np) {
-          const uint4 x0 = lds128(xs + sw64(fr, c4)), x1 = lds128(xs + sw64(fr + 64, c4));
-#pragma unroll
-          for (int qq = 0; qq < 4; ++qq) {
-            const uint4 w = lds128(w1s + (uint32_t)((k0 + qq) * 64 + ((c4 ^ fc) << 4)));  // W1 row k: chunk c4 at c4 ^ ((k >> 2) & 3)
-            c0[qq] = fmaf(__uint_as_float(x0.x), __uint_as_float(w.x), c0[qq]); c1[qq] = fmaf(__uint_as_float(x1.x), __uint_as_float(w.x), c1[qq]);
-            c0[qq] = fmaf(__uint_as_float(x0.y), __uint_as_float(w.y), c0[qq]); c1[qq] = fmaf(__uint_as_float(x1.y), __uint_as_float(w.y), c1[qq]);
-            c0[qq] = fmaf(__uint_as_float(x0.z), __uint_as_float(w.z), c0[qq]); c1[qq] = fmaf(__uint_as_float(x1.z), __uint_as_float(w.z), c1[qq]);
-            c0[qq] = fmaf(__uint_as_float(x0.w), __uint_as_float(w.w), c0[qq]); c1[qq] = fmaf(__uint_as_float(x1.w), __uint_as_float(w.w), c1[qq]);
-          }
-        }
-      }
-      const uint4 a0 = make_uint4(__float_as_uint(fmaxf(c0[0], 0.f)), __float_as_uint(fmaxf(c0[1], 0.f)), __float_as_uint(fmaxf(c0[2], 0.f)), __float_as_uint(fmaxf(c0[3], 0.f)));
-      const uint4 a1 = make_uint4(__float_as_uint(fmaxf(c1[0], 0.f)), __float_as_uint(fmaxf(c1[1], 0.f)), __float_as_uint(fmaxf(c1[2], 0.f)), __float_as_uint(fmaxf(c1[3], 0.f)));
-      store_chunk(st + A_HI, st + A_LO, km_off, a0, split);
-      store_chunk(st + A_HI, st + A_LO, km_off + 4096u, a1, split);
-      if (p.l1.store) {  // the first hidden activation, for the backward pass
-        const int t = tile_of(q / nkb);
-        float* hs = p.l1.store + (int64_t)(t / tiles_m) * p.l1.store_gs + (int64_t)((t % tiles_m) * BM + fr) * g.K + k0;
-        *reinterpret_cast<uint4*>(hs) = a0;
-        *reinterpret_cast<uint4*>(hs + (int64_t)64 * g.K) = a1;
-      }
-    } else if (a_km) {
-      store_chunk(st + A_HI, st + A_LO, km_off, lds128(raw + RAW_A), split);
-      store_chunk(st + A_HI, st + A_LO, km_off + 4096u, lds128(raw + RAW_A + THREADS * 16), split);
-    } else if (wg == 0) {
-      uint4 v[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) v[k] = lds128(raw + RAW_A + k * (THREADS / 2) * 16);
-      store_block_t(st + A_HI, st + A_LO, a_c4, a_kg, v, split);
-    }
-    if (b_km) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) store_chunk(st + B_HI, st + B_LO, km_off + (uint32_t)j * 4096u, lds128(raw + RAW_B + j * THREADS * 16), split);
-    } else {
-      uint4 v[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) v[k] = lds128(raw + RAW_B + k * THREADS * 16);
-      store_block_t(st + B_HI, st + B_LO, b_c4, b_kg, v, split);
-    }
-  };
-
-  auto stage_l1 = [&](int t) {  // FUSE: first-layer parameters and input rows of tile t (its split must not have started)
-    const int grp = t / tiles_m, m0 = (t % tiles_m) * BM, xk = p.l1.x_k;
-    const float* w1 = p.l1.w1 + (int64_t)grp * p.l1.gs;
-    const float* b1 = p.l1.b1 + (int64_t)grp * p.l1.gs;
-    const float* x = p.l1.x + (int64_t)(grp / p.l1.x_gdiv) * p.l1.x_gs + (int64_t)m0 * p.l1.x_ld;
-    float* w1f = reinterpret_cast<float*>(smem + l1_off(FUSE));
-    float* b1f = reinterpret_cast<float*>(smem + l1_off(FUSE) + L1_W_BYTES);
-    float* xf = reinterpret_cast<float*>(smem + l1_off(FUSE) + L1_W_BYTES + L1_B_BYTES);
-    for (int i = tid; i < L1_ROWS * L1_MAXK; i += THREADS) {  // zero-padded to [256][16]
-      const int k = i / L1_MAXK, j = i % L1_MAXK;
-      w1f[k * L1_MAXK + ((((j >> 2) ^ ((k >> 2) & 3)) << 2) | (j & 3))] = (k < g.K && j < xk) ? __ldg(w1 + (int64_t)k * xk + j) : 0.f;
-    }
-    for (int i = tid; i < L1_ROWS; i += THREADS) b1f[i] = i < g.K ? __ldg(b1 + i) : 0.f;
-    for (int i = tid; i < BM * L1_MAXK; i += THREADS) {
-      const int r = i / L1_MAXK, j = i % L1_MAXK;
-      xf[(sw64(r, j >> 2) >> 2) + (j & 3)] = j < xk ? __ldg(x + (int64_t)r * p.l1.x_ld + j) : 0.f;
-    }
-  };
-
-  // ---- prologue: fill the raw ring, split k-block 0 ----
-#pragma unroll 1
-  for (int q = 0; q < RAW_STAGES; ++q) copy_kb(q);
-  if (FUSE) {
-    stage_l1(tile_of(0));
-    __syncthreads();
   }
-  cp_async_wait<RAW_STAGES - 1>();
-  split_kb(0);
-  copy_kb(RAW_STAGES);
-  fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
-  __syncthreads();
-  const uint64_t a_desc0 = make_desc(stage0 + (uint32_t)wg * 4096u), b_desc0 = make_desc(stage0);  // this warpgroup's 64 rows of A
+  __syncthreads();  // the only CTA-wide barrier: the mbarriers are initialised
 
-  // ---- tiles blockIdx.x + i gridDim.x; the k-block stream q = i nkb + kb runs on across them ----
-  // The k loop never writes the accumulators outside wgmma (they are zeroed before it and read after it), so nothing in
-  // it makes ptxas wait for the wgmmas in flight: those of k-block q run on across the barrier of step q.
-  float acc[128];
+  if (wg == 0) {
+    // ================= producer warpgroup: copy and split the k-block stream =================
+    setmaxnreg_dec<producer_regs(FUSE)>();
+    const bool a_km = FUSE || g.a_kmajor != 0, b_km = g.b_kmajor != 0, split = p.split != 0;
+    // Per-thread chunks of one k-block, in a map of 256 slots: producer thread pt works slots v = pt and v = pt + 128.
+    // stored [rows, K]: 16-byte chunk fc of rows fr + 64 j (A: j < 2, B: j < 4), fr = v / 4, fc = v % 4
+    // stored [K, rows]: 4 x 4 blocks, rows 4 c4 .. 4 c4 + 3 at k = 4 kg .. 4 kg + 3 (A: 128 blocks in slots v < 128, B: 256 blocks)
+    // Slot v's chunk j sits at (256 j + v) * 16 of its operand's region in the raw slot: the copies and the reads back of a
+    // warp are 512 contiguous bytes. A thread reads back exactly the chunks it copied, so cp.async.wait_group is all the
+    // visibility the raw ring needs (no mbarrier, no barrier of the warpgroup).
+    constexpr int MAP = 2 * PRODUCER_THREADS;
+    const int pt = tid;
+
+    auto copy_kb = [&](int q) {  // k-block q of the stream: raw chunks global -> raw slot q % RAW_STAGES; always one commit group
+      if (q < nq) {
+        const int t = tile_of(q / nkb), kb = q % nkb, grp = t / tiles_m, m0 = (t % tiles_m) * BM;
+        const float* A = g.A + (int64_t)(grp / g.a_gdiv) * g.a_gs;
+        const float* Bg = g.B + (int64_t)(grp / g.b_gdiv) * g.b_gs;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int v = pt + h * PRODUCER_THREADS, fr = v >> 2, fc = v & 3;
+          const uint32_t raw = raw0 + (uint32_t)(q % RAW_STAGES) * RAW_BYTES + (uint32_t)v * 16u;
+          if (!FUSE) {
+            if (a_km) {
+              const float* src = A + (int64_t)(m0 + fr) * g.lda + kb * BK + fc * 4;
+              cp_async16(raw + RAW_A, src);
+              cp_async16(raw + RAW_A + MAP * 16, src + (int64_t)64 * g.lda);
+            } else if (h == 0) {
+              const float* src = A + (int64_t)(kb * BK + ((v >> 5) & 3) * 4) * g.lda + m0 + (v & 31) * 4;
+#pragma unroll
+              for (int k = 0; k < 4; ++k) cp_async16(raw + RAW_A + k * (MAP / 2) * 16, src + (int64_t)k * g.lda);
+            }
+          }
+          const float* src = b_km ? Bg + (int64_t)fr * g.ldb + kb * BK + fc * 4 : Bg + (int64_t)(kb * BK + (v >> 6) * 4) * g.ldb + (v & 63) * 4;
+          const int64_t step = b_km ? (int64_t)64 * g.ldb : (int64_t)g.ldb;  // next chunk j: 64 rows further / the next k
+#pragma unroll
+          for (int j = 0; j < 4; ++j) cp_async16(raw + RAW_B + j * MAP * 16, src + j * step);
+        }
+      }
+      cp_async_commit();
+    };
+
+    auto split_kb = [&](int q, int s) {  // k-block q: split the raw chunks this thread copied (FUSE: compute the A chunks) into hi/lo stage s
+      const uint32_t st = stage0 + (uint32_t)s * STAGE_BYTES;
+#pragma unroll(FUSE ? 1 : 2)  // the first-layer evaluation of both slots at once would not fit the producer's registers
+      for (int h = 0; h < 2; ++h) {
+        const int v = pt + h * PRODUCER_THREADS, fr = v >> 2, fc = v & 3;
+        const uint32_t raw = raw0 + (uint32_t)(q % RAW_STAGES) * RAW_BYTES + (uint32_t)v * 16u;
+        const uint32_t km_off = sw64(fr, fc);  // rows fr + 64 j: + j * 4096 bytes (64 rows = 8 atoms)
+        if (FUSE) {
+          // A chunk values: relu(b1[k] + sum_j x[j] W1[k][j]) for k = 16 kb + 4 fc + {0..3}, rows fr and fr + 64
+          const int kb = q % nkb, k0 = kb * BK + fc * 4;
+          const uint4 bq = lds128(b1s + (uint32_t)k0 * 4u);
+          float c0[4] = {__uint_as_float(bq.x), __uint_as_float(bq.y), __uint_as_float(bq.z), __uint_as_float(bq.w)};
+          float c1[4] = {c0[0], c0[1], c0[2], c0[3]};
+          const int np = (p.l1.x_k + 3) >> 2;
+#pragma unroll
+          for (int c4 = 0; c4 < L1_MAXK / 4; ++c4) {
+            if (c4 < np) {
+              const uint4 x0 = lds128(xs + sw64(fr, c4)), x1 = lds128(xs + sw64(fr + 64, c4));
+#pragma unroll
+              for (int qq = 0; qq < 4; ++qq) {
+                const uint4 w = lds128(w1s + (uint32_t)((k0 + qq) * 64 + ((c4 ^ fc) << 4)));  // W1 row k: chunk c4 at c4 ^ ((k >> 2) & 3)
+                c0[qq] = fmaf(__uint_as_float(x0.x), __uint_as_float(w.x), c0[qq]); c1[qq] = fmaf(__uint_as_float(x1.x), __uint_as_float(w.x), c1[qq]);
+                c0[qq] = fmaf(__uint_as_float(x0.y), __uint_as_float(w.y), c0[qq]); c1[qq] = fmaf(__uint_as_float(x1.y), __uint_as_float(w.y), c1[qq]);
+                c0[qq] = fmaf(__uint_as_float(x0.z), __uint_as_float(w.z), c0[qq]); c1[qq] = fmaf(__uint_as_float(x1.z), __uint_as_float(w.z), c1[qq]);
+                c0[qq] = fmaf(__uint_as_float(x0.w), __uint_as_float(w.w), c0[qq]); c1[qq] = fmaf(__uint_as_float(x1.w), __uint_as_float(w.w), c1[qq]);
+              }
+            }
+          }
+          const uint4 a0 = make_uint4(__float_as_uint(fmaxf(c0[0], 0.f)), __float_as_uint(fmaxf(c0[1], 0.f)), __float_as_uint(fmaxf(c0[2], 0.f)), __float_as_uint(fmaxf(c0[3], 0.f)));
+          const uint4 a1 = make_uint4(__float_as_uint(fmaxf(c1[0], 0.f)), __float_as_uint(fmaxf(c1[1], 0.f)), __float_as_uint(fmaxf(c1[2], 0.f)), __float_as_uint(fmaxf(c1[3], 0.f)));
+          store_chunk(st + A_HI, st + A_LO, km_off, a0, split);
+          store_chunk(st + A_HI, st + A_LO, km_off + 4096u, a1, split);
+          if (p.l1.store) {  // the first hidden activation, for the backward pass
+            const int t = tile_of(q / nkb);
+            float* hs = p.l1.store + (int64_t)(t / tiles_m) * p.l1.store_gs + (int64_t)((t % tiles_m) * BM + fr) * g.K + k0;
+            *reinterpret_cast<uint4*>(hs) = a0;
+            *reinterpret_cast<uint4*>(hs + (int64_t)64 * g.K) = a1;
+          }
+        } else if (a_km) {
+          store_chunk(st + A_HI, st + A_LO, km_off, lds128(raw + RAW_A), split);
+          store_chunk(st + A_HI, st + A_LO, km_off + 4096u, lds128(raw + RAW_A + MAP * 16), split);
+        } else if (h == 0) {
+          uint4 va[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) va[k] = lds128(raw + RAW_A + k * (MAP / 2) * 16);
+          store_block_t(st + A_HI, st + A_LO, v & 31, (v >> 5) & 3, va, split);
+        }
+        if (b_km) {
+#pragma unroll
+          for (int j = 0; j < 4; ++j) store_chunk(st + B_HI, st + B_LO, km_off + (uint32_t)j * 4096u, lds128(raw + RAW_B + j * MAP * 16), split);
+        } else {
+          uint4 vb[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) vb[k] = lds128(raw + RAW_B + k * MAP * 16);
+          store_block_t(st + B_HI, st + B_LO, v & 63, v >> 6, vb, split);
+        }
+      }
+    };
+
+    auto stage_l1 = [&](int t) {  // FUSE: first-layer parameters and input rows of tile t
+      const int grp = t / tiles_m, m0 = (t % tiles_m) * BM, xk = p.l1.x_k;
+      const float* w1 = p.l1.w1 + (int64_t)grp * p.l1.gs;
+      const float* b1 = p.l1.b1 + (int64_t)grp * p.l1.gs;
+      const float* x = p.l1.x + (int64_t)(grp / p.l1.x_gdiv) * p.l1.x_gs + (int64_t)m0 * p.l1.x_ld;
+      float* w1f = reinterpret_cast<float*>(smem + l1_off(FUSE));
+      float* b1f = reinterpret_cast<float*>(smem + l1_off(FUSE) + L1_W_BYTES);
+      float* xf = reinterpret_cast<float*>(smem + l1_off(FUSE) + L1_W_BYTES + L1_B_BYTES);
+#pragma unroll 1  // rolled: once per tile, and the producer has few registers
+      for (int i = pt; i < L1_ROWS * L1_MAXK; i += PRODUCER_THREADS) {  // zero-padded to [256][16]
+        const int k = i / L1_MAXK, j = i % L1_MAXK;
+        w1f[k * L1_MAXK + ((((j >> 2) ^ ((k >> 2) & 3)) << 2) | (j & 3))] = (k < g.K && j < xk) ? __ldg(w1 + (int64_t)k * xk + j) : 0.f;
+      }
+      for (int i = pt; i < L1_ROWS; i += PRODUCER_THREADS) b1f[i] = i < g.K ? __ldg(b1 + i) : 0.f;
 #pragma unroll 1
-  for (int i = 0, q = 0; i < my_tiles; ++i) {
+      for (int i = pt; i < BM * L1_MAXK; i += PRODUCER_THREADS) {
+        const int r = i / L1_MAXK, j = i % L1_MAXK;
+        xf[(sw64(r, j >> 2) >> 2) + (j & 3)] = j < xk ? __ldg(x + (int64_t)r * p.l1.x_ld + j) : 0.f;
+      }
+    };
+
+    // Per k-block q: wait until stage s is empty (the consumers' wgmmas of q - N_STAGES are done), wait for this thread's
+    // chunks of q, split them into stage s, mark it full and copy q + RAW_STAGES into the raw slot just read back. The
+    // producer runs up to N_STAGES k-blocks ahead of the wgmmas, across tile boundaries, so the next tile's first stages
+    // are split while the consumers run this tile's epilogue.
+#pragma unroll 1
+    for (int q = 0; q < RAW_STAGES; ++q) copy_kb(q);
+    int s = 0;
+    uint32_t ph = 1;  // parity of the empty phase to wait for: the first pass over the stages finds them empty
+#pragma unroll 1
+    for (int q = 0; q < nq; ++q) {
+      if (FUSE && q % nkb == 0) {  // the first k-block of a tile: its first-layer staging, once every split of the previous tile is done
+        if (q > 0) named_bar_sync<PRODUCER_BAR, PRODUCER_THREADS>();
+        stage_l1(tile_of(q / nkb));
+        named_bar_sync<PRODUCER_BAR, PRODUCER_THREADS>();
+      }
+      mbar_wait(empty0 + 8 * s, ph);
+      cp_async_wait<RAW_STAGES - 1>();  // this thread's chunks of k-block q
+      split_kb(q, s);
+      fence_proxy_async();              // the generic-proxy stores -> visible to the tensor core (async proxy)
+      mbar_arrive(full0 + 8 * s);
+      copy_kb(q + RAW_STAGES);
+      if (++s == N_STAGES) { s = 0; ph ^= 1; }
+    }
+    cp_async_wait<0>();  // the trailing (empty) commit groups
+    return;
+  }
+
+  // ================= consumer warpgroups 1 and 2: wgmma and the epilogue =================
+  // Consumer warpgroup cw owns rows [64 cw, 64 cw + 64) of the tile. Per k-block: wait until its stage is full, issue
+  // the wgmmas, wgmma.wait_group 1 (the wgmmas of the previous k-block are done) and release that previous stage.
+  // The k loop never writes the accumulators outside wgmma (they are zeroed before it and read after it), so nothing in
+  // it makes ptxas wait for the wgmmas in flight.
+  setmaxnreg_inc<consumer_regs(FUSE)>();
+  const int cw = wg - 1, ct = tid - PRODUCER_THREADS;
+  const uint64_t a_desc0 = make_desc(stage0 + (uint32_t)cw * 4096u), b_desc0 = make_desc(stage0);  // this warpgroup's 64 rows of A
+  const bool split = p.split != 0;
+  float acc[128];
+  int s = 0;
+  uint32_t ph = 0;  // parity of the full phase to wait for
+#pragma unroll 1
+  for (int i = 0; i < my_tiles; ++i) {
 #pragma unroll
     for (int j = 0; j < 128; ++j) acc[j] = 0.f;
+    int prev = 0;
 #pragma unroll 1
-    for (int kb = 0; kb < nkb; ++kb, ++q) {  // step q multiplies k-block q, splits q + 1 and copies q + 1 + RAW_STAGES
-      const uint32_t cur = (uint32_t)(q % N_STAGES) * STAGE_BYTES;
+    for (int kb = 0; kb < nkb; ++kb) {
+      mbar_wait(full0 + 8 * s, ph);
+      const uint32_t cur = (uint32_t)s * STAGE_BYTES;
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < BK / 8; ++kk) {  // per MMA (K = 8 tf32): 32 bytes further inside the swizzled 64-byte rows
@@ -318,33 +401,27 @@ __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
         wgmma_tf32(acc, ah, bh);
       }
       wgmma_commit();
-      if (q + 1 < nq) {
-        if (FUSE && kb == nkb - 1) {  // the next split starts the next tile: its first-layer staging (every split of this tile is done: barrier of step q - 1)
-          stage_l1(tile_of(i + 1));
-          __syncthreads();
-        }
-        cp_async_wait<RAW_STAGES - 1>();  // this thread's chunks of k-block q + 1
-        split_kb(q + 1);                  // into the stage the wgmmas of q - 2 read (done in both warpgroups: wait + barrier of step q - 1)
-      }
-      copy_kb(q + 1 + RAW_STAGES);        // into the raw slot this thread just read back
-      wgmma_wait<1>();                    // the wgmmas of q - 1 are done; those of q keep running across the barrier
-      fence_proxy_async();
-      __syncthreads();
+      wgmma_wait<1>();                               // the wgmmas of the previous k-block are done
+      if (kb > 0) mbar_arrive(empty0 + 8 * prev);   // ... so its stage is free for the producer
+      prev = s;
+      if (++s == N_STAGES) { s = 0; ph ^= 1; }
     }
 
     // ---- epilogue of tile i: acc[4 c + {0, 1}] = row r0, columns 8 c + 2 (lane % 4) + {0, 1}; acc[4 c + {2, 3}] = row r0 + 8 ----
     const int t = tile_of(i), grp = t / tiles_m, m0 = (t % tiles_m) * BM;
-    if (EPI == 4 || EPI == 6) {  // this tile's fused-head bias / weights, staged while the last wgmmas finish (the previous tile's epilogue
-                                 // finished reading head_s before the barriers of this tile's k loop); BN == THREADS: element tid of each row
+    if (EPI == 4 || EPI == 6) {  // this tile's fused-head bias / weights, staged while the last wgmmas finish, once both consumer
+                                 // warpgroups are done reading the previous tile's; BN == CONSUMER_THREADS: element ct of each row
+      named_bar_sync<CONSUMER_BAR, CONSUMER_THREADS>();
       const float* wsrc = p.head_w + (int64_t)grp * p.head_gs;
-      if (EPI == 4) head_s[tid] = __ldg(g.bias + (int64_t)grp * g.bias_gs + tid);
+      if (EPI == 4) head_s[ct] = __ldg(g.bias + (int64_t)grp * g.bias_gs + ct);
 #pragma unroll
       for (int j = 0; j < HEAD_MAX; ++j)
-        if (j < p.head_n) head_s[BN + j * BN + tid] = __ldg(wsrc + (int64_t)j * p.head_js + (int64_t)tid * p.head_ns);
+        if (j < p.head_n) head_s[BN + j * BN + ct] = __ldg(wsrc + (int64_t)j * p.head_js + (int64_t)ct * p.head_ns);
     }
     wgmma_wait<0>();
-    if (EPI == 4 || EPI == 6) __syncthreads();
-    const int r0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), cl = (lane & 3) * 2;
+    mbar_arrive(empty0 + 8 * prev);
+    if (EPI == 4 || EPI == 6) named_bar_sync<CONSUMER_BAR, CONSUMER_THREADS>();
+    const int r0 = m0 + cw * 64 + (warp & 3) * 16 + (lane >> 2), cl = (lane & 3) * 2;
     float* C = g.C + (int64_t)grp * g.c_gs + (int64_t)r0 * g.ldc + cl;
     const int64_t c8 = (int64_t)8 * g.ldc;
     const float* bias = (EPI == 1 || (EPI == 3 && g.bias)) ? g.bias + (int64_t)grp * g.bias_gs + cl : nullptr;
@@ -428,8 +505,8 @@ __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
       }
     }
   }
-  cp_async_wait<0>();  // the trailing (empty) commit groups
 }
+
 
 // bias gradient for the dW products routed to the tensor-core engine: out[g, n] = sum_b dY[g, b, n]
 __global__ void colsum_kernel(const float* __restrict__ A, int64_t a_gs, int a_gdiv, int lda, int K, int M, float* __restrict__ out, int64_t out_gs) {
