@@ -126,6 +126,9 @@ SIGNATURES = {
   'il_fill_uniform': (C.c_int, [vp, vp, i64, u64, u64, vp, vp]),
   'il_counter_add': (C.c_int, [vp, vp, u64, vp]),
   'il_fill_beta': (C.c_int, [vp, vp, C.c_int, i64, vp, u64, u64, vp, vp]),
+  'il_fill_normal_r': (C.c_int, [vp, vp, C.c_int, i64, vp, u64, vp, vp]),
+  'il_fill_uniform_r': (C.c_int, [vp, vp, C.c_int, i64, vp, u64, vp, vp]),
+  'il_fill_beta_r': (C.c_int, [vp, vp, C.c_int, i64, vp, vp, u64, vp, vp]),
   'il_actor_workspace_bytes': (i64, [P(Mlp), C.c_int, C.c_int]),
   'il_actor_forward': (C.c_int, [vp, P(Mlp), C.c_int, C.c_int, vp, i64, C.c_int, vp, vp, vp, vp, vp, vp, vp, i64, vp]),
   'il_critic_workspace_bytes': (i64, [P(Mlp), C.c_int, C.c_int]),
@@ -139,6 +142,7 @@ SIGNATURES = {
   'il_adam_step_polyak': (C.c_int, [vp, vp, vp, P(Adam), i64, vp, C.c_float, vp]),
   'il_adam_step_polyak_r': (C.c_int, [vp, vp, vp, P(Adam), i64, vp, vp, vp]),
   'il_fill_dropout_mask': (C.c_int, [vp, vp, i64, f32, u64, u64, vp, vp]),
+  'il_fill_dropout_mask_r': (C.c_int, [vp, vp, C.c_int, i64, f32, vp, u64, vp, vp]),
   'il_actor_dropout_workspace_bytes': (i64, [P(Mlp), C.c_int, C.c_int]),
   'il_actor_log_prob_dropout': (C.c_int, [vp, P(Mlp), C.c_int, C.c_int, C.c_int, vp, i64, C.c_int, vp, vp, P(vp), vp, vp, i64, vp]),
   'il_bc_update_dropout': (C.c_int, [vp, P(BcArgs), vp, P(vp), vp]),
@@ -151,6 +155,7 @@ SIGNATURES = {
   'il_replay_wrap_absorbing': (C.c_int, [vp, P(Replay), C.c_int, vp, vp]),
   'il_replay_transfer': (C.c_int, [vp, P(Replay), C.c_int, P(Replay), vp]),
   'il_replay_sample_indices': (C.c_int, [vp, P(Replay), C.c_int, C.c_int, vp, vp, u64, u64, vp, vp]),
+  'il_replay_sample_indices_r': (C.c_int, [vp, P(Replay), C.c_int, C.c_int, vp, vp, vp, u64, vp, vp]),
   'il_replay_gather': (C.c_int, [vp, P(Replay), C.c_int, vp, P(Batch), vp]),
   'il_mix_expert_rows': (C.c_int, [vp, P(Batch), P(Batch), C.c_int, vp]),
   'il_adril_relabel': (C.c_int, [vp, P(Batch), P(Batch), C.c_int, C.c_int, C.c_int, vp, vp, f32, vp, C.c_int, C.c_int, vp, vp, vp]),
@@ -250,6 +255,11 @@ def mask_array(masks):
   arr = (vp * MAX_LAYERS)()
   for i, t in enumerate(masks or []): arr[i] = None if t is None else t.data_ptr()
   return arr
+
+
+def seed_array(seeds, device) -> torch.Tensor:
+  """The [R] uint64 per-replica key array of the il_*_r RNG entries (stored as int64: seeds are below 2**63)."""
+  return torch.tensor([int(s) for s in seeds], dtype=torch.int64, device=device)
 
 
 def ptr(t: Optional[torch.Tensor]) -> Optional[int]:

@@ -109,6 +109,11 @@ UNUSED_KEYS = {'GAIL': ('imitation.discriminator.input_dropout', 'imitation.disc
 # replicas share, so there they stay grouping keys.
 PER_REPLICA_ALGORITHM = {'AdRIL': ('imitation.update_freq', 'imitation.balanced'), 'PWIL': ('imitation.reward_scale', 'imitation.reward_bandwidth_scale'),
                          'DRIL': ('imitation.quantile_cutoff', )}
+# The run's seed: per replica, every random stream of replica r is keyed by its own seed at replica-local indices (Trainer(per_replica={'seed': ...})),
+# so replica r is the single run with that seed. It stays a grouping key where a stream cannot be split per replica: with device_rng false
+# (the host numpy index stream is one per rank), and with imitation.subsample > 1 when the run builds an expert memory (get_dataset draws the
+# subsampling offsets from the seeded numpy stream, and all replicas share that memory).
+PER_REPLICA_SEED = ('seed', )
 _CHOICES = {'imitation.loss_function': ('BCE', 'Mixup', 'PUGAIL'), 'imitation.discriminator.reward_function': ('AIRL', 'FAIRL', 'GAIL')}
 _SWEEP_FUNCTIONS = re.compile(r'^(range|choice|interval|glob|sort|shuffle|tag)\s*\(')
 
@@ -200,9 +205,36 @@ def vectorised_keys(cfg: Config) -> Tuple[str, ...]:
   return keys
 
 
+def per_replica_keys(cfg: Config) -> Tuple[str, ...]:
+  """Every key Trainer(per_replica=...) takes in this configuration: vectorised_keys plus `seed` where it can be per replica (seed_per_replica)."""
+  return vectorised_keys(cfg) + (PER_REPLICA_SEED if seed_per_replica(cfg) else ())
+
+
+def needs_expert_memory(cfg: Config) -> bool:
+  """Whether the run builds the expert memory (train.py:55-61; SAC only for BC pre-training or the BC auxiliary loss)."""
+  return cfg.get('algorithm') != 'SAC' or cfg.bc_pretraining.get('iterations', 0) > 0 or bool(cfg.imitation.get('bc_aux_loss', False))
+
+
+def seed_per_replica(cfg: Config) -> bool:
+  """Whether `seed` can take per-replica values in this configuration (PER_REPLICA_SEED)."""
+  return bool(cfg.get('device_rng', True)) and not (cfg.imitation.get('subsample', 1) > 1 and needs_expert_memory(cfg))
+
+
 def group_jobs(jobs: List[SweepJob], conf_dir: str = CONF_DIR) -> List[SweepGroup]:
-  """Partitions the jobs of a sweep: swept vectorised keys become per-job values, every other swept key separates groups. Groups are
-  ordered by their first job."""
+  """Partitions the jobs of a sweep: swept vectorised keys become per-job values, every other swept key (`seed` included) separates groups.
+  Groups are ordered by their first job. Each group is one program with one seed, replica jR + k initialised from seed + jR + k."""
+  return _partition(jobs, conf_dir, vectorised_keys)
+
+
+def sweep_groups(jobs: List[SweepJob], conf_dir: str = CONF_DIR) -> List[SweepGroup]:
+  """The programs a multirun runs (train.run_sweep): group_jobs' partition with `seed` a per-replica key where seed_per_replica holds, so
+  groups that differ only in their seed are one program whose replicas draw their random numbers by their own seeds (per_replica_keys)."""
+  return _partition(jobs, conf_dir, per_replica_keys)
+
+
+def _partition(jobs: List[SweepJob], conf_dir: str, keys_of) -> List[SweepGroup]:
+  """Jobs that agree on every swept key outside keys_of(config) form one group, in the order of their first job; the swept keys inside it
+  become per-job values."""
   swept = {}
   for j in jobs:
     for o in j.overrides:
@@ -213,13 +245,13 @@ def group_jobs(jobs: List[SweepJob], conf_dir: str = CONF_DIR) -> List[SweepGrou
   for j in jobs:
     ov = dict(o.partition('=')[::2] for o in j.overrides)
     cfg = load_config(j.overrides, conf_dir)
-    vec = set(vectorised_keys(cfg)) | set(UNUSED_KEYS.get(cfg.get('algorithm'), ()))
+    vec = set(keys_of(cfg)) | set(UNUSED_KEYS.get(cfg.get('algorithm'), ()))
     key = tuple((k, ov.get(k)) for k in swept if k not in vec)
     g = groups.setdefault(key, SweepGroup([]))
     g.jobs.append(j)
   for g in groups.values():
     cfgs = [load_config(j.overrides, conf_dir) for j in g.jobs]
-    vec = vectorised_keys(cfgs[0])
+    vec = keys_of(cfgs[0])
     for k in swept:
       if k in vec: g.per_job[k] = [get_key(c, k) for c in cfgs]
     for k in PER_REPLICA_WIDTH: _check_width_classes(k, g.per_job.get(k, []))
@@ -245,9 +277,13 @@ def _check_width_classes(k: str, vals: Sequence[Any]):
 
 
 def _per_replica_value(k: str, x: Any) -> Any:
-  """A per-replica value as the config holds it: a name of _CHOICES[k], a bool for spectral_norm, a positive int for a width, a float otherwise."""
+  """A per-replica value as the config holds it: a name of _CHOICES[k], a bool for spectral_norm, a positive int for a width, a non-negative
+  int for a seed, a float otherwise."""
   if k in PER_REPLICA_WIDTH:
     if isinstance(x, bool) or not isinstance(x, int) or x <= 0: raise SweepError(f'{k}={x!r}: not a positive integer')
+    return x
+  if k in PER_REPLICA_SEED:  # np.random.seed (train.py:51) takes 0 <= seed < 2**32
+    if isinstance(x, bool) or not isinstance(x, int) or not 0 <= x < 2**32: raise SweepError(f'{k}={x!r}: not an integer in [0, 2**32)')
     return x
   if k in _CHOICES:
     if x not in _CHOICES[k]: raise SweepError(f'{k}={x!r}: not one of {", ".join(_CHOICES[k])}')  # train.py:42,44
@@ -257,6 +293,13 @@ def _per_replica_value(k: str, x: Any) -> Any:
     return x
   if isinstance(x, (bool, str)): raise SweepError(f'{k}={x!r}: not a number')
   return float(x)
+
+
+def replica_values(k: str, per_job: Sequence[Any], R: int) -> List[Any]:
+  """The J * R replica values of a group from its J job values: job j's value for each of its R replicas, except a seed, where replica i of
+  job j takes s_j + i (a seed sweep with replicas=R runs each job as the replicas=R run of its seed)."""
+  if k not in PER_REPLICA_SEED: return [v for v in per_job for _ in range(R)]
+  return [_per_replica_value(k, s) + i for s in per_job for i in range(R)]
 
 
 def _algorithm_value(k: str, x: Any, r: int) -> Any:
@@ -286,11 +329,11 @@ def _check_gail_replicas(cfg: Config, arrays: Dict[str, List[Any]], R: int):
 
 def split_per_replica(cfg: Config, per_replica: Optional[Dict[str, Sequence[Any]]], R: int) -> Tuple[Config, Dict[str, List[Any]]]:
   """(config, arrays) for Trainer(per_replica=...): a key whose R values are all equal becomes that scalar in a copy of the config (the
-  uniform path, bit for bit); the others stay per-replica lists. Keys outside vectorised_keys(cfg) and values the reference's asserts refuse
+  uniform path, bit for bit); the others stay per-replica lists. Keys outside per_replica_keys(cfg) and values the reference's asserts refuse
   (train.py:37-49, per replica) are refused."""
   cfg = copy.deepcopy(cfg)
   arrays = {}
-  allowed = vectorised_keys(cfg)
+  allowed = per_replica_keys(cfg)
   for k, vals in (per_replica or {}).items():
     if k not in allowed: raise SweepError(f'{k} cannot take per-replica values in this configuration (per-replica keys: {", ".join(allowed)})')
     per_alg = k in PER_REPLICA_ALGORITHM.get(cfg.get('algorithm'), ())

@@ -134,9 +134,13 @@ extern "C" int il_row_layout(int S, int A, int32_t* off, int32_t* row_len) {
 
 namespace {
 
-// 4 outputs per Philox call; element i uses counter (base + i / 4), lane i % 4.
-__global__ void fill_kernel(float* __restrict__ out, int64_t n, uint64_t seed, uint64_t stream_id, const uint64_t* __restrict__ counter, int normal) {
+// 4 outputs per Philox call; element i uses counter (base + i / 4), lane i % 4. seed_r (per-replica keys): blockIdx.y is the replica r, n its
+// element count, and replica r draws with key seed_r[r] at local indices into out + r * n, as a call over that replica alone would; NULL =
+// one key `seed` over all n elements (gridDim.y == 1).
+__global__ void fill_kernel(float* __restrict__ out, int64_t n, uint64_t seed, uint64_t stream_id, const uint64_t* __restrict__ counter, int normal,
+                            const uint64_t* __restrict__ seed_r) {
   const uint64_t base = counter ? *counter : 0ull;
+  if (seed_r) { seed = seed_r[blockIdx.y]; out += (int64_t)blockIdx.y * n; }
   const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
   for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q * 4 < n; q += (int64_t)gridDim.x * blockDim.x) {
     const uint64_t c = base + (uint64_t)q;
@@ -177,15 +181,18 @@ __device__ float log_gamma_mt(float a, uint64_t c, uint64_t stream_id, uint32_t 
   return logf(d);
 }
 
-// One thread per element; element i of replica r = i / n uses counter (base + i / 4), lane i % 4 (the il_fill_uniform mapping).
+// One thread per element; element i of replica r = i / n uses counter (base + i / 4), lane i % 4 (the il_fill_uniform mapping). seed_r
+// (per-replica keys): blockIdx.y is the replica r, i runs over its n local elements of out + r * n and the key is seed_r[r]; NULL = one key
+// `seed` over all `total` elements (gridDim.y == 1).
 __global__ void beta_fill_kernel(float* __restrict__ out, int64_t total, int64_t n, const float* __restrict__ alpha_r, uint64_t seed, uint64_t stream_id,
-                                 const uint64_t* __restrict__ counter) {
+                                 const uint64_t* __restrict__ counter, const uint64_t* __restrict__ seed_r) {
   const uint64_t base = counter ? *counter : 0ull;
+  if (seed_r) { seed = seed_r[blockIdx.y]; out += (int64_t)blockIdx.y * n; total = n; }
   const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const uint64_t c = base + (uint64_t)(i >> 2);
     const uint32_t lane = (uint32_t)(i & 3);
-    const float alpha = alpha_r[i / n];
+    const float alpha = alpha_r[seed_r ? (int64_t)blockIdx.y : i / n];
     float v;
     if (alpha == 1.f) {  // Beta(1, 1) = U(0, 1): the il_fill_uniform value
       const uint4 q = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), (uint32_t)stream_id, (uint32_t)(stream_id >> 32)), key);
@@ -210,13 +217,29 @@ __global__ void beta_fill_kernel(float* __restrict__ out, int64_t total, int64_t
 
 __global__ void counter_add_kernel(uint64_t* c, uint64_t inc) { *c += inc; }
 
+// grid.x covers one replica's (or, seed_r == NULL, the whole call's) `units` work items at 256 per block, at most 16 blocks per SM in total
+dim3 rng_grid(il_handle* h, int64_t units, int R) {
+  int64_t blocks = (units + 255) / 256;
+  const int64_t cap = (int64_t)h->sm_count * 16 / R;
+  if (blocks > cap) blocks = cap;
+  if (blocks < 1) blocks = 1;
+  return dim3((unsigned)blocks, (unsigned)R);
+}
+
 int fill(il_handle* h, float* out, int64_t n, uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream, int normal) {
   IL_CHECK(h && out && n >= 0, "il_fill: bad argument");
   if (n == 0) return 0;
   int64_t blocks = (n / 4 + 255) / 256;
   if (blocks > (int64_t)h->sm_count * 16) blocks = (int64_t)h->sm_count * 16;
   if (blocks < 1) blocks = 1;
-  IL_LAUNCH(h, fill_kernel, (unsigned)blocks, 256, 0, (cudaStream_t)stream, out, n, seed, stream_id, counter, normal);
+  IL_LAUNCH(h, fill_kernel, (unsigned)blocks, 256, 0, (cudaStream_t)stream, out, n, seed, stream_id, counter, normal, nullptr);
+  return 0;
+}
+
+int fill_r(il_handle* h, float* out, int R, int64_t n_per_replica, const uint64_t* seed_r, uint64_t stream_id, const uint64_t* counter, void* stream, int normal) {
+  IL_CHECK(h && out && seed_r && R > 0 && R <= IL_MAX_GRID_Y && n_per_replica >= 0, "il_fill_%s_r: bad argument (R = %d)", normal ? "normal" : "uniform", R);
+  if (n_per_replica == 0) return 0;
+  IL_LAUNCH(h, fill_kernel, rng_grid(h, (n_per_replica + 3) / 4, R), 256, 0, (cudaStream_t)stream, out, n_per_replica, 0ull, stream_id, counter, normal, seed_r);
   return 0;
 }
 
@@ -228,6 +251,12 @@ extern "C" int il_fill_normal(il_handle* h, float* out, int64_t n, uint64_t seed
 extern "C" int il_fill_uniform(il_handle* h, float* out, int64_t n, uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream) {
   return fill(h, out, n, seed, stream_id, counter, stream, 0);
 }
+extern "C" int il_fill_normal_r(il_handle* h, float* out, int R, int64_t n_per_replica, const uint64_t* seed_r, uint64_t stream_id, const uint64_t* counter, void* stream) {
+  return fill_r(h, out, R, n_per_replica, seed_r, stream_id, counter, stream, 1);
+}
+extern "C" int il_fill_uniform_r(il_handle* h, float* out, int R, int64_t n_per_replica, const uint64_t* seed_r, uint64_t stream_id, const uint64_t* counter, void* stream) {
+  return fill_r(h, out, R, n_per_replica, seed_r, stream_id, counter, stream, 0);
+}
 extern "C" int il_fill_beta(il_handle* h, float* out, int R, int64_t n_per_replica, const float* alpha_r, uint64_t seed, uint64_t stream_id, const uint64_t* counter,
                             void* stream) {
   IL_CHECK(h && out && alpha_r && R > 0 && n_per_replica >= 0, "il_fill_beta: bad argument");
@@ -235,7 +264,14 @@ extern "C" int il_fill_beta(il_handle* h, float* out, int R, int64_t n_per_repli
   if (total == 0) return 0;
   int64_t blocks = (total + 255) / 256;
   if (blocks > (int64_t)h->sm_count * 16) blocks = (int64_t)h->sm_count * 16;
-  IL_LAUNCH(h, beta_fill_kernel, (unsigned)blocks, 256, 0, (cudaStream_t)stream, out, total, n_per_replica, alpha_r, seed, stream_id, counter);
+  IL_LAUNCH(h, beta_fill_kernel, (unsigned)blocks, 256, 0, (cudaStream_t)stream, out, total, n_per_replica, alpha_r, seed, stream_id, counter, nullptr);
+  return 0;
+}
+extern "C" int il_fill_beta_r(il_handle* h, float* out, int R, int64_t n_per_replica, const float* alpha_r, const uint64_t* seed_r, uint64_t stream_id,
+                              const uint64_t* counter, void* stream) {
+  IL_CHECK(h && out && alpha_r && seed_r && R > 0 && R <= IL_MAX_GRID_Y && n_per_replica >= 0, "il_fill_beta_r: bad argument (R = %d)", R);
+  if (n_per_replica == 0) return 0;
+  IL_LAUNCH(h, beta_fill_kernel, rng_grid(h, n_per_replica, R), 256, 0, (cudaStream_t)stream, out, n_per_replica, n_per_replica, alpha_r, 0ull, stream_id, counter, seed_r);
   return 0;
 }
 extern "C" int il_counter_add(il_handle* h, uint64_t* counter, uint64_t inc, void* stream) {

@@ -9,6 +9,8 @@
 
 #include "../../include/il_b200.h"
 
+#define IL_MAX_GRID_Y 65535  // the per-replica RNG launches put the replica on gridDim.y
+
 struct ProfiledLaunch {
   cudaEvent_t start, stop;
   double flops;

@@ -36,10 +36,13 @@ __global__ void dropout_bwd_kernel(float* __restrict__ t_, const float* __restri
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t < n) t_[t] = t_[t] * act_grad_from_output(y[t], act) * (mask ? mask[t] : 1.f);
 }
-// Bernoulli(1 - p) / (1 - p) from Philox4x32-10
-__global__ void dropout_mask_kernel(float* __restrict__ out, int64_t n, float p, uint64_t seed, uint64_t stream_id, const uint64_t* __restrict__ counter) {
+// Bernoulli(1 - p) / (1 - p) from Philox4x32-10, one thread per quad at counter (*counter + quad). seed_r (per-replica keys): blockIdx.y is the
+// replica r, n its element count, and its quads of out + r * n draw key seed_r[r] at local counters; NULL = one key `seed` over all n.
+__global__ void dropout_mask_kernel(float* __restrict__ out, int64_t n, float p, uint64_t seed, uint64_t stream_id, const uint64_t* __restrict__ counter,
+                                    const uint64_t* __restrict__ seed_r) {
   const int64_t i4 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i4 * 4 >= n) return;
+  if (seed_r) { seed = seed_r[blockIdx.y]; out += (int64_t)blockIdx.y * n; }
   const uint64_t c = (counter ? *counter : 0ull) + (uint64_t)i4;
   const uint4 r = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), (uint32_t)stream_id, (uint32_t)(stream_id >> 32)), make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
   const float keep = 1.f / (1.f - p);
@@ -251,7 +254,15 @@ __global__ void dril_reward_kernel(const float* __restrict__ log_prob, int R, in
 
 extern "C" int il_fill_dropout_mask(il_handle* h, float* out, int64_t n, float p, uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream) {
   IL_CHECK(h && out && n > 0 && p >= 0.f && p < 1.f, "il_fill_dropout_mask: bad argument (p = %f)", (double)p);
-  IL_LAUNCH(h, dropout_mask_kernel, dblocks((n + 3) / 4), 256, 0, (cudaStream_t)stream, out, n, p, seed, stream_id, counter);
+  IL_LAUNCH(h, dropout_mask_kernel, dblocks((n + 3) / 4), 256, 0, (cudaStream_t)stream, out, n, p, seed, stream_id, counter, nullptr);
+  return 0;
+}
+extern "C" int il_fill_dropout_mask_r(il_handle* h, float* out, int R, int64_t n_per_replica, float p, const uint64_t* seed_r, uint64_t stream_id, const uint64_t* counter,
+                                      void* stream) {
+  IL_CHECK(h && out && seed_r && R > 0 && R <= IL_MAX_GRID_Y && n_per_replica > 0 && p >= 0.f && p < 1.f, "il_fill_dropout_mask_r: bad argument (R = %d, p = %f)", R,
+           (double)p);
+  IL_LAUNCH(h, dropout_mask_kernel, dim3(dblocks((n_per_replica + 3) / 4), (unsigned)R), 256, 0, (cudaStream_t)stream, out, n_per_replica, p, 0ull, stream_id, counter,
+            seed_r);
   return 0;
 }
 

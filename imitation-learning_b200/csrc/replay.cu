@@ -80,11 +80,21 @@ __global__ void replay_wrap_kernel(il_replay mem, int R, const int32_t* __restri
 }
 
 // memory.py:51-59: uniform over [0, size) (full) or [0, idx-1) (not full), never the newest row (idx-1) % size.
+// seed_r (per-replica keys): blockIdx.y is the replica r, and its index k of n draws key seed_r[r] at counter (*counter + k), as a call over
+// that replica alone would; NULL = one key `seed`, index i of all R * n at counter (*counter + i).
 __global__ void replay_sample_idx_kernel(il_replay mem, int R, int n, int32_t* __restrict__ out, const float* __restrict__ uniform, uint64_t seed, uint64_t stream_id,
-                                         const uint64_t* __restrict__ counter) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (int64_t)R * n) return;
-  const int r = (int)(i / n);
+                                         const uint64_t* __restrict__ counter, const uint64_t* __restrict__ seed_r) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, k = i;
+  int r;
+  if (seed_r) {
+    if (k >= n) return;
+    r = (int)blockIdx.y;
+    seed = seed_r[r];
+    i = (int64_t)r * n + k;
+  } else {
+    if (i >= (int64_t)R * n) return;
+    r = (int)(i / n);
+  }
   const int mi = mem.shared ? 0 : r;
   const int idx = mem.idx[mi], full = mem.full[mi];
   uint32_t bits;
@@ -92,7 +102,7 @@ __global__ void replay_sample_idx_kernel(il_replay mem, int R, int n, int32_t* _
     const float u = fminf(fmaxf(uniform[i], 0.f), 0.99999994f);
     bits = (uint32_t)(u * 4294967296.f);
   } else {
-    const uint64_t c = (counter ? *counter : 0ull) + (uint64_t)i;
+    const uint64_t c = (counter ? *counter : 0ull) + (uint64_t)k;
     bits = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), (uint32_t)stream_id, (uint32_t)(stream_id >> 32)), make_uint2((uint32_t)seed, (uint32_t)(seed >> 32))).x;
   }
   int j;
@@ -252,7 +262,17 @@ extern "C" int il_replay_sample_indices(il_handle* h, const il_replay* mem, int 
                                         const uint64_t* counter, void* stream) {
   IL_CHECK(h && idx_out && R > 0 && n > 0, "il_replay_sample_indices: bad argument");
   IL_TRY(check_replay(mem, "il_replay_sample_indices"));
-  IL_LAUNCH(h, replay_sample_idx_kernel, (unsigned)(((int64_t)R * n + 255) / 256), 256, 0, (cudaStream_t)stream, *mem, R, n, idx_out, uniform, seed, stream_id, counter);
+  IL_LAUNCH(h, replay_sample_idx_kernel, (unsigned)(((int64_t)R * n + 255) / 256), 256, 0, (cudaStream_t)stream, *mem, R, n, idx_out, uniform, seed, stream_id, counter,
+            nullptr);
+  return 0;
+}
+
+extern "C" int il_replay_sample_indices_r(il_handle* h, const il_replay* mem, int R, int n, int32_t* idx_out, const float* uniform, const uint64_t* seed_r,
+                                          uint64_t stream_id, const uint64_t* counter, void* stream) {
+  IL_CHECK(h && idx_out && seed_r && R > 0 && R <= IL_MAX_GRID_Y && n > 0, "il_replay_sample_indices_r: bad argument (R = %d)", R);
+  IL_TRY(check_replay(mem, "il_replay_sample_indices_r"));
+  IL_LAUNCH(h, replay_sample_idx_kernel, dim3((unsigned)((n + 255) / 256), (unsigned)R), 256, 0, (cudaStream_t)stream, *mem, R, n, idx_out, uniform, 0ull, stream_id,
+            counter, seed_r);
   return 0;
 }
 

@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes as C
 import math
 from types import SimpleNamespace
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -107,14 +107,22 @@ class D4RLEnv:
     self._eval_batches: Dict[int, EnvBatch] = {}
 
   # ---- reference surface ----
-  def seed(self, seed: int) -> List[int]:  # environments.py:42-43
-    self._seed = seed
-    self._gen = torch.Generator().manual_seed(seed)
-    return [seed]
+  def seed(self, seed: Union[int, Sequence[int]]) -> List[int]:  # environments.py:42-43
+    """One seed, or one per replica (seed sweeps): replica r then draws its reset noise from its own generator, as a single-replica env
+    seeded seed[r] does."""
+    if isinstance(seed, int):
+      self._seed, self._gen = seed, torch.Generator().manual_seed(seed)
+      return [seed]
+    assert len(seed) == self.replicas, f'{len(seed)} seeds for {self.replicas} replicas'
+    self._seed, self._gen = list(seed), [torch.Generator().manual_seed(s) for s in seed]
+    return list(seed)
 
   def reset_noise(self, n: int) -> Tensor:
-    """U[0,1) initial-state draws [n, obs] from the env's seeded host generator (the analogue of gym's seeded reset)."""
-    return torch.rand(n, self.obs, generator=self._gen).to(self.device)
+    """U[0,1) initial-state draws [n, obs] from the env's seeded host generator (the analogue of gym's seeded reset). With per-replica seeds,
+    n is replica-major and replica r's n / R rows come from its own generator."""
+    if isinstance(self._gen, torch.Generator): return torch.rand(n, self.obs, generator=self._gen).to(self.device)
+    assert n % self.replicas == 0
+    return torch.cat([torch.rand(n // self.replicas, self.obs, generator=g) for g in self._gen]).to(self.device)
 
   def reset(self, u: Optional[Tensor] = None) -> Tensor:  # environments.py:29-33
     u = self.reset_noise(self.replicas) if u is None else torch.as_tensor(u, dtype=torch.float32).to(self.device).reshape(self.replicas, self.obs).contiguous()

@@ -7,7 +7,7 @@ read. The reference's 8 field tensors are exposed as strided views of that buffe
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Optional, Union
+from typing import Dict, List, Optional, Sequence, Union
 
 import numpy as np
 import torch
@@ -114,6 +114,17 @@ class ReplayMemory:
       self._idx.fill_(n % size)
       self._full.fill_(int(n % size == 0 and n > 0))
 
+  @property
+  def seed(self) -> Union[int, List[int]]:
+    """Key of the device index draws: one key, or R per-replica keys (seed sweeps), with which replica r draws the indices a single-replica
+    memory seeded seed[r] draws (il_replay_sample_indices_r)."""
+    return self._seed
+
+  @seed.setter
+  def seed(self, seed: Union[int, Sequence[int]]):
+    if not isinstance(seed, int): assert len(seed) == self.replicas, f'{len(seed)} seeds for {self.replicas} replicas'
+    self._seed, self._seed_r = (seed, None) if isinstance(seed, int) else (list(seed), _lib.seed_array(seed, self.device))
+
   # ---- reference attributes (host reads synchronise; used by the drop-in path only) ----
   @property
   def idx(self): return int(self._idx[0]) if self._idx.numel() == 1 else self._idx
@@ -212,10 +223,13 @@ class ReplayMemory:
     drawn by numpy on the host like the reference) replaces the device Philox draws."""
     R = self.replicas
     if out is None: out = torch.empty(R, n, dtype=torch.int32, device=self.device)
-    m = self.c_struct()
-    _lib.check(_lib.lib().il_replay_sample_indices(_lib.handle(), C.byref(m), R, n, out.data_ptr(), _lib.ptr(uniform), self.seed, stream_id, self._rng_counter.data_ptr(),
-                                                   _lib.stream()))
-    if uniform is None: _lib.check(_lib.lib().il_counter_add(_lib.handle(), self._rng_counter.data_ptr(), R * n, _lib.stream()))
+    m, lib = self.c_struct(), _lib.lib()
+    if self._seed_r is None:
+      _lib.check(lib.il_replay_sample_indices(_lib.handle(), C.byref(m), R, n, out.data_ptr(), _lib.ptr(uniform), self.seed, stream_id, self._rng_counter.data_ptr(), _lib.stream()))
+    else:
+      _lib.check(lib.il_replay_sample_indices_r(_lib.handle(), C.byref(m), R, n, out.data_ptr(), _lib.ptr(uniform), self._seed_r.data_ptr(), stream_id, self._rng_counter.data_ptr(),
+                                                _lib.stream()))
+    if uniform is None: _lib.check(lib.il_counter_add(_lib.handle(), self._rng_counter.data_ptr(), R * n if self._seed_r is None else n, _lib.stream()))
     return out
 
   def sample(self, n: int, device_rng: bool = False) -> TransitionBatch:

@@ -8,7 +8,7 @@ from __future__ import annotations
 import copy
 import ctypes as C
 from math import sqrt
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 from torch import Tensor
@@ -34,30 +34,46 @@ def _as_rns(x: Tensor, R: int, width: int, device) -> Tensor:
 
 
 class _RNG:
-  """Device noise source (Philox, il_fill_normal / il_fill_uniform) standing in for torch's global RNG draws."""
+  """Device noise source (Philox, il_fill_normal / il_fill_uniform) standing in for torch's global RNG draws.
 
-  def __init__(self, seed: int = 0, device=None):
+  `seed` is one key, or a list of R per-replica keys (seed sweeps): then every draw has a leading replica axis of R, and replica r's slice
+  is what a single-replica source keyed seed[r] draws for that slice alone (il_fill_*_r, local element indices), with the counter advancing
+  by one replica's share."""
+
+  def __init__(self, seed: Union[int, Sequence[int]] = 0, device=None):
     self.seed = seed
     self.counter = None
     self.device = device
+    self.seed_r = None if isinstance(seed, int) else _lib.seed_array(seed, device)
 
   def _ctr(self, device):
     if self.counter is None: self.counter = torch.zeros(1, dtype=torch.int64, device=device)
     return self.counter
 
+  def _per_key(self, out: Tensor) -> int:
+    """Elements one key draws: all of `out`, or one replica's share of it."""
+    if self.seed_r is None: return out.numel()
+    assert out.numel() % self.seed_r.numel() == 0, f'{tuple(out.shape)} does not split over {self.seed_r.numel()} replica keys'
+    return out.numel() // self.seed_r.numel()
+
+  def _advance(self, ctr: Tensor, n: int):
+    _lib.check(_lib.lib().il_counter_add(_lib.handle(), ctr.data_ptr(), (n + 3) // 4, _lib.stream()))
+
+  def _fill(self, out: Tensor, stream_id: int, normal: bool) -> Tensor:
+    lib, ctr, n = _lib.lib(), self._ctr(out.device), self._per_key(out)
+    if self.seed_r is None: _lib.check((lib.il_fill_normal if normal else lib.il_fill_uniform)(_lib.handle(), out.data_ptr(), n, self.seed, stream_id, ctr.data_ptr(), _lib.stream()))
+    else: _lib.check((lib.il_fill_normal_r if normal else lib.il_fill_uniform_r)(_lib.handle(), out.data_ptr(), self.seed_r.numel(), n, self.seed_r.data_ptr(), stream_id, ctr.data_ptr(),
+                                                                                   _lib.stream()))
+    self._advance(ctr, n)
+    return out
+
   def normal(self, shape, device, stream_id: int = 1, out: Optional[Tensor] = None) -> Tensor:
     out = torch.empty(shape, device=device, dtype=torch.float32) if out is None else out
-    ctr = self._ctr(device)
-    _lib.check(_lib.lib().il_fill_normal(_lib.handle(), out.data_ptr(), out.numel(), self.seed, stream_id, ctr.data_ptr(), _lib.stream()))
-    _lib.check(_lib.lib().il_counter_add(_lib.handle(), ctr.data_ptr(), (out.numel() + 3) // 4, _lib.stream()))
-    return out
+    return self._fill(out, stream_id, normal=True)
 
   def uniform(self, shape, device, stream_id: int = 2, out: Optional[Tensor] = None) -> Tensor:
     out = torch.empty(shape, device=device, dtype=torch.float32) if out is None else out
-    ctr = self._ctr(device)
-    _lib.check(_lib.lib().il_fill_uniform(_lib.handle(), out.data_ptr(), out.numel(), self.seed, stream_id, ctr.data_ptr(), _lib.stream()))
-    _lib.check(_lib.lib().il_counter_add(_lib.handle(), ctr.data_ptr(), (out.numel() + 3) // 4, _lib.stream()))
-    return out
+    return self._fill(out, stream_id, normal=False)
 
   def beta(self, shape, alpha_r: Tensor, device, stream_id: int = 2, out: Optional[Tensor] = None) -> Tensor:
     """[R, ...] Beta(alpha_r[r], alpha_r[r]) draws (il_fill_beta); alpha_r is an [R] float32 device tensor. Where alpha is 1 the values are
@@ -65,9 +81,20 @@ class _RNG:
     out = torch.empty(shape, device=device, dtype=torch.float32) if out is None else out
     R = alpha_r.numel()
     assert out.numel() % R == 0 and alpha_r.dtype == torch.float32 and alpha_r.is_cuda
-    ctr = self._ctr(device)
-    _lib.check(_lib.lib().il_fill_beta(_lib.handle(), out.data_ptr(), R, out.numel() // R, alpha_r.data_ptr(), self.seed, stream_id, ctr.data_ptr(), _lib.stream()))
-    _lib.check(_lib.lib().il_counter_add(_lib.handle(), ctr.data_ptr(), (out.numel() + 3) // 4, _lib.stream()))
+    lib, ctr, n = _lib.lib(), self._ctr(device), self._per_key(out)
+    if self.seed_r is None: _lib.check(lib.il_fill_beta(_lib.handle(), out.data_ptr(), R, n // R, alpha_r.data_ptr(), self.seed, stream_id, ctr.data_ptr(), _lib.stream()))
+    else:
+      assert self.seed_r.numel() == R
+      _lib.check(lib.il_fill_beta_r(_lib.handle(), out.data_ptr(), R, n, alpha_r.data_ptr(), self.seed_r.data_ptr(), stream_id, ctr.data_ptr(), _lib.stream()))
+    self._advance(ctr, n)
+    return out
+
+  def dropout_mask(self, out: Tensor, p: float, stream_id: int) -> Tensor:
+    """Bernoulli(1 - p) / (1 - p) draws into `out` (il_fill_dropout_mask), the analogue of nn.Dropout's draws from torch's global stream."""
+    lib, ctr, n = _lib.lib(), self._ctr(out.device), self._per_key(out)
+    if self.seed_r is None: _lib.check(lib.il_fill_dropout_mask(_lib.handle(), out.data_ptr(), n, p, self.seed, stream_id, ctr.data_ptr(), _lib.stream()))
+    else: _lib.check(lib.il_fill_dropout_mask_r(_lib.handle(), out.data_ptr(), self.seed_r.numel(), n, p, self.seed_r.data_ptr(), stream_id, ctr.data_ptr(), _lib.stream()))
+    self._advance(ctr, n)
     return out
 
 
@@ -77,6 +104,13 @@ default_rng = _RNG(0)
 def manual_seed(seed: int):
   """Seeds the device noise source used when noise is not injected."""
   default_rng.seed, default_rng.counter = seed, None
+
+
+def _mask_rng(offset: int, replicas: int, per_replica: bool, device) -> _RNG:
+  """The dropout-mask source of DRIL's policy ensemble / RED's predictor, keyed default_rng.seed + offset. per_replica (seed sweeps): every
+  replica draws its masks as a single-replica run does, under the same key at its own local indices."""
+  key = default_rng.seed + offset
+  return _RNG([key] * replicas if per_replica else key, device)
 
 
 class _Module:
@@ -149,6 +183,7 @@ class SoftActor(_Module):
   """:84-102. `actor(state)` returns a TanhNormalPolicy; state is [n, S] (R == 1) or [R, n, S]."""
 
   ENSEMBLE = 5  # :105
+  per_replica_masks = False  # True (seed sweeps): each replica draws the dropout masks of a single-replica run (_mask_rng)
 
   def __init__(self, state_size: int, action_size: int, model_cfg, replicas: int = 1, rng: Optional[ReplicaRNG] = None, device=None):
     # :88 — a policy with dropout is DRIL's "discriminator" (train.py:74); its density / BC update run on the dropout MLP program (csrc/dropout_nets.cu)
@@ -200,15 +235,11 @@ class SoftActor(_Module):
   def draw_masks(self, n: int) -> List[Optional[Tensor]]:
     """[input mask [R, n, S] or None, one [R, n, H] mask per hidden layer or None]: Bernoulli(1 - p) / (1 - p) draws on the device (Philox), the analogue
     of nn.Dropout's draws from torch's global stream."""
-    if self._drop_rng is None: self._drop_rng = _RNG(default_rng.seed + 977, self.device)
-    rng, R, lib = self._drop_rng, self.replicas, _lib.lib()
+    if self._drop_rng is None: self._drop_rng = _mask_rng(977, self.replicas, self.per_replica_masks, self.device)
+    rng, R = self._drop_rng, self.replicas
     def draw(width, p):
       if p <= 0: return None
-      out = torch.empty(R, n, width, device=self.device)
-      ctr = rng._ctr(self.device)
-      _lib.check(lib.il_fill_dropout_mask(_lib.handle(), out.data_ptr(), out.numel(), p, rng.seed, 31, ctr.data_ptr(), _lib.stream()))
-      _lib.check(lib.il_counter_add(_lib.handle(), ctr.data_ptr(), (out.numel() + 3) // 4, _lib.stream()))
-      return out
+      return rng.dropout_mask(torch.empty(R, n, width, device=self.device), p, 31)
     return [draw(self.state_size, self.input_dropout)] + [draw(self.mlp.dims[l + 1], self.dropout) for l in range(self.mlp.n_layers - 1)]
 
   def _log_prob_dropout(self, state: Tensor, action: Tensor, repeat: int = 1, masks: Optional[List[Optional[Tensor]]] = None) -> Tensor:
@@ -729,6 +760,7 @@ class PWILDiscriminator:
 
 class REDDiscriminator(_Module):
   """:252-284 — predictor (with dropout) and frozen random target embedding networks (din -> hidden^depth -> din), one pair per replica."""
+  per_replica_masks = False  # as SoftActor.per_replica_masks
 
   def __init__(self, state_size: int, action_size: int, imitation_cfg, replicas: int = 1, rng: Optional[ReplicaRNG] = None, device=None):
     cfg = imitation_cfg.discriminator
@@ -773,15 +805,11 @@ class REDDiscriminator(_Module):
     return self._ws
 
   def draw_masks(self, n: int) -> List[Optional[Tensor]]:
-    if self._rng is None: self._rng = _RNG(default_rng.seed + 1979, self.device)
-    rng, R, lib = self._rng, self.replicas, _lib.lib()
+    if self._rng is None: self._rng = _mask_rng(1979, self.replicas, self.per_replica_masks, self.device)
+    rng, R = self._rng, self.replicas
     def draw(width, p):
       if p <= 0: return None
-      out = torch.empty(R, n, width, device=self.device)
-      ctr = rng._ctr(self.device)
-      _lib.check(lib.il_fill_dropout_mask(_lib.handle(), out.data_ptr(), out.numel(), p, rng.seed, 32, ctr.data_ptr(), _lib.stream()))
-      _lib.check(lib.il_counter_add(_lib.handle(), ctr.data_ptr(), (out.numel() + 3) // 4, _lib.stream()))
-      return out
+      return rng.dropout_mask(torch.empty(R, n, width, device=self.device), p, 32)
     return [draw(self.predictor.dims[0], self.input_dropout)] + [draw(self.predictor.dims[l + 1], self.dropout) for l in range(self.predictor.n_layers - 1)]
 
   def _batch_of(self, state: Tensor, action: Tensor) -> TransitionBatch:

@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import contextlib
 import ctypes as C
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Union
 
 import torch
 from torch import Tensor, nn
@@ -17,14 +17,16 @@ from . import _lib
 
 
 class ReplicaRNG:
-  """Per-replica CPU RNG streams so that replica r initialises exactly like a reference run with seed + r
-  (train.py:51-52 seeds the global torch RNG once; constructors then draw from it in order)."""
+  """Per-replica CPU RNG streams so that replica r initialises exactly like a reference run with seed + r, or with seed[r] when `seed` is a
+  list of per-replica seeds (train.py:51-52 seeds the global torch RNG once; constructors then draw from it in order). A replica's state
+  keeps advancing with every draw made under `replica(r)`, as the single run's global stream does."""
 
-  def __init__(self, seed: int, replicas: int):
+  def __init__(self, seed: Union[int, Sequence[int]], replicas: int = 0):
+    seeds = [seed + r for r in range(replicas)] if isinstance(seed, int) else list(seed)
     self.states = []
-    for r in range(replicas):
+    for s in seeds:
       g = torch.Generator()
-      g.manual_seed(seed + r)
+      g.manual_seed(s)
       self.states.append(g.get_state())
 
   @classmethod

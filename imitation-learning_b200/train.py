@@ -3,7 +3,8 @@
 `Trainer.rollout()` is train.py:150-168 and `Trainer.update()` is train.py:171-203, each a fixed sequence of C-ABI
 calls on one CUDA stream with every piece of per-step state (env state, replay ring indices, optimiser step
 counts, RNG counters, the `step` counter) resident on the device — so both sequences are captured once as CUDA
-graphs and replayed without host involvement. Replica r is a reference-equivalent run with seed `cfg.seed + r`.
+graphs and replayed without host involvement. Replica r is a reference-equivalent run with seed `cfg.seed + r`; with per-replica seeds
+(`per_replica={'seed': [...]}`, a seed sweep) replica r draws every random number as the single run with seed[r] does, so it is that run.
 
 `Trainer(per_replica={key: R values})` gives the replicas their own values of the shape-preserving hyper-parameters
 (config.VECTORISED, for GAIL the discriminator choices of config.PER_REPLICA_DISCRIMINATOR and its hidden size, config.PER_REPLICA_WIDTH, and
@@ -22,7 +23,7 @@ import torch
 from torch import Tensor
 
 from . import _lib, distributed
-from .config import Config, SweepJob, expand_sweep, get_key, group_jobs, load_config, split_per_replica
+from .config import Config, SweepError, SweepJob, expand_sweep, get_key, load_config, needs_expert_memory, replica_values, split_per_replica, sweep_groups
 from .environments import D4RLEnv, ENVS
 from .evaluation import evaluate_agent
 from .memory import ReplayMemory, TransitionBatch
@@ -63,11 +64,14 @@ def check_config(cfg: Config, per_replica: Optional[Dict[str, Sequence]] = None)
 class Trainer:
   def __init__(self, cfg: Config, replicas: Optional[int] = None, seed_offset: int = 0, fast_init: bool = False, device=None,
                per_replica: Optional[Dict[str, Sequence[float]]] = None):
-    """per_replica: dotted config key (config.vectorised_keys) -> R values, replica r training with value r; a key whose values are all equal
-    runs as that scalar. None: every replica uses the config's values."""
+    """per_replica: dotted config key (config.per_replica_keys) -> R values, replica r training with value r; a key whose values are all equal
+    runs as that scalar. None: every replica uses the config's values. Per-replica seeds key every random stream of replica r by seed[r]
+    (device Philox draws at replica-local indices, host reset noise, initial weights and pre-training permutations)."""
     R = int(cfg.get('replicas', 1) if replicas is None else replicas)
     self.per_replica: Dict[str, List[float]] = {}
     if per_replica: cfg, self.per_replica = split_per_replica(cfg, per_replica, R)
+    seeds = self.seeds = self.per_replica.get('seed')  # None: uniform mode (one program seed, replica r initialised from seed + r)
+    if seeds is not None and fast_init: raise SweepError('per-replica seeds need each replica\'s own initial weights; fast_init replicates replica 0\'s')
     for k in ('imitation.grad_penalty', 'imitation.entropy_bonus'): assert min(self.per_replica.get(k, [0.0])) >= 0, k  # train.py:48-49
     check_config(cfg, self.per_replica)
     self.cfg = cfg
@@ -75,21 +79,23 @@ class Trainer:
     self.device = dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
     self.lib, self.h = _lib.lib(), _lib.handle(dev.index)
     _lib.check(self.lib.il_set_gemm_mode(self.h, _lib.GEMM_MODE[cfg.get('gemm_mode', 'fp32')]))
-    self.seed = seed = cfg.seed + seed_offset
+    self.seed = seed = cfg.seed + seed_offset if seeds is None else seeds[0]
     np.random.seed(seed)
     torch.manual_seed(seed)  # train.py:51-52
     self.algorithm = cfg.algorithm
     absorbing = bool(cfg.imitation.absorbing)
     # train.py:55-61
     self.env, self.eval_env = D4RLEnv(cfg.env, absorbing, load_data=True, replicas=R, device=dev), D4RLEnv(cfg.env, absorbing, replicas=R, device=dev)
-    self.env.seed(seed)
-    self.eval_env.seed(seed)
+    self.env.seed(seed if seeds is None else seeds)
+    self.eval_env.seed(seed if seeds is None else seeds)
     self.normalization_max, self.normalization_min = self.env.env.ref_max_score, self.env.env.ref_min_score
-    need_expert = self.algorithm != 'SAC' or cfg.bc_pretraining.iterations > 0 or cfg.imitation.bc_aux_loss
-    self.expert_memory = self.env.get_dataset(trajectories=cfg.imitation.trajectories, subsample=cfg.imitation.subsample) if need_expert else None
+    self.expert_memory = self.env.get_dataset(trajectories=cfg.imitation.trajectories, subsample=cfg.imitation.subsample) if needs_expert_memory(cfg) else None
     self.S, self.A = S, A = self.env.observation_space.shape[0], self.env.action_space.shape[0]
-    # train.py:64-67 — replica r draws its initial weights from the stream of seed + r (fast_init: one stream, replicated)
-    rng = None if (R == 1 or fast_init) else ReplicaRNG(seed, R)
+    # train.py:64-67 — replica r draws its initial weights from the stream of seed + r, or of seeds[r] (fast_init: one stream, replicated).
+    # With per-replica seeds the streams go on to draw the pre-training permutations, as the single run's global stream does.
+    if seeds is not None: rng = ReplicaRNG(seeds)
+    else: rng = None if (R == 1 or fast_init) else ReplicaRNG(seed, R)
+    self._init_rng = rng
     nrep = 1 if fast_init else R
     self.actor, self.critic = SoftActor(S, A, cfg.reinforcement.actor, replicas=nrep, rng=rng, device=dev), TwinCritic(S, A, cfg.reinforcement.critic, replicas=nrep, rng=rng, device=dev)
     self.discriminator = None
@@ -106,6 +112,9 @@ class Trainer:
       if d_rng is not rng: torch.set_rng_state(d_rng.states[0])  # the global stream goes on as after a fast_init run of replica 0's width
     elif self.algorithm == 'DRIL': self.discriminator = SoftActor(S, A, cfg.imitation.discriminator, replicas=nrep, rng=rng, device=dev)  # train.py:74
     elif self.algorithm == 'RED': self.discriminator = REDDiscriminator(S, A, cfg.imitation, replicas=nrep, rng=rng, device=dev)  # train.py:82
+    # the dropout masks are keyed on models.default_rng.seed, which no run sets: single runs of any seed draw the same mask stream, and so do
+    # the replicas of a seed sweep, each at its own local indices
+    if self.algorithm in ('DRIL', 'RED'): self.discriminator.per_replica_masks = seeds is not None
     if fast_init and R > 1:
       self._replicate()
       if self.algorithm == 'GAIL' and (rf is not None or sn is not None):
@@ -138,7 +147,7 @@ class Trainer:
       raise MemoryError(f'replay rings need {need / 2**30:.1f} GiB ({R} replicas x memory.size {cfg.memory.size} rows x {_lib.py_row_layout(S, A)[1] * 4} B) but only {free / 2**30:.1f} GiB '
                         f'are free on {dev}; lower memory.size (train.py:30 caps it at `steps`) or `replicas`')
     self.memory = ReplayMemory(cfg.memory.size, S, A, absorbing, replicas=R, device=dev)
-    self.memory.seed = seed
+    self.memory.seed = seed if seeds is None else seeds
     # train.py:70-84
     if self.algorithm in ('DRIL', 'GAIL', 'RED'):
       self.discriminator_optimiser = AdamW(self.discriminator.parameters(), lr=hp('imitation.learning_rate'), weight_decay=hp('imitation.weight_decay'))  # train.py:83-84
@@ -152,7 +161,7 @@ class Trainer:
     elif self.algorithm == 'PWIL':
       self.discriminator = PWILDiscriminator(S, A, cfg.imitation, self.expert_memory, self.env.max_episode_steps, replicas=R, device=dev,
                                              reward_scale=hp('imitation.reward_scale'), reward_bandwidth_scale=hp('imitation.reward_bandwidth_scale'))
-    if self.expert_memory is not None: self.expert_memory.seed = seed + 7919
+    if self.expert_memory is not None: self.expert_memory.seed = seed + 7919 if seeds is None else [s + 7919 for s in seeds]
     if self.algorithm == 'PWIL' and cfg.imitation.mix_expert_data != 'none': self._pwil_relabel_expert()  # train.py:136-140
     if self.algorithm in ('GMMIL', 'PWIL') and cfg.imitation.mix_expert_data == 'prefill_memory': self.memory.transfer_transitions(self.expert_memory)  # train.py:141,143
     # ---- per-step device state -------------------------------------------------------------------------------
@@ -173,7 +182,7 @@ class Trainer:
     self.eps_gp, self.eps_mix, self.eps_next, self.eps_new = f(R, B), f(R, B), f(R, B, A), f(R, B, A)
     self.sac_out = dict(log_probs=f(R, B), q_values=f(R, B), losses=f(R, 3))
     self.gail_losses = f(R, 2)
-    self.rng = _RNG(seed, dev)
+    self.rng = _RNG(seed if seeds is None else seeds, dev)
     self.inject = False  # tests: True = all noise / index buffers are filled by the caller before each step
     self.dril_masks = None  # tests (inject): the dropout masks of this step's DRIL ensemble pass
     self.device_rng = bool(cfg.get('device_rng', True))
@@ -310,7 +319,7 @@ class Trainer:
     per_epoch = max(n // B, 1)
     perm = None
     for it in range(iterations):
-      if it % per_epoch == 0: perm = torch.stack([torch.randperm(n) for _ in range(self.R)]).to(self.device, torch.int32)
+      if it % per_epoch == 0: perm = self._permutations(n)
       j = it % per_epoch
       idx = perm[:, j * B:(j + 1) * B] if n >= B else perm[:, torch.arange(B) % n]
       self.expert_memory.gather(idx.contiguous(), out=self.expert_batch)
@@ -328,7 +337,7 @@ class Trainer:
     for it in range(iterations):
       if batches is not None: idx = torch.as_tensor(batches[it], dtype=torch.int32).to(self.device).reshape(-1, B)
       else:
-        if it % per_epoch == 0: perm = torch.stack([torch.randperm(n) for _ in range(self.R)]).to(self.device, torch.int32)
+        if it % per_epoch == 0: perm = self._permutations(n)
         j = it % per_epoch
         idx = perm[:, j * B:(j + 1) * B] if n >= B else perm[:, torch.arange(B) % n]
       self.expert_memory.gather(idx.contiguous(), out=self.expert_batch)
@@ -346,6 +355,16 @@ class Trainer:
       d.eval()  # train.py:147
     if cfg.imitation.mix_expert_data == 'prefill_memory': self.memory.transfer_transitions(self.expert_memory)  # train.py:133
     self._pretrained = True
+
+  def _permutations(self, n: int) -> Tensor:
+    """[R, n] epoch permutations of the expert rows: from the global torch stream in replica order, or with per-replica seeds from each
+    replica's own stream (the draws its single run makes)."""
+    if self.seeds is None: perms = [torch.randperm(n) for _ in range(self.R)]
+    else:
+      perms = []
+      for r in range(self.R):
+        with self._init_rng.replica(r): perms.append(torch.randperm(n))
+    return torch.stack(perms).to(self.device, torch.int32)
 
   def _will_update(self, step: int) -> bool:
     return step >= self.cfg.training.start and step % self.cfg.training.interval == 0  # train.py:171
@@ -503,13 +522,14 @@ def _train(cfg: Config, blocks, per_replica: Optional[Dict[str, Sequence[float]]
 
 
 def run_sweep(jobs: List[SweepJob]) -> List[float]:
-  """A multirun on one GPU: the jobs are partitioned into groups (config.group_jobs); a group of J jobs is exactly the run
+  """A multirun on one GPU: the jobs are partitioned into groups (config.sweep_groups); a group of J jobs is exactly the run
   `train.py <group overrides> replicas=J*R` with job j's vectorised values given to replica block [jR, (j+1)R) — so replica jR+k starts
-  like a run with seed `seed + jR + k`. Groups run one after another. Job j writes the single-run files of its replicas, plus
+  like a run with seed `seed + jR + k`. A swept seed s_j is per replica instead: replica jR+k is the single run with seed s_j + k, so with
+  replicas=1 job j is `train.py <its overrides>` bit for bit. Groups run one after another. Job j writes the single-run files of its replicas, plus
   overrides.yaml, to <output_dir>/<ALG>_<ENV>_sweeper/<timestamp>/<j>/ (hydra.sweep.dir). Returns the per-job scores."""
   import yaml
   if int(os.environ.get('WORLD_SIZE', '1')) > 1: raise NotImplementedError('a multirun sweep runs on one GPU; sweeps across ranks are not supported')
-  groups = group_jobs(jobs)
+  groups = sweep_groups(jobs)
   cfg0 = load_config(jobs[0].overrides)
   base = os.path.join(cfg0.get('output_dir', './outputs'), f'{cfg0.algorithm}_{cfg0.env}_sweeper', time.strftime('%m-%d_%H-%M-%S'))
   print(f'sweep: {len(jobs)} job(s) in {len(groups)} group(s)', flush=True)
@@ -519,7 +539,7 @@ def run_sweep(jobs: List[SweepJob]) -> List[float]:
       cfg = load_config(g.overrides)
       R, J = int(cfg.get('replicas', 1)), len(g.jobs)
       cfg.replicas = J * R
-      per_replica = {k: [v for v in vals for _ in range(R)] for k, vals in g.per_job.items()}
+      per_replica = {k: replica_values(k, vals, R) for k, vals in g.per_job.items()}
       blocks = []
       for i, j in enumerate(g.jobs):
         d = os.path.join(base, str(j.num))

@@ -124,6 +124,14 @@ int il_counter_add(il_handle* h, uint64_t* counter, uint64_t inc, void* stream);
  * the draw at normal 0). alpha must be > 0 (other values give NaN). An element's value depends only on (seed, stream_id, *counter, i, its replica's alpha). */
 int il_fill_beta(il_handle* h, float* out, int R, int64_t n_per_replica, const float* alpha_r, uint64_t seed, uint64_t stream_id, const uint64_t* counter,
                  void* stream);
+/* Per-replica keys (seed sweeps): seed_r is an [R] uint64 device array (non-NULL), 1 <= R <= 65535, and out is [R, n_per_replica]. Replica r
+ * draws exactly what the scalar call over that replica alone draws with seed seed_r[r]: its element i uses the Philox counter
+ * (*counter + i / 4), lane i % 4, and the caller advances the counter by ceil(n_per_replica / 4), as for one replica (not by the R-replica
+ * total). Normal values pair lanes (0, 1) and (2, 3) of one counter, so pairs stay within a replica. One launch, graph-capturable. */
+int il_fill_normal_r(il_handle* h, float* out, int R, int64_t n_per_replica, const uint64_t* seed_r, uint64_t stream_id, const uint64_t* counter, void* stream);
+int il_fill_uniform_r(il_handle* h, float* out, int R, int64_t n_per_replica, const uint64_t* seed_r, uint64_t stream_id, const uint64_t* counter, void* stream);
+int il_fill_beta_r(il_handle* h, float* out, int R, int64_t n_per_replica, const float* alpha_r, const uint64_t* seed_r, uint64_t stream_id,
+                   const uint64_t* counter, void* stream);
 
 /* ---- SoftActor (models.py:84-102) --------------------------------------------------------------------- */
 /* forward + tanh-Gaussian head for n states per replica. eps == NULL: greedy (tanh(mean), models.py:101-102).
@@ -190,6 +198,10 @@ int il_bc_update(il_handle* h, const il_bc_args* a, void* stream);
  * Dropout masks are explicit inputs, pre-scaled {0, 1/(1-p)}: mask_in [R, n, dims[0]] for the input, mask_hid[l] [R, n, dims[l+1]] for hidden
  * layer l (applied BEFORE the activation, models.py:54-61); NULL = no dropout at that site. il_fill_dropout_mask draws them (Philox). */
 int il_fill_dropout_mask(il_handle* h, float* out, int64_t n, float p, uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream);
+/* Per-replica keys (see il_fill_normal_r): out [R, n_per_replica]; replica r is the il_fill_dropout_mask call over n_per_replica elements with
+ * seed seed_r[r]; the caller advances the counter by ceil(n_per_replica / 4). */
+int il_fill_dropout_mask_r(il_handle* h, float* out, int R, int64_t n_per_replica, float p, const uint64_t* seed_r, uint64_t stream_id, const uint64_t* counter,
+                           void* stream);
 int64_t il_actor_dropout_workspace_bytes(const il_mlp* actor, int R, int n);
 /* SoftActor.log_prob(state, action) (models.py:97-99) of a dropout policy; rows of states / given_action are repeated `repeat` times
  * (torch.repeat_interleave of the 5-member MC-dropout ensemble, models.py:105): n = repeat * source rows. */
@@ -250,6 +262,11 @@ int il_replay_wrap_absorbing(il_handle* h, const il_replay* mem, int R, const in
  * U[0,1) draws supplied by the caller (e.g. numpy on the host, like the reference) instead of device Philox. */
 int il_replay_sample_indices(il_handle* h, const il_replay* mem, int R, int n, int32_t* idx_out, const float* uniform,
                              uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream);
+/* Per-replica keys (seed sweeps): seed_r [R] uint64 on the device (non-NULL), 1 <= R <= 65535. Replica r's row of idx_out is the
+ * il_replay_sample_indices call over that replica alone (R = 1, its own ring or the shared one) with seed seed_r[r]: index k uses the
+ * Philox counter (*counter + k), and the caller advances the counter by n. */
+int il_replay_sample_indices_r(il_handle* h, const il_replay* mem, int R, int n, int32_t* idx_out, const float* uniform,
+                               const uint64_t* seed_r, uint64_t stream_id, const uint64_t* counter, void* stream);
 /* sample's gather (memory.py:60-62): out.rows[r, i, :] = mem.rows[r, idx[r, i], :] */
 int il_replay_gather(il_handle* h, const il_replay* mem, int R, const int32_t* idx, const il_batch* out, void* stream);
 /* mix_expert_agent_transitions (models.py:287-290): first B/2 rows <- expert rows (all fields). */
