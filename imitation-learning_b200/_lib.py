@@ -79,7 +79,7 @@ class GailxUpdateArgs(C.Structure):
 
 
 class Red(C.Structure):
-  _fields_ = [('predictor', Mlp), ('target', Mlp), ('sigma', vp), ('state_only', C.c_int32), ('_pad', C.c_int32)]
+  _fields_ = [('predictor', Mlp), ('target', Mlp), ('sigma', vp), ('state_only', C.c_int32), ('_pad', C.c_int32), ('activation_r', vp)]
 
 
 class RedUpdateArgs(C.Structure):
@@ -141,11 +141,11 @@ SIGNATURES = {
   'il_adam_step': (C.c_int, [vp, vp, vp, P(Adam), i64, vp]),
   'il_adam_step_polyak': (C.c_int, [vp, vp, vp, P(Adam), i64, vp, C.c_float, vp]),
   'il_adam_step_polyak_r': (C.c_int, [vp, vp, vp, P(Adam), i64, vp, vp, vp]),
-  'il_fill_dropout_mask': (C.c_int, [vp, vp, i64, f32, u64, u64, vp, vp]),
-  'il_fill_dropout_mask_r': (C.c_int, [vp, vp, C.c_int, i64, f32, vp, u64, vp, vp]),
+  'il_fill_dropout_mask': (C.c_int, [vp, vp, i64, f32, u64, u64, vp, vp, vp, C.c_int]),
+  'il_fill_dropout_mask_r': (C.c_int, [vp, vp, C.c_int, i64, f32, vp, u64, vp, vp, vp]),
   'il_actor_dropout_workspace_bytes': (i64, [P(Mlp), C.c_int, C.c_int]),
-  'il_actor_log_prob_dropout': (C.c_int, [vp, P(Mlp), C.c_int, C.c_int, C.c_int, vp, i64, C.c_int, vp, vp, P(vp), vp, vp, i64, vp]),
-  'il_bc_update_dropout': (C.c_int, [vp, P(BcArgs), vp, P(vp), vp]),
+  'il_actor_log_prob_dropout': (C.c_int, [vp, P(Mlp), C.c_int, C.c_int, C.c_int, vp, i64, C.c_int, vp, vp, P(vp), vp, vp, i64, vp, vp]),
+  'il_bc_update_dropout': (C.c_int, [vp, P(BcArgs), vp, P(vp), vp, vp]),
   'il_dril_reward': (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, i64, C.c_int, vp, vp]),
   'il_red_workspace_bytes': (i64, [P(Red), C.c_int, C.c_int]),
   'il_red_update': (C.c_int, [vp, P(RedUpdateArgs), vp]),
@@ -185,6 +185,10 @@ SIGNATURES = {
   'il_return_allreduce': (C.c_int, [vp, vp, vp, i64, vp, vp]),
 }
 
+# Optional trailing arguments added to an entry after it first shipped, with the defaults that keep the earlier behaviour (NULL / 0): calls that
+# omit them still work.
+TRAILING_DEFAULTS = {'il_fill_dropout_mask': (None, 0), 'il_fill_dropout_mask_r': (None, ), 'il_actor_log_prob_dropout': (None, ), 'il_bc_update_dropout': (None, )}
+
 _lock = threading.Lock()
 _lib: Optional[C.CDLL] = None
 _handles: Dict[int, int] = {}
@@ -209,8 +213,20 @@ def lib() -> C.CDLL:
       for name, (res, args) in SIGNATURES.items():
         fn = getattr(l, name)  # AttributeError if the library does not export a declared symbol
         fn.restype, fn.argtypes = res, args
+      for name, defaults in TRAILING_DEFAULTS.items(): setattr(l, name, _with_trailing_defaults(getattr(l, name), defaults))
       _lib = l
   return _lib
+
+
+def _with_trailing_defaults(fn, defaults):
+  n = len(fn.argtypes)
+
+  def call(*args):
+    missing = n - len(args)
+    if 0 < missing <= len(defaults): args += tuple(defaults[len(defaults) - missing:])
+    return fn(*args)
+  call.__name__, call.argtypes, call.restype = fn.__name__, fn.argtypes, fn.restype
+  return call
 
 
 def last_error() -> str:

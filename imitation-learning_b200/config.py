@@ -114,6 +114,13 @@ PER_REPLICA_ALGORITHM = {'AdRIL': ('imitation.update_freq', 'imitation.balanced'
 # (the host numpy index stream is one per rank), and with imitation.subsample > 1 when the run builds an expert memory (get_dataset draws the
 # subsampling offsets from the seeded numpy stream, and all replicas share that memory).
 PER_REPLICA_SEED = ('seed', )
+# RED's and DRIL's dropout rates and activation: per-replica values of the dropout program (csrc/dropout_nets.cu: the mask fill reads each replica's
+# rate, the activation passes each replica's activation). Only whether a rate is 0 is structural (the nn.Sequential indices and state_dict keys,
+# which mask draws happen, and for DRIL whether the dropout program runs at all), so sweep_groups groups on that presence (_dropout_presence) and
+# Trainer(per_replica=...) refuses a mix of 0 and > 0 for one site. DRIL's activation is per replica only with a dropout site: without one the
+# policy runs on the fused MLP kernels, which take one activation. Like `seed`, these keys are per replica in sweep_groups only (per_replica_keys).
+PER_REPLICA_DROPOUT = ('imitation.discriminator.input_dropout', 'imitation.discriminator.dropout', 'imitation.discriminator.activation')
+_ACTIVATIONS = ('relu', 'sigmoid', 'tanh')  # models.py:17 ACTIVATION_FUNCTIONS
 _CHOICES = {'imitation.loss_function': ('BCE', 'Mixup', 'PUGAIL'), 'imitation.discriminator.reward_function': ('AIRL', 'FAIRL', 'GAIL')}
 _SWEEP_FUNCTIONS = re.compile(r'^(range|choice|interval|glob|sort|shuffle|tag)\s*\(')
 
@@ -206,8 +213,29 @@ def vectorised_keys(cfg: Config) -> Tuple[str, ...]:
 
 
 def per_replica_keys(cfg: Config) -> Tuple[str, ...]:
-  """Every key Trainer(per_replica=...) takes in this configuration: vectorised_keys plus `seed` where it can be per replica (seed_per_replica)."""
-  return vectorised_keys(cfg) + (PER_REPLICA_SEED if seed_per_replica(cfg) else ())
+  """Every key Trainer(per_replica=...) takes in this configuration: vectorised_keys plus `seed` where it can be per replica (seed_per_replica)
+  and RED's / DRIL's dropout keys (dropout_keys)."""
+  return vectorised_keys(cfg) + (PER_REPLICA_SEED if seed_per_replica(cfg) else ()) + dropout_keys(cfg)
+
+
+def dropout_keys(cfg: Config) -> Tuple[str, ...]:
+  """The keys of PER_REPLICA_DROPOUT this configuration takes per replica: all three for RED; for DRIL the rates, and the activation when the
+  policy has a dropout site."""
+  alg = cfg.get('algorithm')
+  if alg == 'RED': return PER_REPLICA_DROPOUT
+  if alg != 'DRIL': return ()
+  d = cfg.imitation.get('discriminator') or {}
+  return PER_REPLICA_DROPOUT if any(_positive(d.get(k)) for k in ('input_dropout', 'dropout')) else PER_REPLICA_DROPOUT[:2]
+
+
+def _positive(x: Any) -> bool:
+  return isinstance(x, (int, float)) and not isinstance(x, bool) and x > 0
+
+
+def _dropout_presence(cfg: Config, keys) -> Tuple:
+  """Whether each dropout site whose rate is a per-replica key is present (rate > 0): the structural part of a rate, a grouping key."""
+  d = cfg.imitation.get('discriminator') or {}
+  return tuple((k, _positive(d.get(k.rsplit('.', 1)[1]))) for k in PER_REPLICA_DROPOUT[:2] if k in keys)
 
 
 def needs_expert_memory(cfg: Config) -> bool:
@@ -245,8 +273,9 @@ def _partition(jobs: List[SweepJob], conf_dir: str, keys_of) -> List[SweepGroup]
   for j in jobs:
     ov = dict(o.partition('=')[::2] for o in j.overrides)
     cfg = load_config(j.overrides, conf_dir)
-    vec = set(keys_of(cfg)) | set(UNUSED_KEYS.get(cfg.get('algorithm'), ()))
-    key = tuple((k, ov.get(k)) for k in swept if k not in vec)
+    keys = keys_of(cfg)
+    vec = set(keys) | set(UNUSED_KEYS.get(cfg.get('algorithm'), ()))
+    key = tuple((k, ov.get(k)) for k in swept if k not in vec) + _dropout_presence(cfg, [k for k in swept if k in keys])
     g = groups.setdefault(key, SweepGroup([]))
     g.jobs.append(j)
   for g in groups.values():
@@ -316,6 +345,17 @@ def _algorithm_value(k: str, x: Any, r: int) -> Any:
   return float(x)
 
 
+def _dropout_value(k: str, x: Any, r: int) -> Any:
+  """A value of PER_REPLICA_DROPOUT for replica r: an activation of models.py:17, or a rate in [0, 1) (nn.Dropout refuses p outside [0, 1], and
+  p = 1 scales by 1 / 0; the scalar path refuses it too)."""
+  if k == 'imitation.discriminator.activation':
+    if x not in _ACTIVATIONS: raise SweepError(f'replica {r}: {k}={x!r}: not one of {", ".join(_ACTIVATIONS)}')
+    return x
+  if isinstance(x, bool) or not isinstance(x, (int, float)): raise SweepError(f'replica {r}: {k}={x!r}: not a number')
+  if not 0 <= x < 1: raise SweepError(f'replica {r}: {k}={x!r}: not in [0, 1)')
+  return float(x)
+
+
 def _check_gail_replicas(cfg: Config, arrays: Dict[str, List[Any]], R: int):
   """The reference's GAIL asserts (train.py:42-47) for every replica: alpha > 0 for Mixup replicas, 0 <= prior <= 1 and margin >= 0 for PUGAIL ones."""
   val = lambda k, r: arrays[k][r] if k in arrays else get_key(cfg, k)
@@ -337,9 +377,11 @@ def split_per_replica(cfg: Config, per_replica: Optional[Dict[str, Sequence[Any]
   for k, vals in (per_replica or {}).items():
     if k not in allowed: raise SweepError(f'{k} cannot take per-replica values in this configuration (per-replica keys: {", ".join(allowed)})')
     per_alg = k in PER_REPLICA_ALGORITHM.get(cfg.get('algorithm'), ())
-    vals = [_algorithm_value(k, x, r) if per_alg else _per_replica_value(k, x) for r, x in enumerate(vals)]
+    vals = [_dropout_value(k, x, r) if k in PER_REPLICA_DROPOUT else _algorithm_value(k, x, r) if per_alg else _per_replica_value(k, x) for r, x in enumerate(vals)]
     if len(vals) != R: raise SweepError(f'{k}: {len(vals)} values for {R} replicas')
     if k in PER_REPLICA_WIDTH: _check_width_classes(k, vals)
+    if k in PER_REPLICA_DROPOUT[:2] and len({x > 0 for x in vals}) > 1:
+      raise SweepError(f'{k}: replicas mix rate 0 and rate > 0 ({vals}); whether a dropout site exists is a grouping key, only its rate is per replica')
     if all(x == vals[0] for x in vals): set_key(cfg, k, vals[0])
     else: arrays[k] = vals
   if cfg.get('algorithm') == 'GAIL': _check_gail_replicas(cfg, arrays, R)

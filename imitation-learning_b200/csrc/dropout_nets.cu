@@ -26,33 +26,62 @@ __global__ void input_mask_kernel(const float* __restrict__ X, int64_t x_gs, int
   const float v = X[(int64_t)g * x_gs + (int64_t)(i / rep) * ldx + k];
   out[t] = mask ? v * mask[t] : v;
 }
-// y = act(z * mask) in place
-__global__ void dropout_act_kernel(float* __restrict__ z, const float* __restrict__ mask, int64_t n, int act) {
+// y = act(z * mask) in place. act_r (per-replica activations, IL_ACT_*): blockIdx.y is the replica g and n its element count in the [G, n_g, H]
+// layout; NULL = `act` over all n.
+__global__ void dropout_act_kernel(float* __restrict__ z, const float* __restrict__ mask, int64_t n, int act, const int32_t* __restrict__ act_r) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (act_r) {
+    const int64_t o = (int64_t)blockIdx.y * n;
+    act = act_r[blockIdx.y]; z += o;
+    if (mask) mask += o;
+  }
   if (t < n) z[t] = act_apply(mask ? z[t] * mask[t] : z[t], act);
 }
-// t = t * act'(y) * mask in place (y = activation output)
-__global__ void dropout_bwd_kernel(float* __restrict__ t_, const float* __restrict__ y, const float* __restrict__ mask, int64_t n, int act) {
+// t = t * act'(y) * mask in place (y = activation output); act_r as in dropout_act_kernel
+__global__ void dropout_bwd_kernel(float* __restrict__ t_, const float* __restrict__ y, const float* __restrict__ mask, int64_t n, int act, const int32_t* __restrict__ act_r) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (act_r) {
+    const int64_t o = (int64_t)blockIdx.y * n;
+    act = act_r[blockIdx.y]; t_ += o; y += o;
+    if (mask) mask += o;
+  }
   if (t < n) t_[t] = t_[t] * act_grad_from_output(y[t], act) * (mask ? mask[t] : 1.f);
 }
+__device__ __forceinline__ float drop_keep(float u, float p) { return u >= p ? 1.f / (1.f - p) : 0.f; }
 // Bernoulli(1 - p) / (1 - p) from Philox4x32-10, one thread per quad at counter (*counter + quad). seed_r (per-replica keys): blockIdx.y is the
 // replica r, n its element count, and its quads of out + r * n draw key seed_r[r] at local counters; NULL = one key `seed` over all n.
+// p_r (per-replica rates): replica r draws with rate p_r[r] instead of p; with seed_r that is the replica blockIdx.y, without it element i belongs
+// to replica i / n_per_p, and a quad may straddle two replicas (n_per_p % 4 != 0). The counter and Philox lanes do not depend on the rates.
 __global__ void dropout_mask_kernel(float* __restrict__ out, int64_t n, float p, uint64_t seed, uint64_t stream_id, const uint64_t* __restrict__ counter,
-                                    const uint64_t* __restrict__ seed_r) {
+                                    const uint64_t* __restrict__ seed_r, const float* __restrict__ p_r, int64_t n_per_p) {
   const int64_t i4 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i4 * 4 >= n) return;
-  if (seed_r) { seed = seed_r[blockIdx.y]; out += (int64_t)blockIdx.y * n; }
+  if (seed_r) {
+    seed = seed_r[blockIdx.y]; out += (int64_t)blockIdx.y * n;
+    if (p_r) p = p_r[blockIdx.y];
+  }
   const uint64_t c = (counter ? *counter : 0ull) + (uint64_t)i4;
   const uint4 r = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), (uint32_t)stream_id, (uint32_t)(stream_id >> 32)), make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
-  const float keep = 1.f / (1.f - p);
   const uint32_t bits[4] = {r.x, r.y, r.z, r.w};
+  if (p_r && !seed_r) {
+    int64_t g = i4 * 4 / n_per_p, end = (g + 1) * n_per_p;  // one division per quad; later elements step over replica boundaries
+    for (int e = 0; e < 4 && i4 * 4 + e < n; ++e) {
+      while (i4 * 4 + e >= end) { ++g; end += n_per_p; }
+      out[i4 * 4 + e] = drop_keep(u32_to_unit(bits[e]), p_r[g]);
+    }
+    return;
+  }
   for (int e = 0; e < 4; ++e)
-    if (i4 * 4 + e < n) out[i4 * 4 + e] = u32_to_unit(bits[e]) >= p ? keep : 0.f;
+    if (i4 * 4 + e < n) out[i4 * 4 + e] = drop_keep(u32_to_unit(bits[e]), p);
 }
 
+// grid of an element-wise pass over cnt = G * per-net elements: one flat range, or (per-net blocks, G) with per-net activations (act_r)
+dim3 act_grid(int64_t cnt, int G, const int32_t* act_r) { return act_r ? dim3(dblocks(cnt / G), (unsigned)G) : dim3(dblocks(cnt)); }
+
 // forward: hid[l] = act((x_l W_l^T + b_l) * mask_l), out = x_{L-1} W_L^T + b_L. X must already carry the input mask (see input_mask_kernel).
-int mlp_forward_dropout(il_handle* h, const il_mlp* m, int G, int n, MatView X, const DropMasks& mk, const MlpActs& acts, float* out, int64_t out_gs, int ld_out, cudaStream_t st) {
+// act_r: [G] per-net activations (IL_ACT_*), NULL = m->activation for every net.
+int mlp_forward_dropout(il_handle* h, const il_mlp* m, int G, int n, MatView X, const DropMasks& mk, const MlpActs& acts, float* out, int64_t out_gs, int ld_out,
+                        const int32_t* act_r, cudaStream_t st) {
   const MlpOffsets o = mlp_offsets(m->dims, m->n_layers);
   const int L = m->n_layers;
   for (int l = 0; l < L; ++l) {
@@ -68,7 +97,7 @@ int mlp_forward_dropout(il_handle* h, const il_mlp* m, int G, int n, MatView X, 
     IL_TRY(launch_gemm(h, a, st));
     if (l < L - 1) {
       const int64_t cnt = (int64_t)G * n * m->dims[l + 1];
-      IL_LAUNCH(h, dropout_act_kernel, dblocks(cnt), 256, 0, st, acts.hid[l], mk.hid[l], cnt, m->activation);
+      IL_LAUNCH(h, dropout_act_kernel, act_grid(cnt, G, act_r), 256, 0, st, acts.hid[l], mk.hid[l], act_r ? cnt / G : cnt, m->activation, act_r);
     }
   }
   return 0;
@@ -76,7 +105,7 @@ int mlp_forward_dropout(il_handle* h, const il_mlp* m, int G, int n, MatView X, 
 
 // backward from dOut (gradient at the linear head); grads in the flat parameter layout
 int mlp_backward_dropout(il_handle* h, const il_mlp* m, int G, int n, MatView X, const DropMasks& mk, const MlpActs& acts, MatView dOut, float* grads, int64_t grad_stride, float* tmpA,
-                         float* tmpB, cudaStream_t st) {
+                         float* tmpB, const int32_t* act_r, cudaStream_t st) {
   const MlpOffsets o = mlp_offsets(m->dims, m->n_layers);
   const int L = m->n_layers;
   MatView dZ = dOut;
@@ -100,7 +129,7 @@ int mlp_backward_dropout(il_handle* h, const il_mlp* m, int G, int n, MatView X,
       a.M = n; a.N = m->dims[l]; a.K = m->dims[l + 1]; a.G = G;
       IL_TRY(launch_gemm(h, a, st));
       const int64_t cnt = (int64_t)G * n * m->dims[l];
-      IL_LAUNCH(h, dropout_bwd_kernel, dblocks(cnt), 256, 0, st, next_tmp, acts.hid[l - 1], mk.hid[l - 1], cnt, m->activation);
+      IL_LAUNCH(h, dropout_bwd_kernel, act_grid(cnt, G, act_r), 256, 0, st, next_tmp, acts.hid[l - 1], mk.hid[l - 1], act_r ? cnt / G : cnt, m->activation, act_r);
       dZ = MatView{next_tmp, (int64_t)n * m->dims[l], 1, m->dims[l]};
       next_tmp = next_tmp == tmpA ? tmpB : tmpA;
     }
@@ -213,18 +242,22 @@ int red_validate(const il_red* d, const il_batch* b, const char* what) {
   IL_CHECK(b->row == row_layout(b->S, b->A).len, "%s: bad row length", what);
   return 0;
 }
+int act_r_validate(const int32_t* act_r, int R, const char* what) {
+  IL_CHECK(!act_r || (R > 0 && R <= IL_MAX_GRID_Y), "%s: per-replica activations need 0 < R <= %d (R = %d)", what, IL_MAX_GRID_Y, R);
+  return 0;
+}
 // prediction (with the given masks) and target for the rows of `b`
 int red_forward(il_handle* h, const il_red* d, int R, const il_batch* b, const DropMasks& mk, RedWs& w, cudaStream_t st) {
   const int B = b->B, din = d->predictor.dims[0];
   MatView X{b->rows, b->replica_stride, 1, b->row};
   if (mk.in) {
     IL_LAUNCH(h, input_mask_kernel, dblocks((int64_t)R * B * din), 256, 0, st, b->rows, b->replica_stride, b->row, 1, mk.in, w.xin, R, B, din);
-    IL_TRY(mlp_forward_dropout(h, &d->predictor, R, B, MatView{w.xin, (int64_t)B * din, 1, din}, mk, w.pacts, w.pred, (int64_t)B * din, din, st));
+    IL_TRY(mlp_forward_dropout(h, &d->predictor, R, B, MatView{w.xin, (int64_t)B * din, 1, din}, mk, w.pacts, w.pred, (int64_t)B * din, din, d->activation_r, st));
   } else {
-    IL_TRY(mlp_forward_dropout(h, &d->predictor, R, B, X, mk, w.pacts, w.pred, (int64_t)B * din, din, st));
+    IL_TRY(mlp_forward_dropout(h, &d->predictor, R, B, X, mk, w.pacts, w.pred, (int64_t)B * din, din, d->activation_r, st));
   }
-  DropMasks none{};
-  return mlp_forward_dropout(h, &d->target, R, B, X, none, w.tacts, w.targ, (int64_t)B * din, din, st);
+  DropMasks none{};  // the frozen target takes the replica's activation, as its predictor does
+  return mlp_forward_dropout(h, &d->target, R, B, X, none, w.tacts, w.targ, (int64_t)B * din, din, d->activation_r, st);
 }
 DropMasks masks_of(const float* in, const float* const* hid) {
   DropMasks m{};
@@ -252,17 +285,19 @@ __global__ void dril_reward_kernel(const float* __restrict__ log_prob, int R, in
 
 }  // namespace
 
-extern "C" int il_fill_dropout_mask(il_handle* h, float* out, int64_t n, float p, uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream) {
+extern "C" int il_fill_dropout_mask(il_handle* h, float* out, int64_t n, float p, uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream, const float* p_r,
+                                    int R) {
   IL_CHECK(h && out && n > 0 && p >= 0.f && p < 1.f, "il_fill_dropout_mask: bad argument (p = %f)", (double)p);
-  IL_LAUNCH(h, dropout_mask_kernel, dblocks((n + 3) / 4), 256, 0, (cudaStream_t)stream, out, n, p, seed, stream_id, counter, nullptr);
+  IL_CHECK(!p_r || (R > 0 && n % R == 0), "il_fill_dropout_mask: per-replica rates need n (%lld) to split over R = %d replicas", (long long)n, R);
+  IL_LAUNCH(h, dropout_mask_kernel, dblocks((n + 3) / 4), 256, 0, (cudaStream_t)stream, out, n, p, seed, stream_id, counter, nullptr, p_r, p_r ? n / R : n);
   return 0;
 }
 extern "C" int il_fill_dropout_mask_r(il_handle* h, float* out, int R, int64_t n_per_replica, float p, const uint64_t* seed_r, uint64_t stream_id, const uint64_t* counter,
-                                      void* stream) {
+                                      void* stream, const float* p_r) {
   IL_CHECK(h && out && seed_r && R > 0 && R <= IL_MAX_GRID_Y && n_per_replica > 0 && p >= 0.f && p < 1.f, "il_fill_dropout_mask_r: bad argument (R = %d, p = %f)", R,
            (double)p);
   IL_LAUNCH(h, dropout_mask_kernel, dim3(dblocks((n_per_replica + 3) / 4), (unsigned)R), 256, 0, (cudaStream_t)stream, out, n_per_replica, p, 0ull, stream_id, counter,
-            seed_r);
+            seed_r, p_r, n_per_replica);
   return 0;
 }
 
@@ -277,6 +312,7 @@ extern "C" int il_red_update(il_handle* h, const il_red_update_args* a, void* st
   const il_red* d = &a->disc;
   IL_TRY(red_validate(d, &a->batch, "il_red_update"));
   const int R = a->R, B = a->batch.B, din = d->predictor.dims[0];
+  IL_TRY(act_r_validate(d->activation_r, R, "il_red_update"));
   IL_CHECK(R > 0 && a->opt.m && a->opt.v && a->opt.step && a->workspace && a->workspace_bytes >= il_red_workspace_bytes(d, R, B), "il_red_update: bad optimiser state / workspace");
   RedWs w = red_layout(d, R, B, static_cast<char*>(a->workspace), true);
   const DropMasks mk = masks_of(a->mask_in, a->mask_hid);
@@ -286,7 +322,7 @@ extern "C" int il_red_update(il_handle* h, const il_red_update_args* a, void* st
   IL_LAUNCH(h, red_loss_kernel, R, 256, 0, st, w.pred, w.targ, a->batch.rows, a->batch.replica_stride, a->batch.row, RL.weight, w.dpred, a->out_loss, B, din);
   IL_CUDA(cudaMemsetAsync(w.grads, 0, (size_t)R * d->predictor.stride * 4, st));
   const MatView X = mk.in ? MatView{w.xin, (int64_t)B * din, 1, din} : MatView{a->batch.rows, a->batch.replica_stride, 1, a->batch.row};
-  IL_TRY(mlp_backward_dropout(h, &d->predictor, R, B, X, mk, w.pacts, MatView{w.dpred, (int64_t)B * din, 1, din}, w.grads, d->predictor.stride, w.tmpA, w.tmpB, st));
+  IL_TRY(mlp_backward_dropout(h, &d->predictor, R, B, X, mk, w.pacts, MatView{w.dpred, (int64_t)B * din, 1, din}, w.grads, d->predictor.stride, w.tmpA, w.tmpB, d->activation_r, st));
   return launch_adam(h, d->predictor.params, w.grads, &a->opt, (int64_t)R * d->predictor.stride, st);
 }
 
@@ -295,6 +331,7 @@ extern "C" int il_red_sigma(il_handle* h, const il_red* d, int R, const il_batch
   IL_CHECK(h && d && d->sigma && workspace, "il_red_sigma: null argument");
   cudaStream_t st = (cudaStream_t)stream;
   IL_TRY(red_validate(d, batch, "il_red_sigma"));
+  IL_TRY(act_r_validate(d->activation_r, R, "il_red_sigma"));
   const int B = batch->B, din = d->predictor.dims[0];
   IL_CHECK(workspace_bytes >= il_red_workspace_bytes(d, R, B), "il_red_sigma: workspace too small");
   RedWs w = red_layout(d, R, B, static_cast<char*>(workspace), true);
@@ -309,6 +346,7 @@ extern "C" int il_red_reward(il_handle* h, const il_red* d, int R, const il_batc
   IL_CHECK(h && d && d->sigma && reward && workspace, "il_red_reward: null argument");
   cudaStream_t st = (cudaStream_t)stream;
   IL_TRY(red_validate(d, batch, "il_red_reward"));
+  IL_TRY(act_r_validate(d->activation_r, R, "il_red_reward"));
   const int B = batch->B, din = d->predictor.dims[0];
   IL_CHECK(workspace_bytes >= il_red_workspace_bytes(d, R, B), "il_red_reward: workspace too small");
   RedWs w = red_layout(d, R, B, static_cast<char*>(workspace), true);
@@ -347,9 +385,11 @@ extern "C" int64_t il_actor_dropout_workspace_bytes(const il_mlp* actor, int R, 
 
 // log pi(given_action | state) of R dropout policies on n rows each; rows of `states` / `given_action` are repeated `repeat` times (n = repeat * source rows).
 extern "C" int il_actor_log_prob_dropout(il_handle* h, const il_mlp* actor, int R, int n, int repeat, const float* states, int64_t states_rs, int ld_states, const float* given_action,
-                                         const float* mask_in, const float* const* mask_hid, float* log_prob, void* workspace, int64_t workspace_bytes, void* stream) {
+                                         const float* mask_in, const float* const* mask_hid, float* log_prob, void* workspace, int64_t workspace_bytes, void* stream,
+                                         const int32_t* activation_r) {
   IL_CHECK(h && states && given_action && log_prob && workspace && R > 0 && n > 0 && repeat >= 1 && n % repeat == 0, "il_actor_log_prob_dropout: bad argument");
   IL_TRY(mlp_validate(actor, "il_actor_log_prob_dropout"));
+  IL_TRY(act_r_validate(activation_r, R, "il_actor_log_prob_dropout"));
   IL_CHECK(workspace_bytes >= il_actor_dropout_workspace_bytes(actor, R, n), "il_actor_log_prob_dropout: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const int S = actor->dims[0], out = actor->dims[actor->n_layers], A = out / 2;
@@ -357,7 +397,7 @@ extern "C" int il_actor_log_prob_dropout(il_handle* h, const il_mlp* actor, int 
   const DropMasks mk = masks_of(mask_in, mask_hid);
   IL_LAUNCH(h, input_mask_kernel, dblocks((int64_t)R * n * S), 256, 0, st, states, states_rs, ld_states, repeat, mask_in, w.xin, R, n, S);
   IL_LAUNCH(h, input_mask_kernel, dblocks((int64_t)R * n * A), 256, 0, st, given_action, (int64_t)(n / repeat) * A, A, repeat, nullptr, w.given, R, n, A);
-  IL_TRY(mlp_forward_dropout(h, actor, R, n, MatView{w.xin, (int64_t)n * S, 1, S}, mk, w.acts, w.head, (int64_t)n * out, out, st));
+  IL_TRY(mlp_forward_dropout(h, actor, R, n, MatView{w.xin, (int64_t)n * S, 1, S}, mk, w.acts, w.head, (int64_t)n * out, out, activation_r, st));
   HeadFwdArgs ha{};
   ha.head = w.head; ha.given = w.given; ha.log_prob = log_prob; ha.R = R; ha.n = n; ha.A = A;
   return launch_actor_head(h, ha, st);
@@ -374,11 +414,12 @@ extern "C" int il_dril_reward(il_handle* h, const float* log_prob, int R, int B,
 int bc_head_backward_launch(il_handle* h, const float* head, const il_batch* batch, float* dhead, float* row_loss, int R, cudaStream_t st);
 int bc_row_mean_launch(il_handle* h, const float* row_loss, float* out_loss, int R, int B, cudaStream_t st);
 
-extern "C" int il_bc_update_dropout(il_handle* h, const il_bc_args* a, const float* mask_in, const float* const* mask_hid, void* stream) {
+extern "C" int il_bc_update_dropout(il_handle* h, const il_bc_args* a, const float* mask_in, const float* const* mask_hid, void* stream, const int32_t* activation_r) {
   IL_CHECK(h && a, "il_bc_update_dropout: null argument");
   cudaStream_t st = (cudaStream_t)stream;
   const int R = a->R, B = a->batch.B, S = a->batch.S, A = a->batch.A;
   IL_TRY(mlp_validate(&a->actor, "il_bc_update_dropout"));
+  IL_TRY(act_r_validate(activation_r, R, "il_bc_update_dropout"));
   IL_CHECK(R > 0 && B > 0 && a->actor.dims[0] == S && a->actor.dims[a->actor.n_layers] == 2 * A, "il_bc_update_dropout: actor dims do not match the batch");
   IL_CHECK(a->batch.rows && a->batch.row == row_layout(S, A).len && a->workspace && a->workspace_bytes >= il_actor_dropout_workspace_bytes(&a->actor, R, B), "il_bc_update_dropout: bad batch / workspace");
   ActWs w = actor_layout(&a->actor, R, B, static_cast<char*>(a->workspace), true);
@@ -390,10 +431,10 @@ extern "C" int il_bc_update_dropout(il_handle* h, const il_bc_args* a, const flo
     IL_LAUNCH(h, input_mask_kernel, dblocks((int64_t)R * B * S), 256, 0, st, a->batch.rows, a->batch.replica_stride, a->batch.row, 1, mask_in, w.xin, R, B, S);
     X = MatView{w.xin, (int64_t)B * S, 1, S};
   }
-  IL_TRY(mlp_forward_dropout(h, &a->actor, R, B, X, mk, w.acts, w.head, (int64_t)B * out, out, st));
+  IL_TRY(mlp_forward_dropout(h, &a->actor, R, B, X, mk, w.acts, w.head, (int64_t)B * out, out, activation_r, st));
   IL_TRY(bc_head_backward_launch(h, w.head, &a->batch, w.dhead, a->out_loss ? w.row_loss : nullptr, R, st));
   if (a->out_loss) IL_TRY(bc_row_mean_launch(h, w.row_loss, a->out_loss, R, B, st));
   IL_CUDA(cudaMemsetAsync(w.grads, 0, (size_t)R * a->actor.stride * 4, st));
-  IL_TRY(mlp_backward_dropout(h, &a->actor, R, B, X, mk, w.acts, MatView{w.dhead, (int64_t)B * out, 1, out}, w.grads, a->actor.stride, w.tmpA, w.tmpB, st));
+  IL_TRY(mlp_backward_dropout(h, &a->actor, R, B, X, mk, w.acts, MatView{w.dhead, (int64_t)B * out, 1, out}, w.grads, a->actor.stride, w.tmpA, w.tmpB, activation_r, st));
   return launch_adam(h, a->actor.params, w.grads, &a->opt, (int64_t)R * a->actor.stride, st);
 }

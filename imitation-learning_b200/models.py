@@ -89,11 +89,17 @@ class _RNG:
     self._advance(ctr, n)
     return out
 
-  def dropout_mask(self, out: Tensor, p: float, stream_id: int) -> Tensor:
-    """Bernoulli(1 - p) / (1 - p) draws into `out` (il_fill_dropout_mask), the analogue of nn.Dropout's draws from torch's global stream."""
+  def dropout_mask(self, out: Tensor, p: float, stream_id: int, p_r: Optional[Tensor] = None) -> Tensor:
+    """Bernoulli(1 - p) / (1 - p) draws into `out` (il_fill_dropout_mask), the analogue of nn.Dropout's draws from torch's global stream.
+    p_r: an [R] float32 device tensor of per-replica rates (out's leading axis is R); each element draws what it draws with one rate, at its
+    replica's rate."""
     lib, ctr, n = _lib.lib(), self._ctr(out.device), self._per_key(out)
-    if self.seed_r is None: _lib.check(lib.il_fill_dropout_mask(_lib.handle(), out.data_ptr(), n, p, self.seed, stream_id, ctr.data_ptr(), _lib.stream()))
-    else: _lib.check(lib.il_fill_dropout_mask_r(_lib.handle(), out.data_ptr(), self.seed_r.numel(), n, p, self.seed_r.data_ptr(), stream_id, ctr.data_ptr(), _lib.stream()))
+    if p_r is not None: assert p_r.dtype == torch.float32 and p_r.is_cuda and p_r.numel() == out.size(0)
+    if self.seed_r is None:
+      _lib.check(lib.il_fill_dropout_mask(_lib.handle(), out.data_ptr(), n, p, self.seed, stream_id, ctr.data_ptr(), _lib.stream(), _lib.ptr(p_r), 0 if p_r is None else p_r.numel()))
+    else:
+      _lib.check(lib.il_fill_dropout_mask_r(_lib.handle(), out.data_ptr(), self.seed_r.numel(), n, p, self.seed_r.data_ptr(), stream_id, ctr.data_ptr(), _lib.stream(),
+                                            _lib.ptr(p_r)))
     self._advance(ctr, n)
     return out
 
@@ -111,6 +117,32 @@ def _mask_rng(offset: int, replicas: int, per_replica: bool, device) -> _RNG:
   replica draws its masks as a single-replica run does, under the same key at its own local indices."""
   key = default_rng.seed + offset
   return _RNG([key] * replicas if per_replica else key, device)
+
+
+class _DropoutChoices:
+  """Per-replica activation and dropout rates of a network with dropout (DRIL's policy, RED's predictor): each one value or R values. Whether a
+  rate is 0 is the same for every replica (it decides the nn.Sequential indices and which mask draws happen); the rates and the activation may
+  differ. R equal values are the uniform path: no device array is made. The arrays are made once, before any graph capture."""
+
+  def __init__(self, cfg, replicas: int, device, activation=None, input_dropout=None, dropout=None):
+    self.activations = [str(x) for x in _per_replica_choice(cfg.activation if activation is None else activation, replicas)]
+    rate = lambda x, k: [float(v or 0) for v in _per_replica_choice(float(_cfg_get(cfg, k, 0) or 0) if x is None else x, replicas)]
+    self.input_dropouts, self.dropouts = rate(input_dropout, 'input_dropout'), rate(dropout, 'dropout')
+    for a in self.activations:
+      if a not in _lib.ACT: raise ValueError(f'activation {a!r} not in {sorted(_lib.ACT)}')
+    for name, ps in (('input_dropout', self.input_dropouts), ('dropout', self.dropouts)):
+      if not all(0 <= p < 1 for p in ps): raise ValueError(f'{name}: rates must be in [0, 1), got {ps}')
+      if len({p > 0 for p in ps}) > 1: raise ValueError(f'{name}: some replicas have dropout and some do not ({ps}); presence must be the same for every replica')
+    device = torch.device('cuda') if device is None else torch.device(device)
+    f32 = lambda ps: None if len(set(ps)) == 1 else torch.tensor(ps, dtype=torch.float32, device=device)  # each rounded once from the double, as ctypes rounds `float p`
+    self.input_dropout_r, self.dropout_r = f32(self.input_dropouts), f32(self.dropouts)
+    self.activation_r = None if len(set(self.activations)) == 1 else list(self.activations)
+    self.act_r = None if self.activation_r is None else torch.tensor([_lib.ACT[a] for a in self.activations], dtype=torch.int32, device=device)
+
+
+def _masks_of(rng: _RNG, R: int, n: int, device, sites, stream_id: int) -> List[Optional[Tensor]]:
+  """One mask per (width, p, p_r) site: None where p is 0, else an [R, n, width] draw at the replicas' rates."""
+  return [None if p <= 0 else rng.dropout_mask(torch.empty(R, n, w, device=device), p, stream_id, p_r) for w, p, p_r in sites]
 
 
 class _Module:
@@ -185,18 +217,25 @@ class SoftActor(_Module):
   ENSEMBLE = 5  # :105
   per_replica_masks = False  # True (seed sweeps): each replica draws the dropout masks of a single-replica run (_mask_rng)
 
-  def __init__(self, state_size: int, action_size: int, model_cfg, replicas: int = 1, rng: Optional[ReplicaRNG] = None, device=None):
+  def __init__(self, state_size: int, action_size: int, model_cfg, replicas: int = 1, rng: Optional[ReplicaRNG] = None, device=None, activation=None,
+               input_dropout=None, dropout=None):
+    """activation / input_dropout / dropout: None = the config's value; otherwise one value, or one value per replica (DRIL sweeps: replica r is
+    initialised with its own activation's gain and trained and rewarded with its own activation and rates). Per-replica activations need a
+    dropout policy, whose passes run on the dropout program."""
     # :88 — a policy with dropout is DRIL's "discriminator" (train.py:74); its density / BC update run on the dropout MLP program (csrc/dropout_nets.cu)
-    self.input_dropout, self.dropout = float(_cfg_get(model_cfg, 'input_dropout', 0) or 0), float(_cfg_get(model_cfg, 'dropout', 0) or 0)
+    ch = self._choices = _DropoutChoices(model_cfg, replicas, device, activation, input_dropout, dropout)
+    self.input_dropout, self.dropout = ch.input_dropouts[0], ch.dropouts[0]
+    self.activation_r = ch.activation_r
+    if self.activation_r is not None and not self.has_dropout: raise ValueError('per-replica activations need a dropout policy (input_dropout or dropout > 0)')
     self.training, self.q, self._drop_ws, self._drop_rng = True, None, None, None
     self.state_size, self.action_size, self.replicas = state_size, action_size, replicas
     self.log_std_dev_min, self.log_std_dev_max = -20, 2  # :87 (the kernel hard-codes the same clamp)
     dims = [state_size] + [model_cfg.hidden_size] * model_cfg.depth + [2 * action_size]
-    self.mlp = ReplicaMLP(dims, model_cfg.activation, replicas, 1, device)
+    self.mlp = ReplicaMLP(dims, ch.activations[0], replicas, 1, device)
     self.device = self.mlp.device
     for r in range(replicas):
       with (rng.replica(r) if rng is not None else _null_ctx()):
-        self.mlp.load_params(r, 0, init_fcnn_params(dims, model_cfg.activation))
+        self.mlp.load_params(r, 0, init_fcnn_params(dims, ch.activations[r]))
     self._ws = None
 
   def _squeeze(self, t: Tensor) -> Tensor:
@@ -208,6 +247,7 @@ class SoftActor(_Module):
     return [(f'actor.{base + step * l}.{n}', v[2 * l + i]) for l in range(self.mlp.n_layers) for i, n in enumerate(('weight', 'bias'))]
 
   def _run(self, state: Tensor, eps: Optional[Tensor] = None, given: Optional[Tensor] = None, want=('action', )) -> Dict[str, Tensor]:
+    if self.activation_r is not None: raise NotImplementedError('per-replica activations run on the dropout program only (log_prob in train mode or with masks)')
     R, A = self.replicas, self.action_size
     s = _as_rns(state, R, self.state_size, self.device)
     n = s.size(1)
@@ -236,11 +276,9 @@ class SoftActor(_Module):
     """[input mask [R, n, S] or None, one [R, n, H] mask per hidden layer or None]: Bernoulli(1 - p) / (1 - p) draws on the device (Philox), the analogue
     of nn.Dropout's draws from torch's global stream."""
     if self._drop_rng is None: self._drop_rng = _mask_rng(977, self.replicas, self.per_replica_masks, self.device)
-    rng, R = self._drop_rng, self.replicas
-    def draw(width, p):
-      if p <= 0: return None
-      return rng.dropout_mask(torch.empty(R, n, width, device=self.device), p, 31)
-    return [draw(self.state_size, self.input_dropout)] + [draw(self.mlp.dims[l + 1], self.dropout) for l in range(self.mlp.n_layers - 1)]
+    ch = self._choices
+    sites = [(self.state_size, self.input_dropout, ch.input_dropout_r)] + [(self.mlp.dims[l + 1], self.dropout, ch.dropout_r) for l in range(self.mlp.n_layers - 1)]
+    return _masks_of(self._drop_rng, self.replicas, n, self.device, sites, 31)
 
   def _log_prob_dropout(self, state: Tensor, action: Tensor, repeat: int = 1, masks: Optional[List[Optional[Tensor]]] = None) -> Tensor:
     R, S, A = self.replicas, self.state_size, self.action_size
@@ -253,7 +291,7 @@ class SoftActor(_Module):
     if self._drop_ws is None or self._drop_ws.numel() < need: self._drop_ws = torch.zeros(need, dtype=torch.uint8, device=self.device)
     out = torch.empty(R, n, device=self.device)
     _lib.check(_lib.lib().il_actor_log_prob_dropout(_lib.handle(), C.byref(m), R, n, repeat, s.data_ptr(), s.stride(0), s.stride(1), a.data_ptr(), _lib.ptr(masks[0]), _lib.mask_array(masks[1:]),
-                                                    out.data_ptr(), self._drop_ws.data_ptr(), self._drop_ws.numel(), _lib.stream()))
+                                                    out.data_ptr(), self._drop_ws.data_ptr(), self._drop_ws.numel(), _lib.stream(), _lib.ptr(self._choices.act_r)))
     return out
 
   def _get_action_uncertainty(self, state: Tensor, action: Tensor, masks=None) -> Tensor:  # :104-107
@@ -762,20 +800,23 @@ class REDDiscriminator(_Module):
   """:252-284 — predictor (with dropout) and frozen random target embedding networks (din -> hidden^depth -> din), one pair per replica."""
   per_replica_masks = False  # as SoftActor.per_replica_masks
 
-  def __init__(self, state_size: int, action_size: int, imitation_cfg, replicas: int = 1, rng: Optional[ReplicaRNG] = None, device=None):
+  def __init__(self, state_size: int, action_size: int, imitation_cfg, replicas: int = 1, rng: Optional[ReplicaRNG] = None, device=None, activation=None,
+               input_dropout=None, dropout=None):
+    """activation / input_dropout / dropout: as SoftActor's. Replica r's predictor and frozen target both use replica r's activation."""
     cfg = imitation_cfg.discriminator
     self.state_only, self.replicas = bool(imitation_cfg.state_only), replicas
     self.state_size, self.action_size = state_size, action_size
     din = state_size if self.state_only else state_size + action_size
     dims = [din] + [cfg.hidden_size] * cfg.depth + [din]
-    self.input_dropout, self.dropout = float(_cfg_get(cfg, 'input_dropout', 0) or 0), float(_cfg_get(cfg, 'dropout', 0) or 0)
-    self.predictor, self.target = ReplicaMLP(dims, cfg.activation, replicas, 1, device), ReplicaMLP(dims, cfg.activation, replicas, 1, device)
+    ch = self._choices = _DropoutChoices(cfg, replicas, device, activation, input_dropout, dropout)
+    self.input_dropout, self.dropout, self.activation_r = ch.input_dropouts[0], ch.dropouts[0], ch.activation_r
+    self.predictor, self.target = ReplicaMLP(dims, ch.activations[0], replicas, 1, device), ReplicaMLP(dims, ch.activations[0], replicas, 1, device)
     self.mlp = self.predictor  # parameters(): only the predictor trains (:267-268; AdamW skips the frozen target, train.py:84)
     self.device = self.predictor.device
     for r in range(replicas):
       with (rng.replica(r) if rng is not None else _null_ctx()):
-        self.predictor.load_params(r, 0, init_fcnn_params(dims, cfg.activation))  # :265
-        self.target.load_params(r, 0, init_fcnn_params(dims, cfg.activation))     # :266
+        self.predictor.load_params(r, 0, init_fcnn_params(dims, ch.activations[r]))  # :265
+        self.target.load_params(r, 0, init_fcnn_params(dims, ch.activations[r]))     # :266
     s1 = _cfg_get(imitation_cfg, 'reward_bandwidth_scale', None)
     self.sigma = torch.full((replicas, ), float(s1) if s1 else 0.0, device=self.device)  # :269
     self._sigma_set = bool(s1)
@@ -787,6 +828,7 @@ class REDDiscriminator(_Module):
   def c_struct(self) -> _lib.Red:
     d = _lib.Red()
     d.predictor, d.target, d.sigma, d.state_only = self.predictor.c_struct(), self.target.c_struct(), self.sigma.data_ptr(), int(self.state_only)
+    d.activation_r = _lib.ptr(self._choices.act_r)
     return d
 
   def _state_items(self):
@@ -806,11 +848,9 @@ class REDDiscriminator(_Module):
 
   def draw_masks(self, n: int) -> List[Optional[Tensor]]:
     if self._rng is None: self._rng = _mask_rng(1979, self.replicas, self.per_replica_masks, self.device)
-    rng, R = self._rng, self.replicas
-    def draw(width, p):
-      if p <= 0: return None
-      return rng.dropout_mask(torch.empty(R, n, width, device=self.device), p, 32)
-    return [draw(self.predictor.dims[0], self.input_dropout)] + [draw(self.predictor.dims[l + 1], self.dropout) for l in range(self.predictor.n_layers - 1)]
+    ch, dims = self._choices, self.predictor.dims
+    sites = [(dims[0], self.input_dropout, ch.input_dropout_r)] + [(dims[l + 1], self.dropout, ch.dropout_r) for l in range(self.predictor.n_layers - 1)]
+    return _masks_of(self._rng, self.replicas, n, self.device, sites, 32)
 
   def _batch_of(self, state: Tensor, action: Tensor) -> TransitionBatch:
     R = self.replicas

@@ -7,8 +7,8 @@ graphs and replayed without host involvement. Replica r is a reference-equivalen
 (`per_replica={'seed': [...]}`, a seed sweep) replica r draws every random number as the single run with seed[r] does, so it is that run.
 
 `Trainer(per_replica={key: R values})` gives the replicas their own values of the shape-preserving hyper-parameters
-(config.VECTORISED, for GAIL the discriminator choices of config.PER_REPLICA_DISCRIMINATOR and its hidden size, config.PER_REPLICA_WIDTH, and
-the AdRIL / PWIL / DRIL keys of config.PER_REPLICA_ALGORITHM); `main` runs a multirun sweep (`-m key=a,b,...`) as groups of such Trainers, one replica block per job.
+(config.VECTORISED, for GAIL the discriminator choices of config.PER_REPLICA_DISCRIMINATOR and its hidden size, config.PER_REPLICA_WIDTH,
+the AdRIL / PWIL / DRIL keys of config.PER_REPLICA_ALGORITHM, and RED's / DRIL's dropout rates and activation, config.PER_REPLICA_DROPOUT); `main` runs a multirun sweep (`-m key=a,b,...`) as groups of such Trainers, one replica block per job.
 """
 from __future__ import annotations
 
@@ -23,7 +23,7 @@ import torch
 from torch import Tensor
 
 from . import _lib, distributed
-from .config import Config, SweepError, SweepJob, expand_sweep, get_key, load_config, needs_expert_memory, replica_values, split_per_replica, sweep_groups
+from .config import PER_REPLICA_DROPOUT, Config, SweepError, SweepJob, expand_sweep, get_key, load_config, needs_expert_memory, replica_values, split_per_replica, sweep_groups
 from .environments import D4RLEnv, ENVS
 from .evaluation import evaluate_agent
 from .memory import ReplayMemory, TransitionBatch
@@ -110,8 +110,15 @@ class Trainer:
       self.discriminator = GAILDiscriminator(S, A, cfg.imitation, cfg.reinforcement.discount, replicas=d_rep, rng=d_rng, device=dev, reward_function=None if fast_init else rf,
                                              spectral_norm=(any(sn) if fast_init else sn) if sn is not None else None, hidden_size=hw)
       if d_rng is not rng: torch.set_rng_state(d_rng.states[0])  # the global stream goes on as after a fast_init run of replica 0's width
-    elif self.algorithm == 'DRIL': self.discriminator = SoftActor(S, A, cfg.imitation.discriminator, replicas=nrep, rng=rng, device=dev)  # train.py:74
-    elif self.algorithm == 'RED': self.discriminator = REDDiscriminator(S, A, cfg.imitation, replicas=nrep, rng=rng, device=dev)  # train.py:82
+    elif self.algorithm in ('DRIL', 'RED'):
+      # per-replica activation / dropout rates (RED / DRIL sweeps): replica r is initialised with its own activation's gain (fast_init: every replica
+      # redraws from replica 0's stream with its own activation, as for GAIL widths; the rates change no draw)
+      drop = {k.rsplit('.', 1)[1]: pr[k] for k in PER_REPLICA_DROPOUT if k in pr}
+      d_rng, d_rep = rng, nrep
+      if fast_init and drop: d_rng, d_rep = ReplicaRNG.repeated(torch.get_rng_state(), R), R
+      if self.algorithm == 'DRIL': self.discriminator = SoftActor(S, A, cfg.imitation.discriminator, replicas=d_rep, rng=d_rng, device=dev, **drop)  # train.py:74
+      else: self.discriminator = REDDiscriminator(S, A, cfg.imitation, replicas=d_rep, rng=d_rng, device=dev, **drop)  # train.py:82
+      if d_rng is not rng: torch.set_rng_state(d_rng.states[0])
     # the dropout masks are keyed on models.default_rng.seed, which no run sets: single runs of any seed draw the same mask stream, and so do
     # the replicas of a seed sweep, each at its own local indices
     if self.algorithm in ('DRIL', 'RED'): self.discriminator.per_replica_masks = seeds is not None

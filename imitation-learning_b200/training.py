@@ -173,8 +173,10 @@ def behavioural_cloning_update(actor: SoftActor, expert_transition, actor_optimi
     need = _lib.lib().il_actor_dropout_workspace_bytes(C.byref(a.actor), R, batch.B)
     ws = _workspace(actor, 'bc_dropout', need, device)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-    _lib.check(_lib.lib().il_bc_update_dropout(_lib.handle(), C.byref(a), _lib.ptr(masks[0]), _lib.mask_array(masks[1:]), _lib.stream()))
+    act_r = getattr(getattr(actor, '_choices', None), 'act_r', None)
+    _lib.check(_lib.lib().il_bc_update_dropout(_lib.handle(), C.byref(a), _lib.ptr(masks[0]), _lib.mask_array(masks[1:]), _lib.stream(), _lib.ptr(act_r)))
     return
+  if getattr(actor, 'activation_r', None) is not None: raise NotImplementedError('per-replica activations run on the dropout program only')
   need = _lib.lib().il_bc_workspace_bytes(C.byref(a))
   ws = _workspace(actor, 'bc', need, device)
   a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()

@@ -197,18 +197,26 @@ int il_bc_update(il_handle* h, const il_bc_args* a, void* stream);
 /* ---- networks with dropout (models.py:48-69 with input_dropout / dropout > 0): DRIL's policy ensemble and RED's predictor -----------
  * Dropout masks are explicit inputs, pre-scaled {0, 1/(1-p)}: mask_in [R, n, dims[0]] for the input, mask_hid[l] [R, n, dims[l+1]] for hidden
  * layer l (applied BEFORE the activation, models.py:54-61); NULL = no dropout at that site. il_fill_dropout_mask draws them (Philox). */
-int il_fill_dropout_mask(il_handle* h, float* out, int64_t n, float p, uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream);
+/* p_r (optional [R] float32, per-replica rates in [0, 1), dropout-rate sweeps): out is [R, n / R] and element i takes the rate of its replica
+ * i / (n / R); every element draws the same Philox counter and lane as without p_r, so replica r's slice is the scalar call with p = p_r[r] over
+ * all n, restricted to that slice. NULL = p everywhere (R is then ignored). */
+int il_fill_dropout_mask(il_handle* h, float* out, int64_t n, float p, uint64_t seed, uint64_t stream_id, const uint64_t* counter, void* stream, const float* p_r,
+                         int R);
 /* Per-replica keys (see il_fill_normal_r): out [R, n_per_replica]; replica r is the il_fill_dropout_mask call over n_per_replica elements with
- * seed seed_r[r]; the caller advances the counter by ceil(n_per_replica / 4). */
+ * seed seed_r[r] (and rate p_r[r] when p_r is given); the caller advances the counter by ceil(n_per_replica / 4). */
 int il_fill_dropout_mask_r(il_handle* h, float* out, int R, int64_t n_per_replica, float p, const uint64_t* seed_r, uint64_t stream_id, const uint64_t* counter,
-                           void* stream);
+                           void* stream, const float* p_r);
 int64_t il_actor_dropout_workspace_bytes(const il_mlp* actor, int R, int n);
 /* SoftActor.log_prob(state, action) (models.py:97-99) of a dropout policy; rows of states / given_action are repeated `repeat` times
- * (torch.repeat_interleave of the 5-member MC-dropout ensemble, models.py:105): n = repeat * source rows. */
+ * (torch.repeat_interleave of the 5-member MC-dropout ensemble, models.py:105): n = repeat * source rows.
+ * activation_r (optional [R] int32 IL_ACT_*, activation sweeps): replica r's hidden layers use activation_r[r] instead of actor->activation, which
+ * is still validated; NULL = actor->activation for every replica. R <= IL_MAX_GRID_Y with activation_r. */
 int il_actor_log_prob_dropout(il_handle* h, const il_mlp* actor, int R, int n, int repeat, const float* states, int64_t states_rs, int ld_states, const float* given_action,
-                              const float* mask_in, const float* const* mask_hid, float* log_prob, void* workspace, int64_t workspace_bytes, void* stream);
-/* behavioural_cloning_update (training.py:57-64) of a dropout policy (train.py:120); workspace: il_actor_dropout_workspace_bytes(actor, R, B). */
-int il_bc_update_dropout(il_handle* h, const il_bc_args* a, const float* mask_in, const float* const* mask_hid, void* stream);
+                              const float* mask_in, const float* const* mask_hid, float* log_prob, void* workspace, int64_t workspace_bytes, void* stream,
+                              const int32_t* activation_r);
+/* behavioural_cloning_update (training.py:57-64) of a dropout policy (train.py:120); workspace: il_actor_dropout_workspace_bytes(actor, R, B).
+ * activation_r as in il_actor_log_prob_dropout. */
+int il_bc_update_dropout(il_handle* h, const il_bc_args* a, const float* mask_in, const float* const* mask_hid, void* stream, const int32_t* activation_r);
 /* DRIL reward (models.py:104-120): reward = +1 where the unbiased variance over the ensemble of exp(log_prob[r, b * ensemble + e]) is <= q, else -1;
  * variance (optional [R, B]) receives the raw uncertainty (set_uncertainty_threshold takes its quantile). reward may be NULL. */
 int il_dril_reward(il_handle* h, const float* log_prob, int R, int B, int ensemble, const float* q, int q_shared, float* reward, int64_t reward_rs, int reward_ld, float* variance,
@@ -220,6 +228,8 @@ typedef struct il_red {
   il_mlp  target;                   /* R nets, frozen random embedding (models.py:266-268) */
   float*  sigma;                    /* [R] sigma_1 (models.py:269,277-280) */
   int32_t state_only, _pad;
+  const int32_t* activation_r;      /* optional [R] IL_ACT_* (activation sweeps): replica r's predictor AND target use activation_r[r] in place of
+                                       predictor.activation / target.activation; NULL = those fields. R <= IL_MAX_GRID_Y with it. */
 } il_red;
 typedef struct il_red_update_args {
   il_red   disc;
