@@ -429,6 +429,8 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_kernel(const GailUpdPa
   // the replica index (order[blockIdx.x] in a width-class launch) and the pointers derived from it are re-derived from shared memory here:
   // kept live from the start in registers they cost the tiled variants spills
   const int rr = __float_as_int(s.scal[6]);
+  // PUGAIL with the clamp active: policy_loss = -margin (training.py:102); its gated terms were left out of loss_bce above
+  if (pu_gate == 0.f) loss_bce -= s.scal[4];
   if (tid == 0 && a.out_losses) { a.out_losses[rr * 2 + 0] = loss_bce; a.out_losses[rr * 2 + 1] = loss_gp; }
 
   // ---- AdamW (train.py:84; torch _single_tensor_adam) -----------------------------------------------------------
@@ -929,6 +931,8 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
   // the replica index (order[blockIdx.x] in a width-class launch) and the pointers derived from it are re-derived from shared memory here:
   // kept live from the start in registers they cost the tiled variants spills
   const int rr = __float_as_int(s.scal[6]);
+  // PUGAIL with the clamp active: policy_loss = -margin (training.py:102); its gated terms were left out of loss_bce above
+  if (pu_gate == 0.f) loss_bce -= s.scal[4];
   if (tid == 0 && a.out_losses) { a.out_losses[rr * 2 + 0] = loss_bce; a.out_losses[rr * 2 + 1] = loss_gp; }
 
   // ---- AdamW (train.py:84; torch _single_tensor_adam) -----------------------------------------------------------

@@ -233,7 +233,8 @@ __global__ void __launch_bounds__(256) gailx_loss_kernel(const LossParams p) {
     }
   }
   loss = block_sum(loss, red);
-  if (threadIdx.x == 0 && p.out_losses) p.out_losses[r * 2 + 0] = loss * invB;
+  const float margin = pu_gate == 0.f ? p.nonnegative_margin : 0.f;  // the clamp is active: policy_loss = -margin (training.py:102)
+  if (threadIdx.x == 0 && p.out_losses) p.out_losses[r * 2 + 0] = loss * invB - margin;
 }
 
 // ---- gradient penalty element-wise pieces -------------------------------------------------------------------------------------

@@ -47,6 +47,17 @@ CASES: Dict[str, dict] = {
                             lr=1e-3, wd=0.1, reward='GAIL', reward_shaping=False, subtract_log_policy=False, state_only=False),
   'gailx_state_only_sigmoid': dict(kind='gailx', S=18, A=6, H=32, depth=2, activation='sigmoid', B=48, steps=2, seed=38, spectral_norm=False, grad_penalty=0.0, entropy_bonus=0.1, loss='Mixup',
                                    lr=1e-3, wd=0.0, reward='FAIRL', reward_shaping=True, subtract_log_policy=False, state_only=True),
+  # the rest of the general program's branches: a linear g (depth 0) under the gradient penalty; PUGAIL with a finite margin whose clamp acts;
+  # a depth-2 tanh h under Mixup + gradient penalty + log-policy term; a depth-3 sigmoid g (the middle layers of the penalty's double backward)
+  'gailx_linear_gp': dict(kind='gailx', S=12, A=3, H=32, depth=0, activation='relu', B=48, steps=2, seed=391, spectral_norm=True, grad_penalty=1.0, entropy_bonus=0.0, loss='BCE',
+                          lr=1e-3, wd=0.1, reward='AIRL', reward_shaping=False, subtract_log_policy=False, state_only=False),
+  'gailx_pugail_margin': dict(kind='gailx', S=12, A=3, H=32, depth=1, activation='tanh', B=48, steps=2, seed=392, spectral_norm=True, grad_penalty=1.0, entropy_bonus=0.0,
+                              loss='PUGAIL', pos_class_prior=0.7, nonnegative_margin=0.05, lr=1e-3, wd=0.1, reward='GAIL', reward_shaping=False, subtract_log_policy=False,
+                              state_only=False),
+  'gailx_shaping_deep_mixup': dict(kind='gailx', S=12, A=3, H=32, depth=2, activation='tanh', B=48, steps=2, seed=393, spectral_norm=True, grad_penalty=1.0, entropy_bonus=0.05,
+                                   loss='Mixup', lr=1e-3, wd=0.1, reward='AIRL', reward_shaping=True, subtract_log_policy=True, state_only=False),
+  'gailx_depth3_sigmoid': dict(kind='gailx', S=18, A=6, H=32, depth=3, activation='sigmoid', B=48, steps=2, seed=394, spectral_norm=False, grad_penalty=0.5, entropy_bonus=0.1,
+                               loss='BCE', lr=1e-3, wd=0.0, reward='FAIRL', reward_shaping=False, subtract_log_policy=False, state_only=False),
   # SURVEY §8f row 2: expert-data ingest (environments.py:63-125) on a D4RL-shaped raw buffer — host logic, no CUDA
   'ingest_absorbing_sub4': dict(kind='ingest', cuda=False, obs=11, A=3, N=900, trajectories=4, subsample=4, absorbing=True, seed=71),
   'ingest_plain_all': dict(kind='ingest', cuda=False, obs=17, A=6, N=500, trajectories=0, subsample=1, absorbing=False, seed=72),
@@ -320,7 +331,7 @@ def run_port(name: str, inp: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
     for s in range(c['steps']):
       pol, exp = _batch_from(inp, f'p{s}_'), _batch_from(inp, f'e{s}_')
       port.gail_update(disc, opt, pol, exp, _t(inp[f's{s}_eps_gp']), loss_function=c['loss'], grad_penalty=c['grad_penalty'], entropy_bonus=c['entropy_bonus'],
-                       eps_mixup=_t(inp[f's{s}_eps_mix']), actor=actor)
+                       pos_class_prior=c.get('pos_class_prior', 0.7), nonnegative_margin=c.get('nonnegative_margin', float('inf')), eps_mixup=_t(inp[f's{s}_eps_mix']), actor=actor)
       with torch.no_grad():
         lp = port.actor_log_prob(actor, pol['states'], pol['actions']) if actor is not None else None
         out[f's{s}_reward'] = _np(disc.predict_reward(pol['states'], pol['actions'], pol['next_states'], pol['terminals'], lp))
@@ -539,7 +550,7 @@ def run_reference(name: str, inp: Dict[str, np.ndarray]) -> Dict[str, np.ndarray
   elif k == 'gailx':
     S, A, H = c['S'], c['A'], c['H']
     icfg = DC(state_only=c['state_only'], spectral_norm=c['spectral_norm'], loss_function=c['loss'], grad_penalty=c['grad_penalty'], mixup_alpha=1, entropy_bonus=c['entropy_bonus'],
-              pos_class_prior=0.7, nonnegative_margin=float('inf'),
+              pos_class_prior=c.get('pos_class_prior', 0.7), nonnegative_margin=c.get('nonnegative_margin', float('inf')),
               discriminator=DC(hidden_size=H, depth=c['depth'], activation=c['activation'], input_dropout=0.5, dropout=0.75, reward_shaping=c['reward_shaping'],
                                subtract_log_policy=c['subtract_log_policy'], reward_function=c['reward']))
     disc = ref.models.GAILDiscriminator(S, A, icfg, 0.97)

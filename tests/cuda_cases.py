@@ -139,7 +139,7 @@ def run_cuda(name, inps):
   elif k == 'gailx':  # reward shaping / subtract_log_policy / depth 2 / tanh / sigmoid / state-only (models.py:157-175) on the general CUDA path
     S, A, H = c['S'], c['A'], c['H']
     icfg = Cfg(state_only=c['state_only'], spectral_norm=c['spectral_norm'], loss_function=c['loss'], grad_penalty=c['grad_penalty'], mixup_alpha=1, entropy_bonus=c['entropy_bonus'],
-               pos_class_prior=0.7, nonnegative_margin=float('inf'),
+               pos_class_prior=c.get('pos_class_prior', 0.7), nonnegative_margin=c.get('nonnegative_margin', float('inf')),
                discriminator=Cfg(hidden_size=H, depth=c['depth'], activation=c['activation'], input_dropout=0.5, dropout=0.75, reward_shaping=c['reward_shaping'],
                                  subtract_log_policy=c['subtract_log_policy'], reward_function=c['reward']))
     disc = il_b200.GAILDiscriminator(S, A, icfg, 0.97, replicas=R)

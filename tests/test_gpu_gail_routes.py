@@ -36,7 +36,8 @@ ENV = {'hopper': (12, 3), 'halfcheetah': (18, 6), 'ant': (112, 8)}  # state (wit
 LR, WD, BETAS, ADAM_EPS, PRIOR = 1e-3, 0.1, (0.9, 0.999), 1e-8, 0.7
 KINK, CLAMP_GAP = 1e-4, 1e-3
 DEV = 'cuda'
-LOSSES = ('BCE', 'PUGAIL', 'PUGAIL0', 'Mixup')  # PUGAIL: margin inf; PUGAIL0: margin 0, where the clamp is active
+LOSSES = ('BCE', 'PUGAIL', 'PUGAIL0', 'Mixup', 'PUGAILm')  # PUGAIL: margin inf; PUGAIL0: margin 0 and PUGAILm: margin 0.05, where the clamp is active
+MARGIN = {'PUGAIL': float('inf'), 'PUGAIL0': 0.0, 'PUGAILm': 0.05}
 TICK = 'gail_tick_kernel'
 REW_TILED, REW = 'gail_reward_tiled_kernel', 'gail_reward_kernel'
 
@@ -70,11 +71,12 @@ def rew(kernel, env, H, B, rf='AIRL', sn=True, ld=1, order=False, tiled_on=1):
 
 
 PRODUCT = list(product(LOSSES, (0.0, 1.0), (0.0, 0.05), (False, True)))  # loss x gradient penalty x entropy bonus x spectral norm
+SPREAD = PRODUCT[:32]  # the first four losses: the spread of the rows outside the full product predates PUGAILm
 
 
 def _opts(i):
   """A spread of the option product for the rows outside the two full-product routes."""
-  loss, gp, ent, sn = PRODUCT[(11 * i + 5) % len(PRODUCT)]
+  loss, gp, ent, sn = SPREAD[(11 * i + 5) % len(SPREAD)]
   return dict(loss=loss, gp=gp, ent=ent, sn=sn)
 
 
@@ -261,7 +263,7 @@ def port_update(p, inp, r, dtype):
   disc = _port_disc(inp.params[r], inp.sn[r], p['sn'], p['state_only'], 'AIRL', dtype)
   pol, exp = (inp.fields(x[r].to(dtype), S, A) for x in (inp.pol, inp.exp))
   loss = 'PUGAIL' if p['loss'].startswith('PUGAIL') else p['loss']
-  margin = 0.0 if p['loss'] == 'PUGAIL0' else float('inf')
+  margin = MARGIN.get(p['loss'], float('inf'))
   out = port.gail_update(disc, _GradOnly(), pol, exp, inp.eps_gp[r].to(dtype) if p['gp'] > 0 else None, loss_function=loss, grad_penalty=p['gp'],
                          entropy_bonus=p['ent'], pos_class_prior=PRIOR, nonnegative_margin=margin,
                          eps_mixup=inp.eps_mix[r].to(dtype) if loss == 'Mixup' else None)
@@ -357,7 +359,7 @@ class Device:
     a.eps_mix = self.eps_mix.data_ptr() if eps_mix and loss == 'Mixup' else None
     a.R, a.loss_function, a.training = R, _lib.LOSS['PUGAIL' if loss.startswith('PUGAIL') else loss], 1
     a.grad_penalty, a.entropy_bonus, a.pos_class_prior = p['gp'], p['ent'], PRIOR
-    a.nonnegative_margin = 0.0 if loss == 'PUGAIL0' else float('inf')
+    a.nonnegative_margin = MARGIN.get(loss, float('inf'))
     a.out_losses = self.losses.data_ptr()
     return a
 
@@ -428,9 +430,9 @@ def _prepare_update(p, inp, active):
   for r in active:
     for z, _, _ in inp.forwards(p, r): assert z.abs().min() >= KINK, 'a hidden pre-activation at the ReLU kink'
     if p['loss'].startswith('PUGAIL'):
-      inner, margin = inp.pugail_inner(p, r), (0.0 if p['loss'] == 'PUGAIL0' else float('inf'))
+      inner, margin = inp.pugail_inner(p, r), MARGIN[p['loss']]
       assert abs(inner + margin) > CLAMP_GAP, f'replica {r}: PUGAIL clamp {inner:.3e} within {CLAMP_GAP} of -margin: change the seed'
-      if p['loss'] == 'PUGAIL0': assert inner < -margin, f'replica {r}: the clamp is not active ({inner:.3e}): change the seed'
+      if margin < float('inf'): assert inner < -margin, f'replica {r}: the clamp is not active ({inner:.3e}): change the seed'
 
 
 def _seed(p): return p['S'] * 7919 + p['A'] * 131 + p['H'] * 17 + p['B'] + 3 * LOSSES.index(p.get('loss', 'BCE')) + int(p['sn'])
