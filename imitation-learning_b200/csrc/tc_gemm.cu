@@ -8,36 +8,48 @@
 //
 // Structure: persistent CTAs, one per SM, each walking the 128 x 256 output tiles blockIdx.x, blockIdx.x + gridDim.x, ...
 // (the two M-tiles of a group run in the same wave, so the second read of B hits L2). The CTA is warp-specialised:
-//   - warpgroup 0, the producer (56 registers per thread after setmaxnreg.dec; 72 with FUSE), copies and splits;
-//   - warpgroups 1 and 2, the consumers (224 registers after setmaxnreg.inc; 216 with FUSE), only multiply and run the
-//     epilogue. Consumer w owns rows [64 w, 64 w + 64) of the tile as the 128 fp32 accumulator registers per thread of
-//     wgmma.mma_async m64n256k8.tf32.
-// wgmma reads 32-bit operands from shared memory in K-major layout only, and every operand needs the hi/lo split (a
-// CUDA-core pass) anyway, so each k-block (16 floats of k) of the CTA's k-block stream (which runs on across tile
-// boundaries) goes through three steps, all running at once on different k-blocks:
-//   1. copy (producer): cp.async 16-byte copies of the raw fp32 chunks global -> a RAW_STAGES-deep shared-memory ring,
-//      no registers held. Each producer thread reads back exactly the chunks it copied, so cp.async.wait_group is all
-//      the visibility the raw ring needs: no mbarrier (cp.async.mbarrier.arrive) and no TMA, which could not feed the
-//      tensor core anyway because the split has to see every element;
-//   2. split (producer): the hi and lo tiles go into one of three hi/lo stages in the canonical K-major SWIZZLE_64B
-//      layout. Operands stored [K, rows] in global memory are transposed on the way: a thread splits a 4 (k) x 4 (rows)
-//      block and stores four 16-byte k-chunks, in a per-thread rotated order that keeps the shared-memory stores
-//      conflict-free. With FUSE the A chunks are computed (the first MLP layer) instead of copied;
-//   3. multiply (consumers): the 6 (3xTF32) or 2 (TF32) wgmmas of the k-block per consumer warpgroup.
+//   - warpgroup 0, the producer (56 registers per thread after setmaxnreg.dec; 72 with FUSE), copies A and B and splits B;
+//   - warpgroups 1 and 2, the consumers (224 registers after setmaxnreg.inc; 216 with FUSE), split their A in registers,
+//     multiply and run the epilogue. Consumer w owns rows [64 w, 64 w + 64) of the tile as the 128 fp32 accumulator
+//     registers per thread of wgmma.mma_async m64n256k8.tf32.
+// wgmma reads B from shared memory in K-major layout only and A either from there or from registers, and every operand
+// needs the hi/lo split (a CUDA-core pass) anyway. Each A row is read by one consumer warpgroup only, so the consumers
+// split A in their own registers and only B goes through shared-memory hi/lo tiles. Each k-block (16 floats of k) of the
+// CTA's k-block stream (which runs on across tile boundaries) goes through three steps, all running at once on
+// different k-blocks:
+//   1. copy (producer): cp.async 16-byte copies of the raw fp32 chunks global -> shared memory, no registers held. B
+//      goes to a RAW_STAGES-deep raw ring; each producer thread reads back exactly the B chunks it copied, so
+//      cp.async.wait_group is all the visibility that ring needs (no TMA, which could not feed the tensor core anyway
+//      because the split has to see every element). A goes straight to an A_STAGES-deep ring in the layout the
+//      consumers read (see A_STAGES); with FUSE the producer computes the A chunks (the first MLP layer) into it instead;
+//   2. split (producer): B's hi and lo tiles go into one of three hi/lo stages in the canonical K-major SWIZZLE_64B
+//      layout. A B stored [K, rows] in global memory is transposed on the way: a thread splits a 4 (k) x 4 (rows) block
+//      and stores four 16-byte k-chunks, in a per-thread rotated order that keeps the shared-memory stores conflict-free;
+//   3. multiply (consumers): each consumer warpgroup loads the raw A fragments of its rows (ldmatrix or 32-bit loads,
+//      conflict-free), splits them in registers and issues the 6 (3xTF32) or 2 (TF32) wgmmas of the k-block, A from
+//      registers and B from the stage. The products, their hi/lo values and their order are the same as with both
+//      operands in shared memory, so the results are too, bit for bit.
 // The stages hand over through full / empty mbarrier pairs with phase bits; the k loop has no CTA barrier. The producer
 // waits for stage q % 3 to be empty, splits k-block q into it, fences the generic-proxy stores to the async proxy and
-// arrives on its full barrier. A consumer waits for the full barrier, issues the wgmmas of q, wgmma.wait_group 1 (the
-// wgmmas of q - 1 are done) and arrives on the empty barrier of q - 1's stage. The producer runs up to three k-blocks
-// ahead, so while the consumers run a tile's epilogue it splits the next tile's first k-blocks.
+// arrives on its full barrier. A consumer waits for the full barrier, loads and splits A, issues the wgmmas of q,
+// wgmma.wait_group 1 (the wgmmas of q - 1 are done) and arrives on the empty barrier of q - 1's stage. The producer runs
+// up to three k-blocks ahead, so while the consumers run a tile's epilogue it splits the next tile's first k-blocks.
+// Shared-memory traffic per k-block in 3xTF32 (counted from the code): cp.async writes 24 KB (A 8, B 16), producer reads
+// of raw B 16 KB, B hi/lo stores 32 KB, consumer reads of raw A 8 KB, wgmma B operand reads 96 KB (2 warpgroups x 2 k8 x
+// 3 MMAs x 8 KB): 176 KB. With A split by the producer too it was 216 KB (A read back, A hi/lo stores 16 KB, A operand
+// reads 24 KB), more than the 12 MMAs of the k-block take at the data-sheet tf32 rate.
 // The epilogue works on the accumulator fragments in registers (bias / activation / activation-derivative mask /
 // fused final linear layer, reduced over the four lanes that share a row) and stores 8-byte pairs; the four lanes of a
 // row fill one 32-byte sector. The fused-head bias and weights are staged by the consumers behind a named barrier of
 // their 256 threads.
 // The k loop never writes the accumulators outside wgmma (they are zeroed before it and read after it), so ptxas adds no
 // wgmma wait of its own and the loop's only wait is wait_group 1.
-// Measured on an H100 80GB HBM3 (SXM, 700 W, 1980 MHz): 3xTF32 256 x 256 x 256 with G = 2048 takes 0.82-0.86 ms per
-// layout (0.48 ms floor at data-sheet rates; the single-role loop this replaced, with a CTA barrier per k-block, took
-// 0.88-0.91 ms). See DESIGN.md §3.
+// ptxas (sm_90a): every variant runs its producer at 56 registers (FUSE 72) and its consumers at 224 (FUSE 216), no
+// spills, no wgmma serialisation remark (C7513 / C7517). -Xptxas -v prints eight informational C7519 remarks per variant
+// ("warpgroup.arrive is injected ... to allow use of registers in GMMA"), four per k-block of the two-way unrolled loop.
+// Measured on an H100 80GB HBM3 (SXM, 700 W, 1980 MHz): 3xTF32 256 x 256 x 256 with G = 2048 takes 0.72-0.78 ms per
+// layout (0.48 ms floor at data-sheet rates; 0.81-0.84 ms with A split by the producer through shared memory). See
+// DESIGN.md §3.
 #include "common.cuh"
 #include <cstdio>
 #include <cstdlib>
@@ -55,11 +67,21 @@ constexpr int producer_regs(bool fuse) { return fuse ? 72 : 56; }
 constexpr int consumer_regs(bool fuse) { return (THREADS * LAUNCH_REGS - PRODUCER_THREADS * producer_regs(fuse)) / CONSUMER_THREADS; }
 static_assert(THREADS * LAUNCH_REGS <= 65536 && consumer_regs(false) % 8 == 0 && consumer_regs(true) % 8 == 0, "tc_gemm: setmaxnreg split");
 constexpr int CONSUMER_BAR = 1, PRODUCER_BAR = 2;                   // named barriers (0 is __syncthreads)
-constexpr int A_BYTES = BM * BK * 4, B_BYTES = BN * BK * 4;          // 8 KB / 16 KB per k-block (hi or lo copy)
-constexpr int A_HI = 0, A_LO = A_BYTES, B_HI = 2 * A_BYTES, B_LO = 2 * A_BYTES + B_BYTES;
-constexpr int STAGE_BYTES = 2 * (A_BYTES + B_BYTES);                 // 48 KB hi/lo stage
+constexpr int A_BYTES = BM * BK * 4, B_BYTES = BN * BK * 4;          // 8 KB / 16 KB per k-block (raw A; B hi or lo copy)
+constexpr int B_HI = 0, B_LO = B_BYTES;
+constexpr int STAGE_BYTES = 2 * B_BYTES;                             // 32 KB hi/lo stage of B
 constexpr int N_STAGES = 3;                                          // hi/lo stages: the producer splits up to two k-blocks ahead of the wgmmas in flight
-constexpr int RAW_STAGES = 3;                                        // raw ring: k-blocks in flight global -> shared memory
+constexpr int RAW_STAGES = 3;                                        // raw B ring: k-blocks in flight global -> shared memory
+// A ring: raw fp32 A of a k-block, which the consumers load into wgmma register fragments and split there. The producer
+// copies k-block q into slot q % A_STAGES (FUSE: computes it there) no earlier than its iteration q - RAW_STAGES, after
+// waiting for the empty phase of k-block q - A_STAGES's stage; the consumers arrive on that phase only after loading
+// the A fragments of k-block q - A_STAGES, the slot's previous content. So the stage barriers guard the A slots too, and
+// the raw A is visible to the consumers through the full barrier of its k-block, like the hi/lo stage.
+constexpr int A_STAGES = N_STAGES + RAW_STAGES;
+// [rows, K] A: SWIZZLE_64B layout (A_BYTES). [K, rows] A: 16 k-rows of BM floats padded to A_T_LD, so that the k values
+// t, t + 4 of a fragment load (t = lane % 4) fall 8 banks apart. FUSE computes [rows, K] A only.
+constexpr int A_T_LD = BM + 8, A_T_BYTES = BK * A_T_LD * 4;
+constexpr int a_slot_bytes(bool fuse) { return fuse ? A_BYTES : A_T_BYTES; }
 constexpr int HEAD_MAX = 8;                                          // fused head: up to 8 output units (N = 1 critic, 2A <= 8 actor)
 constexpr int HEAD_BYTES = (BN + HEAD_MAX * BN) * 4;                 // bias [256] + head weights [8][256]
 // FUSE: the A operand is not loaded but COMPUTED — the previous (first) MLP layer relu(X W1^T + b1) with K0 <= 16 input
@@ -67,11 +89,8 @@ constexpr int HEAD_BYTES = (BN + HEAD_MAX * BN) * 4;                 // bias [25
 // round-trips HBM. W1 [256][16] (zero padded), b1 [256] and the tile's input rows [128][16] are staged once per tile.
 constexpr int L1_MAXK = 16, L1_ROWS = 256;
 constexpr int L1_W_BYTES = L1_ROWS * L1_MAXK * 4, L1_B_BYTES = L1_ROWS * 4, L1_X_BYTES = BM * L1_MAXK * 4;
-// raw ring slot: A (8 KB, absent with FUSE, which computes A) then B (16 KB)
-constexpr int raw_a_bytes(bool fuse) { return fuse ? 0 : A_BYTES; }
-constexpr int raw_bytes(bool fuse) { return raw_a_bytes(fuse) + B_BYTES; }
-constexpr int RAW_OFF = N_STAGES * STAGE_BYTES;
-constexpr int head_off(bool fuse) { return RAW_OFF + RAW_STAGES * raw_bytes(fuse); }
+constexpr int RAW_OFF = N_STAGES * STAGE_BYTES, A_OFF = RAW_OFF + RAW_STAGES * B_BYTES;
+constexpr int head_off(bool fuse) { return A_OFF + A_STAGES * a_slot_bytes(fuse); }
 constexpr int l1_off(bool fuse) { return head_off(fuse) + HEAD_BYTES; }
 // The full / empty mbarrier pairs of the hi/lo stages sit in the BAR_BYTES just below the 512-byte aligned base (SWIZZLE_64B
 // repeats every 512 bytes); with dynamic shared memory at least 16-byte aligned, barriers plus alignment take at most
@@ -107,8 +126,10 @@ template <int R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
-// D (64 x 256, fp32, 128 registers per thread) += A (64 x 8, K-major in shared memory) * B (8 x 256, K-major in shared memory)
-__device__ __forceinline__ void wgmma_tf32(float (&d)[128], uint64_t a_desc, uint64_t b_desc) {
+// D (64 x 256, fp32, 128 registers per thread) += A (64 x 8, registers) * B (8 x 256, K-major in shared memory). The A
+// fragment of warp w of the warpgroup, lane (g = lane / 4, t = lane % 4): a[0] = A[16 w + g][t], a[1] = A[16 w + g + 8][t],
+// a[2] = A[16 w + g][t + 4], a[3] = A[16 w + g + 8][t + 4]. The registers must not change until the wgmma is complete.
+__device__ __forceinline__ void wgmma_tf32(float (&d)[128], const uint32_t (&a)[4], uint64_t b_desc) {
   asm volatile(
       "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {"
       "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
@@ -119,7 +140,7 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[128], uint64_t a_desc, uin
       "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
       "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
       "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127 "
-      "}, %128, %129, 1, 1, 1;"
+      "}, {%128, %129, %130, %131}, %132, 1, 1, 1;"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
         "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
@@ -136,7 +157,7 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[128], uint64_t a_desc, uin
         "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
         "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
         "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-      : "l"(a_desc), "l"(b_desc));
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc));
 }
 // Shared-memory matrix descriptor of a K-major SWIZZLE_64B tile: start >> 4 | LBO >> 4 at bit 16 (unused by swizzled K-major
 // layouts) | SBO >> 4 at bit 32 (512 B: the next 8-row atom) | layout type at bit 62 (2 = SWIZZLE_64B).
@@ -154,8 +175,24 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
   asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
   return v;
 }
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+// four 8 x 4 tiles of 32-bit words (8 x 8 of b16): lane l gives the address of row l % 8 of tile l / 8 and receives word
+// l % 4 of row l / 4 of tile j in v[j]
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&v)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(addr));
+}
 __device__ __forceinline__ uint32_t hi_of(uint32_t x) { return x & 0xFFFFE000u; }
 __device__ __forceinline__ uint32_t lo_of(uint32_t x) { return __float_as_uint(__uint_as_float(x) - __uint_as_float(x & 0xFFFFE000u)); }
+// hi_of and lo_of of a wgmma register operand, as one volatile asm: it stays where it is written, ahead of the
+// wgmma.fence, instead of being sunk between the wgmmas (a definition of a wgmma input register inside the wgmma
+// pipeline makes ptxas serialise the wgmmas)
+__device__ __forceinline__ void split_reg(uint32_t x, uint32_t& hi, uint32_t& lo) {
+  asm volatile("and.b32 %0, %2, 0xFFFFE000;\n\tsub.f32 %1, %2, %0;" : "=&r"(hi), "=r"(lo) : "r"(x));
+}
 // one 16-byte chunk (4 consecutive k of one row) into the hi tile and, for 3xTF32, the lo tile at the same offset
 __device__ __forceinline__ void store_chunk(uint32_t hi_tile, uint32_t lo_tile, uint32_t off, uint4 v, bool split) {
   sts128(hi_tile + off, hi_of(v.x), hi_of(v.y), hi_of(v.z), hi_of(v.w));
@@ -198,10 +235,11 @@ __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + BAR_BYTES + 511) & ~(uintptr_t)511);
   float* head_s = reinterpret_cast<float*>(smem + head_off(FUSE));  // [BN] bias then [HEAD_MAX][BN] head weights
-  const uint32_t stage0 = smem_u32(smem), raw0 = stage0 + RAW_OFF;
+  const uint32_t stage0 = smem_u32(smem), raw0 = stage0 + RAW_OFF, a0s = stage0 + A_OFF;
   const uint32_t full0 = stage0 - BAR_BYTES, empty0 = full0 + N_STAGES * 8;  // mbarriers of hi/lo stage s: full0 + 8 s, empty0 + 8 s
   const uint32_t w1s = stage0 + l1_off(FUSE), b1s = w1s + L1_W_BYTES, xs = b1s + L1_B_BYTES;
-  constexpr uint32_t RAW_A = 0, RAW_B = raw_a_bytes(FUSE), RAW_BYTES = raw_bytes(FUSE);
+  auto a_slot = [&](int q) { return a0s + (uint32_t)(q % A_STAGES) * (uint32_t)a_slot_bytes(FUSE); };
+  const bool a_km = FUSE || p.g.a_kmajor != 0;  // A stored [rows, K] (else [K, rows])
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
   const GemmArgs& g = p.g;
@@ -222,51 +260,55 @@ __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
   if (wg == 0) {
     // ================= producer warpgroup: copy and split the k-block stream =================
     setmaxnreg_dec<producer_regs(FUSE)>();
-    const bool a_km = FUSE || g.a_kmajor != 0, b_km = g.b_kmajor != 0, split = p.split != 0;
+    const bool b_km = g.b_kmajor != 0, split = p.split != 0;
     // Per-thread chunks of one k-block, in a map of 256 slots: producer thread pt works slots v = pt and v = pt + 128.
     // stored [rows, K]: 16-byte chunk fc of rows fr + 64 j (A: j < 2, B: j < 4), fr = v / 4, fc = v % 4
-    // stored [K, rows]: 4 x 4 blocks, rows 4 c4 .. 4 c4 + 3 at k = 4 kg .. 4 kg + 3 (A: 128 blocks in slots v < 128, B: 256 blocks)
-    // Slot v's chunk j sits at (256 j + v) * 16 of its operand's region in the raw slot: the copies and the reads back of a
-    // warp are 512 contiguous bytes. A thread reads back exactly the chunks it copied, so cp.async.wait_group is all the
-    // visibility the raw ring needs (no mbarrier, no barrier of the warpgroup).
+    // stored [K, rows]: B: 4 x 4 blocks, rows 4 c4 .. 4 c4 + 3 at k = 4 kg .. 4 kg + 3; A: in slots v < 128, the chunks
+    //                   of rows 4 c4 .. 4 c4 + 3 at k = 4 kg .. 4 kg + 3 (c4 = v % 32, kg = v / 32)
+    // B: slot v's chunk j sits at (256 j + v) * 16 of the raw B slot, so the copies and the reads back of a warp are 512
+    // contiguous bytes. A thread reads back exactly the B chunks it copied, so cp.async.wait_group is all the visibility
+    // the raw B ring needs (no mbarrier, no barrier of the warpgroup). A: copied straight into the consumers' layout
+    // (SWIZZLE_64B, or k-rows of A_T_LD floats) and never read back by the producer.
     constexpr int MAP = 2 * PRODUCER_THREADS;
     const int pt = tid;
 
-    auto copy_kb = [&](int q) {  // k-block q of the stream: raw chunks global -> raw slot q % RAW_STAGES; always one commit group
+    auto copy_kb = [&](int q) {  // k-block q of the stream: raw chunks global -> raw B slot q % RAW_STAGES and A slot q % A_STAGES; always one commit group
       if (q < nq) {
         const int t = tile_of(q / nkb), kb = q % nkb, grp = t / tiles_m, m0 = (t % tiles_m) * BM;
         const float* A = g.A + (int64_t)(grp / g.a_gdiv) * g.a_gs;
         const float* Bg = g.B + (int64_t)(grp / g.b_gdiv) * g.b_gs;
+        const uint32_t as = a_slot(q);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int v = pt + h * PRODUCER_THREADS, fr = v >> 2, fc = v & 3;
-          const uint32_t raw = raw0 + (uint32_t)(q % RAW_STAGES) * RAW_BYTES + (uint32_t)v * 16u;
+          const uint32_t raw = raw0 + (uint32_t)(q % RAW_STAGES) * B_BYTES + (uint32_t)v * 16u;
           if (!FUSE) {
             if (a_km) {
               const float* src = A + (int64_t)(m0 + fr) * g.lda + kb * BK + fc * 4;
-              cp_async16(raw + RAW_A, src);
-              cp_async16(raw + RAW_A + MAP * 16, src + (int64_t)64 * g.lda);
+              cp_async16(as + sw64(fr, fc), src);
+              cp_async16(as + sw64(fr, fc) + 4096u, src + (int64_t)64 * g.lda);  // rows fr + 64: 8 atoms further
             } else if (h == 0) {
-              const float* src = A + (int64_t)(kb * BK + ((v >> 5) & 3) * 4) * g.lda + m0 + (v & 31) * 4;
+              const int c4 = v & 31, kg = v >> 5;
+              const float* src = A + (int64_t)(kb * BK + kg * 4) * g.lda + m0 + c4 * 4;
 #pragma unroll
-              for (int k = 0; k < 4; ++k) cp_async16(raw + RAW_A + k * (MAP / 2) * 16, src + (int64_t)k * g.lda);
+              for (int k = 0; k < 4; ++k) cp_async16(as + (uint32_t)(((kg * 4 + k) * A_T_LD + c4 * 4) * 4), src + (int64_t)k * g.lda);
             }
           }
           const float* src = b_km ? Bg + (int64_t)fr * g.ldb + kb * BK + fc * 4 : Bg + (int64_t)(kb * BK + (v >> 6) * 4) * g.ldb + (v & 63) * 4;
           const int64_t step = b_km ? (int64_t)64 * g.ldb : (int64_t)g.ldb;  // next chunk j: 64 rows further / the next k
 #pragma unroll
-          for (int j = 0; j < 4; ++j) cp_async16(raw + RAW_B + j * MAP * 16, src + j * step);
+          for (int j = 0; j < 4; ++j) cp_async16(raw + j * MAP * 16, src + j * step);
         }
       }
       cp_async_commit();
     };
 
-    auto split_kb = [&](int q, int s) {  // k-block q: split the raw chunks this thread copied (FUSE: compute the A chunks) into hi/lo stage s
+    auto split_kb = [&](int q, int s) {  // k-block q: split the raw B chunks this thread copied into hi/lo stage s (FUSE: and compute the A chunks into A slot q)
       const uint32_t st = stage0 + (uint32_t)s * STAGE_BYTES;
 #pragma unroll(FUSE ? 1 : 2)  // the first-layer evaluation of both slots at once would not fit the producer's registers
       for (int h = 0; h < 2; ++h) {
         const int v = pt + h * PRODUCER_THREADS, fr = v >> 2, fc = v & 3;
-        const uint32_t raw = raw0 + (uint32_t)(q % RAW_STAGES) * RAW_BYTES + (uint32_t)v * 16u;
+        const uint32_t raw = raw0 + (uint32_t)(q % RAW_STAGES) * B_BYTES + (uint32_t)v * 16u;
         const uint32_t km_off = sw64(fr, fc);  // rows fr + 64 j: + j * 4096 bytes (64 rows = 8 atoms)
         if (FUSE) {
           // A chunk values: relu(b1[k] + sum_j x[j] W1[k][j]) for k = 16 kb + 4 fc + {0..3}, rows fr and fr + 64
@@ -291,30 +333,23 @@ __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
           }
           const uint4 a0 = make_uint4(__float_as_uint(fmaxf(c0[0], 0.f)), __float_as_uint(fmaxf(c0[1], 0.f)), __float_as_uint(fmaxf(c0[2], 0.f)), __float_as_uint(fmaxf(c0[3], 0.f)));
           const uint4 a1 = make_uint4(__float_as_uint(fmaxf(c1[0], 0.f)), __float_as_uint(fmaxf(c1[1], 0.f)), __float_as_uint(fmaxf(c1[2], 0.f)), __float_as_uint(fmaxf(c1[3], 0.f)));
-          store_chunk(st + A_HI, st + A_LO, km_off, a0, split);
-          store_chunk(st + A_HI, st + A_LO, km_off + 4096u, a1, split);
+          const uint32_t as = a_slot(q);  // raw, like a copied A: the consumers split it
+          sts128(as + km_off, a0.x, a0.y, a0.z, a0.w);
+          sts128(as + km_off + 4096u, a1.x, a1.y, a1.z, a1.w);
           if (p.l1.store) {  // the first hidden activation, for the backward pass
             const int t = tile_of(q / nkb);
             float* hs = p.l1.store + (int64_t)(t / tiles_m) * p.l1.store_gs + (int64_t)((t % tiles_m) * BM + fr) * g.K + k0;
             *reinterpret_cast<uint4*>(hs) = a0;
             *reinterpret_cast<uint4*>(hs + (int64_t)64 * g.K) = a1;
           }
-        } else if (a_km) {
-          store_chunk(st + A_HI, st + A_LO, km_off, lds128(raw + RAW_A), split);
-          store_chunk(st + A_HI, st + A_LO, km_off + 4096u, lds128(raw + RAW_A + MAP * 16), split);
-        } else if (h == 0) {
-          uint4 va[4];
-#pragma unroll
-          for (int k = 0; k < 4; ++k) va[k] = lds128(raw + RAW_A + k * (MAP / 2) * 16);
-          store_block_t(st + A_HI, st + A_LO, v & 31, (v >> 5) & 3, va, split);
         }
         if (b_km) {
 #pragma unroll
-          for (int j = 0; j < 4; ++j) store_chunk(st + B_HI, st + B_LO, km_off + (uint32_t)j * 4096u, lds128(raw + RAW_B + j * MAP * 16), split);
+          for (int j = 0; j < 4; ++j) store_chunk(st + B_HI, st + B_LO, km_off + (uint32_t)j * 4096u, lds128(raw + j * MAP * 16), split);
         } else {
           uint4 vb[4];
 #pragma unroll
-          for (int k = 0; k < 4; ++k) vb[k] = lds128(raw + RAW_B + k * MAP * 16);
+          for (int k = 0; k < 4; ++k) vb[k] = lds128(raw + k * MAP * 16);
           store_block_t(st + B_HI, st + B_LO, v & 63, v >> 6, vb, split);
         }
       }
@@ -369,42 +404,77 @@ __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(const TcParams p) {
   }
 
   // ================= consumer warpgroups 1 and 2: wgmma and the epilogue =================
-  // Consumer warpgroup cw owns rows [64 cw, 64 cw + 64) of the tile. Per k-block: wait until its stage is full, issue
-  // the wgmmas, wgmma.wait_group 1 (the wgmmas of the previous k-block are done) and release that previous stage.
+  // Consumer warpgroup cw owns rows [64 cw, 64 cw + 64) of the tile. Per k-block: wait until its stage is full, load the
+  // raw A fragments of its rows from the A slot and split them in registers, issue the wgmmas (A from registers, B from
+  // the hi/lo stage), wgmma.wait_group 1 (the wgmmas of the previous k-block are done) and release that previous stage.
+  // A register operand must not change while its wgmma is in flight, so consecutive k-blocks use the two fragment sets
+  // af[0] and af[1] in turn (the k loop is unrolled by two). In the SASS ptxas folds most of the second set onto the
+  // first: the runtime `split` branch ends each k-block in four gsb0-terminated HGMMA chains, and wait_group 1 leaves
+  // only the last (hi x hi of the second k8) in flight, so only its hi registers get a separate copy. It also means
+  // only about one of a k-block's six MMAs overlaps the issue of the next k-block.
   // The k loop never writes the accumulators outside wgmma (they are zeroed before it and read after it), so nothing in
   // it makes ptxas wait for the wgmmas in flight.
   setmaxnreg_inc<consumer_regs(FUSE)>();
   const int cw = wg - 1, ct = tid - PRODUCER_THREADS;
-  const uint64_t a_desc0 = make_desc(stage0 + (uint32_t)cw * 4096u), b_desc0 = make_desc(stage0);  // this warpgroup's 64 rows of A
+  const uint64_t b_desc0 = make_desc(stage0);
   const bool split = p.split != 0;
+  // Per-thread offsets of the A fragment inside an A slot (rows of this warp: 64 cw + 16 (warp % 4) + {g, g + 8}).
+  // [rows, K]: two ldmatrix.x4 per k-block, one per k8 kk; tile j = lane / 8 is rows + 8 (j % 2) at chunk 2 kk + j / 2, so
+  // v[j] is the fragment's a[j]. The 8 rows of a tile sit in 8 distinct 16-byte bank groups (SWIZZLE_64B).
+  // [K, rows]: a[j] of k8 kk is row g + 8 (j % 2) at k = 8 kk + 4 (j / 2) + t, 4 bytes each; the k-row pitch of A_T_LD
+  // floats puts the four t of a row 8 banks apart.
+  const int wrow = cw * 64 + (warp & 3) * 16, g8 = lane >> 2, t4 = lane & 3;
+  const uint32_t lm_off = sw64(wrow + (lane & 7) + 8 * ((lane >> 3) & 1), lane >> 4);  // ^ 32: chunk + 2 (chunks 0 and 1 here; the swizzle XORs bits 4-5 only)
+  const uint32_t t_off = (uint32_t)((t4 * A_T_LD + wrow + g8) * 4);
+  uint32_t af[2][2][BK / 8][4];  // [fragment set][hi, lo][k8][a0..a3]
   float acc[128];
-  int s = 0;
-  uint32_t ph = 0;  // parity of the full phase to wait for
+  auto kblock = [&](int q, int s, uint32_t (&f)[2][BK / 8][4]) {
+    const uint32_t as = a_slot(q), cur = (uint32_t)s * STAGE_BYTES;
+#pragma unroll
+    for (int kk = 0; kk < BK / 8; ++kk) {
+      uint32_t x[4];
+      if (a_km) {
+        ldsm_x4(as + (lm_off ^ (uint32_t)(kk * 32)), x);
+      } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) x[j] = lds32(as + t_off + (uint32_t)(((8 * kk + 4 * (j >> 1)) * A_T_LD + 8 * (j & 1)) * 4));
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) split_reg(x[j], f[0][kk][j], f[1][kk][j]);
+    }
+    wgmma_fence();  // the fragment registers are written before the wgmmas read them
+#pragma unroll
+    for (int kk = 0; kk < BK / 8; ++kk) {  // per MMA (K = 8 tf32): 32 bytes further inside the swizzled 64-byte rows
+      const uint32_t o = cur + kk * 32;
+      const uint64_t bh = b_desc0 + ((o + B_HI) >> 4), bl = b_desc0 + ((o + B_LO) >> 4);
+      if (split) {
+        wgmma_tf32(acc, f[1][kk], bh);
+        wgmma_tf32(acc, f[0][kk], bl);
+      }
+      wgmma_tf32(acc, f[0][kk], bh);
+    }
+    wgmma_commit();
+  };
+  int s = 0, q = 0;  // q: this CTA's k-block stream
+  uint32_t ph = 0;   // parity of the full phase to wait for
 #pragma unroll 1
   for (int i = 0; i < my_tiles; ++i) {
 #pragma unroll
     for (int j = 0; j < 128; ++j) acc[j] = 0.f;
     int prev = 0;
-#pragma unroll 1
-    for (int kb = 0; kb < nkb; ++kb) {
+    auto step = [&](int kb, uint32_t (&f)[2][BK / 8][4]) {
       mbar_wait(full0 + 8 * s, ph);
-      const uint32_t cur = (uint32_t)s * STAGE_BYTES;
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < BK / 8; ++kk) {  // per MMA (K = 8 tf32): 32 bytes further inside the swizzled 64-byte rows
-        const uint32_t o = cur + kk * 32;
-        const uint64_t ah = a_desc0 + ((o + A_HI) >> 4), al = a_desc0 + ((o + A_LO) >> 4), bh = b_desc0 + ((o + B_HI) >> 4), bl = b_desc0 + ((o + B_LO) >> 4);
-        if (split) {
-          wgmma_tf32(acc, al, bh);
-          wgmma_tf32(acc, ah, bl);
-        }
-        wgmma_tf32(acc, ah, bh);
-      }
-      wgmma_commit();
+      kblock(q, s, f);
       wgmma_wait<1>();                               // the wgmmas of the previous k-block are done
       if (kb > 0) mbar_arrive(empty0 + 8 * prev);   // ... so its stage is free for the producer
       prev = s;
+      ++q;
       if (++s == N_STAGES) { s = 0; ph ^= 1; }
+    };
+#pragma unroll 1
+    for (int kb = 0; kb < nkb; kb += 2) {
+      step(kb, af[0]);
+      if (kb + 1 < nkb) step(kb + 1, af[1]);
     }
 
     // ---- epilogue of tile i: acc[4 c + {0, 1}] = row r0, columns 8 c + 2 (lane % 4) + {0, 1}; acc[4 c + {2, 3}] = row r0 + 8 ----
