@@ -68,14 +68,15 @@ class GailUpdateArgs(C.Structure):
 
 class Gailx(C.Structure):
   _fields_ = [('g', Mlp), ('h', Mlp), ('g_u', vp), ('g_v', vp), ('h_u', vp), ('h_v', vp), ('g_u_stride', C.c_int32), ('g_v_stride', C.c_int32), ('h_u_stride', C.c_int32),
-              ('h_v_stride', C.c_int32), ('state_only', C.c_int32), ('reward_function', C.c_int32), ('subtract_log_policy', C.c_int32), ('discount', C.c_float), ('discount_r', vp)]
+              ('h_v_stride', C.c_int32), ('state_only', C.c_int32), ('reward_function', C.c_int32), ('subtract_log_policy', C.c_int32), ('discount', C.c_float), ('discount_r', vp),
+              ('reward_function_r', vp), ('spectral_norm_r', vp)]
 
 
 class GailxUpdateArgs(C.Structure):
   _fields_ = [('disc', Gailx), ('opt', Adam), ('params_floats', C.c_int64), ('policy', Batch), ('expert', Batch), ('eps_gp', vp), ('eps_mix', vp), ('logp_policy', vp),
               ('logp_expert', vp), ('logp_mix', vp), ('R', C.c_int32), ('loss_function', C.c_int32), ('training', C.c_int32), ('_pad', C.c_int32), ('grad_penalty', C.c_float),
               ('entropy_bonus', C.c_float), ('pos_class_prior', C.c_float), ('nonnegative_margin', C.c_float), ('out_losses', vp), ('workspace', vp), ('workspace_bytes', C.c_int64), ('grad_penalty_r', vp),
-              ('entropy_bonus_r', vp)]
+              ('entropy_bonus_r', vp), ('loss_function_r', vp), ('pos_class_prior_r', vp), ('nonnegative_margin_r', vp), ('penalty_pass_r', vp)]
 
 
 class Red(C.Structure):

@@ -93,9 +93,14 @@ VECTORISED = ('training.learning_rate', 'training.weight_decay', 'reinforcement.
               'imitation.learning_rate', 'imitation.weight_decay', 'imitation.grad_penalty', 'imitation.entropy_bonus', 'bc_pretraining.learning_rate',
               'bc_pretraining.weight_decay')
 # The GAIL discriminator's choices that leave every shape unchanged: per-replica values of the fused discriminator (csrc/gail.cu: one CTA per
-# replica branches on them). The general discriminator (csrc/gail_general.cu) takes only the Mixup alpha per replica.
+# replica branches on them). group_jobs gives the general discriminator (csrc/gail_general.cu) only the Mixup alpha per replica.
 PER_REPLICA_DISCRIMINATOR = ('imitation.loss_function', 'imitation.discriminator.reward_function', 'imitation.spectral_norm', 'imitation.mixup_alpha',
                              'imitation.pos_class_prior', 'imitation.nonnegative_margin')
+# The general discriminator's choices that sweep_groups makes per replica (general_discriminator_keys): its program runs every loss pass any
+# replica needs and masks each replica's dead passes, accesses and penalty pass out (il_gailx_update_args.loss_function_r / penalty_pass_r), so
+# each replica sees the sequence of power iterations and gradient sums of its single run.
+PER_REPLICA_GENERAL_DISCRIMINATOR = ('imitation.loss_function', 'imitation.discriminator.reward_function', 'imitation.spectral_norm', 'imitation.pos_class_prior',
+                                     'imitation.nonnegative_margin', 'imitation.grad_penalty')
 # The fused GAIL discriminator's hidden size: a per-replica shape (each replica keeps a single run's layout inside the stride of the widest; one
 # launch per width class), with at most MAX_WIDTH_CLASSES distinct widths in one program. The general discriminator groups on it.
 PER_REPLICA_WIDTH = ('imitation.discriminator.hidden_size', )
@@ -196,15 +201,19 @@ def expand_sweep(argv: Sequence[str]) -> Tuple[bool, List[SweepJob]]:
   return True, [SweepJob(i, list(c)) for i, c in enumerate(itertools.product(*choices))]
 
 
+def general_discriminator(cfg: Config) -> bool:
+  """Whether a GAIL configuration runs on the general discriminator (csrc/gail_general.cu): reward shaping, the log-policy term, depth != 1 or an
+  activation other than relu (models.GAILDiscriminator.general)."""
+  d = cfg.imitation.get('discriminator') or {}
+  return cfg.get('algorithm') == 'GAIL' and bool(d.get('reward_shaping') or d.get('subtract_log_policy') or d.get('depth', 1) != 1 or d.get('activation', 'relu') != 'relu')
+
+
 def vectorised_keys(cfg: Config) -> Tuple[str, ...]:
   """VECTORISED minus the keys a path of this configuration cannot take per replica, plus the discriminator choices for GAIL and the
-  algorithm's own keys of PER_REPLICA_ALGORITHM: the general GAIL discriminator (csrc/gail_general.cu) batches its gradient-penalty pass over
-  replicas, so a replica with grad_penalty 0 would still take that pass's power iteration, and it takes only mixup_alpha of
-  PER_REPLICA_DISCRIMINATOR; PWIL takes its scales per replica only without expert-data mixing (the expert memory's relabelled rewards
+  algorithm's own keys of PER_REPLICA_ALGORITHM: for the general GAIL discriminator (csrc/gail_general.cu) this partition keeps grad_penalty
+  and every choice but mixup_alpha grouping keys (sweep_groups makes them per replica through general_discriminator_keys); PWIL takes its scales per replica only without expert-data mixing (the expert memory's relabelled rewards
   depend on them and are shared)."""
-  d = cfg.imitation.get('discriminator') or {}
-  gail = cfg.get('algorithm') == 'GAIL'
-  general = gail and bool(d.get('reward_shaping') or d.get('subtract_log_policy') or d.get('depth', 1) != 1 or d.get('activation', 'relu') != 'relu')
+  gail, general = cfg.get('algorithm') == 'GAIL', general_discriminator(cfg)
   keys = tuple(k for k in VECTORISED if not (general and k == 'imitation.grad_penalty'))
   if gail: keys += ('imitation.mixup_alpha', ) if general else PER_REPLICA_DISCRIMINATOR + PER_REPLICA_WIDTH
   alg = cfg.get('algorithm')
@@ -213,9 +222,15 @@ def vectorised_keys(cfg: Config) -> Tuple[str, ...]:
 
 
 def per_replica_keys(cfg: Config) -> Tuple[str, ...]:
-  """Every key Trainer(per_replica=...) takes in this configuration: vectorised_keys plus `seed` where it can be per replica (seed_per_replica)
-  and RED's / DRIL's dropout keys (dropout_keys)."""
-  return vectorised_keys(cfg) + (PER_REPLICA_SEED if seed_per_replica(cfg) else ()) + dropout_keys(cfg)
+  """Every key Trainer(per_replica=...) takes in this configuration: vectorised_keys plus `seed` where it can be per replica (seed_per_replica),
+  RED's / DRIL's dropout keys (dropout_keys) and the general GAIL discriminator's choices (general_discriminator_keys)."""
+  return vectorised_keys(cfg) + (PER_REPLICA_SEED if seed_per_replica(cfg) else ()) + dropout_keys(cfg) + general_discriminator_keys(cfg)
+
+
+def general_discriminator_keys(cfg: Config) -> Tuple[str, ...]:
+  """PER_REPLICA_GENERAL_DISCRIMINATOR for a GAIL configuration on the general discriminator, else nothing. Like `seed` and the dropout keys,
+  these are per replica in sweep_groups only: group_jobs keeps them grouping keys."""
+  return PER_REPLICA_GENERAL_DISCRIMINATOR if general_discriminator(cfg) else ()
 
 
 def dropout_keys(cfg: Config) -> Tuple[str, ...]:

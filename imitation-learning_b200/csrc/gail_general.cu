@@ -28,7 +28,7 @@ namespace {
     }                                                                                                 \
   } while (0)
 
-constexpr int GX_MAX_EVALS = 9;
+constexpr int GX_MAX_EVALS = 12;  // (policy, expert, Mixup, penalty pass) x (g, h(s'), h(s))
 
 __device__ __forceinline__ float act_grad2_from_output(float y, int act) {  // second derivative of the activation through its output
   if (act == IL_ACT_RELU) return 0.f;
@@ -47,14 +47,30 @@ __host__ __device__ inline SnLayout sn_layout(const int32_t* dims, int L) {
   return s;
 }
 
-// One spectral-norm access of every layer of R nets. One CTA per replica. eff receives W / sigma (or W without spectral norm)
-// and the biases; snap receives per layer [u | v | sigma] of THIS access (layout: u_total + v_total + L floats).
+// Whether replica r takes part in one pass of the update (sweeps of the loss function and of the gradient penalty). kind: 0 policy, 1 expert,
+// 2 Mixup, 3 penalty, -1 every replica. A Mixup replica lives in the Mixup pass only, a BCE / PUGAIL one in the policy and expert passes.
+struct Live {
+  const int32_t* loss_r;  // loss_function_r (nullptr: every loss pass is live)
+  const int32_t* pen_r;   // penalty_pass_r (nullptr: the penalty pass is live)
+  int kind;
+};
+__device__ __forceinline__ bool live_at(const Live& l, int r) {
+  if (l.kind == 3) return !l.pen_r || l.pen_r[r] != 0;
+  if (l.kind < 0 || !l.loss_r) return true;
+  return (l.loss_r[r] == IL_LOSS_MIXUP) == (l.kind == 2);
+}
+
+// One spectral-norm access of every layer of R nets. One CTA per replica. eff receives W / sigma (or W / 1 without spectral norm)
+// and the biases; snap receives per layer [u | v | sigma] of THIS access (layout: u_total + v_total + L floats). A replica without spectral
+// norm, or whose access is dead, runs no power iteration and leaves its u / v alone (sigma = 1, u / v of the snapshot unwritten).
 struct SnAccessParams {
   il_mlp net, eff;
   float *u, *v;      // persistent buffers (nullptr: no spectral norm)
   int u_stride, v_stride;
   float* snap;
   int snap_stride, training;
+  const int32_t* sn_r;  // [R] per-replica spectral-norm flag (nullptr: u != nullptr for every replica)
+  Live live;
 };
 __global__ void __launch_bounds__(256) sn_access_kernel(const SnAccessParams p) {
   __shared__ float red[32];
@@ -65,6 +81,7 @@ __global__ void __launch_bounds__(256) sn_access_kernel(const SnAccessParams p) 
   const float* prm = p.net.params + (int64_t)r * p.net.stride;
   float* eff = p.eff.params + (int64_t)r * p.eff.stride;
   float* snap = p.snap + (int64_t)r * p.snap_stride;
+  const bool sn = p.u && (!p.sn_r || p.sn_r[r] != 0) && live_at(p.live, r);
   int off = 0, uo = 0, vo = 0;  // running offsets of layer l: parameters (mlp_offsets rule), u, v
   for (int l = 0; l < L; ++l) {
     const int od = p.net.dims[l + 1], in = p.net.dims[l];
@@ -72,7 +89,7 @@ __global__ void __launch_bounds__(256) sn_access_kernel(const SnAccessParams p) 
     off = (b_off + od + 3) / 4 * 4;
     const float* W = prm + w_off;
     float sigma = 1.f;
-    if (p.u) {
+    if (sn) {
       float* u = p.u + (int64_t)r * p.u_stride + uo;
       float* v = p.v + (int64_t)r * p.v_stride + vo;
       __syncthreads();
@@ -105,7 +122,8 @@ __global__ void __launch_bounds__(256) sn_access_kernel(const SnAccessParams p) 
   }
 }
 
-// dL/dW_orig += (G - <G, W_eff> u v^T) / sigma per layer; biases add directly. One CTA per replica.
+// dL/dW_orig += (G - <G, W_eff> u v^T) / sigma per layer; biases add directly. One CTA per replica. A replica whose access is dead adds
+// nothing (not even zeros: a signed zero would change the sum's bits).
 struct SnProjectParams {
   il_mlp eff;
   const float* g_eff;   // [R, eff.stride] gradient w.r.t. the effective parameters
@@ -113,10 +131,14 @@ struct SnProjectParams {
   int snap_stride, has_sn;
   float* g_out;         // flat gradient buffer, this net's slice: element (r, i) at g_out + r * out_stride + i
   int64_t out_stride;
+  const int32_t* sn_r;  // [R] per-replica spectral-norm flag (nullptr: has_sn for every replica)
+  Live live;
 };
 __global__ void __launch_bounds__(256) sn_project_kernel(const SnProjectParams p) {
   __shared__ float red[32];
   const int r = blockIdx.x, tid = threadIdx.x, L = p.eff.n_layers;
+  if (!live_at(p.live, r)) return;
+  const bool sn = p.has_sn && (!p.sn_r || p.sn_r[r] != 0);
   int u_total = 0, v_total = 0;
   for (int l = 0; l < L; ++l) { u_total += p.eff.dims[l + 1]; v_total += p.eff.dims[l]; }
   const float* eff = p.eff.params + (int64_t)r * p.eff.stride;
@@ -128,7 +150,7 @@ __global__ void __launch_bounds__(256) sn_project_kernel(const SnProjectParams p
     const int od = p.eff.dims[l + 1], in = p.eff.dims[l];
     const int w_off = off, b_off = (off + od * in + 3) / 4 * 4;
     off = (b_off + od + 3) / 4 * 4;
-    if (p.has_sn) {
+    if (sn) {
       float s = 0.f;
       for (int i = tid; i < od * in; i += 256) s = fmaf(G[w_off + i], eff[w_off + i], s);
       const float inner = block_sum(s, red), sigma = snap[u_total + v_total + l];
@@ -167,12 +189,15 @@ struct PassView {        // one discriminator forward (models.py:172-175) on a b
   int kind;              // 0 policy, 1 expert, 2 mixup
 };
 struct LossParams {
-  PassView pass[2];
+  PassView pass[3];
   int n_pass, B, row, off_terminal, off_weight, loss_function, shaping;
   float discount, entropy_bonus, pos_class_prior, nonnegative_margin;
   float* out_losses;     // [R, 2]
   const float* discount_r;       // [R] per-replica values (nullptr = the scalar)
   const float* entropy_bonus_r;
+  const int32_t* loss_function_r;  // with it the passes are policy, expert (and Mixup), each live where Live says
+  const float* pos_class_prior_r;
+  const float* nonnegative_margin_r;
 };
 __device__ __forceinline__ float pass_logit(const PassView& v, const LossParams& p, int r, int b, float* one_minus_t) {
   const int64_t i = (int64_t)r * p.B + b;
@@ -188,13 +213,18 @@ __device__ __forceinline__ float pass_logit(const PassView& v, const LossParams&
   return f;
 }
 // training.py:94-114,130-132: loss value and d loss / d logits for every pass, then the output gradients of g, h(s'), h(s). One CTA per replica.
+// A dead pass of the replica (per-replica loss functions) adds nothing to its loss, in the accumulation order of its single run, and gets zero
+// output gradients.
 __global__ void __launch_bounds__(256) gailx_loss_kernel(const LossParams p) {
   __shared__ float red[32];
   const int r = blockIdx.x, B = p.B;
   const float invB = 1.f / (float)B;
   const float discount = p.discount_r ? p.discount_r[r] : p.discount, entropy_bonus = p.entropy_bonus_r ? p.entropy_bonus_r[r] : p.entropy_bonus;
+  const int loss_function = p.loss_function_r ? p.loss_function_r[r] : p.loss_function;
+  const float prior = p.pos_class_prior_r ? p.pos_class_prior_r[r] : p.pos_class_prior;
+  const float nonnegative_margin = p.nonnegative_margin_r ? p.nonnegative_margin_r[r] : p.nonnegative_margin;
   float pu_gate = 1.f;
-  if (p.loss_function == IL_LOSS_PUGAIL) {  // the clamp of training.py:102 needs the batch scalar first
+  if (loss_function == IL_LOSS_PUGAIL) {  // the clamp of training.py:102 needs the batch scalar first (passes 0 / 1: policy, expert)
     float sp = 0.f, se = 0.f;
     for (int b = threadIdx.x; b < B; b += blockDim.x) {
       float omt;
@@ -204,12 +234,19 @@ __global__ void __launch_bounds__(256) gailx_loss_kernel(const LossParams p) {
     }
     sp = block_sum(sp, red);
     se = block_sum(se, red);
-    pu_gate = (p.pos_class_prior * (se * invB) - sp * invB) >= -p.nonnegative_margin ? 1.f : 0.f;
+    pu_gate = (prior * (se * invB) - sp * invB) >= -nonnegative_margin ? 1.f : 0.f;
   }
   float loss = 0.f;
   for (int k = 0; k < p.n_pass; ++k) {
     const PassView& v = p.pass[k];
+    const bool live = live_at(Live{p.loss_function_r, nullptr, v.kind}, r);
     for (int b = threadIdx.x; b < B; b += blockDim.x) {
+      if (!live) {
+        const int64_t i = (int64_t)r * B + b;
+        v.dg[i] = 0.f;
+        if (p.shaping) { v.dhn[i] = 0.f; v.dhs[i] = 0.f; }
+        continue;
+      }
       float omt;
       const float f = pass_logit(v, p, r, b, &omt), sg = sigmoidf(f);
       const float w = v.rows[(int64_t)r * v.rs + (int64_t)b * p.row + p.off_weight];
@@ -218,11 +255,11 @@ __global__ void __launch_bounds__(256) gailx_loss_kernel(const LossParams p) {
         const float e = v.eps[(int64_t)r * B + b];
         df = w * (sg - e) * invB;
         loss += e * w * softplusf(-f) + (1.f - e) * w * softplusf(f);
-      } else if (p.loss_function == IL_LOSS_BCE) {
+      } else if (loss_function == IL_LOSS_BCE) {
         df = v.kind == 1 ? w * (sg - 1.f) * invB : w * sg * invB;
         loss += v.kind == 1 ? w * softplusf(-f) : w * softplusf(f);
       } else {
-        const float pr = p.pos_class_prior;
+        const float pr = prior;
         df = v.kind == 1 ? pr * w * (sg - 1.f) * invB + pu_gate * pr * w * sg * invB : -pu_gate * w * sg * invB;
         loss += v.kind == 1 ? pr * w * softplusf(-f) + pu_gate * pr * w * softplusf(f) : -pu_gate * w * softplusf(f);
       }
@@ -233,7 +270,7 @@ __global__ void __launch_bounds__(256) gailx_loss_kernel(const LossParams p) {
     }
   }
   loss = block_sum(loss, red);
-  const float margin = pu_gate == 0.f ? p.nonnegative_margin : 0.f;  // the clamp is active: policy_loss = -margin (training.py:102)
+  const float margin = pu_gate == 0.f ? nonnegative_margin : 0.f;  // the clamp is active: policy_loss = -margin (training.py:102)
   if (threadIdx.x == 0 && p.out_losses) p.out_losses[r * 2 + 0] = loss * invB - margin;
 }
 
@@ -272,11 +309,13 @@ __global__ void gp_linear_gx_kernel(const float* __restrict__ w1, int64_t w_gs, 
   float* dst = gin + rb * ld + j;
   *dst = accumulate ? *dst + v : v;
 }
-// P_b = lambda w_b |g_in|^2;  gbar = 2 lambda w_b / B * g_in (in place);  loss = mean(P). One CTA per replica.
+// P_b = lambda w_b |g_in|^2;  gbar = 2 lambda w_b / B * g_in (in place);  loss = mean(P). One CTA per replica. A replica outside the
+// pass (penalty_pass_r[r] == 0) leaves its loss entry alone, as a run without a penalty does; its gbar is never projected.
 __global__ void __launch_bounds__(256) gp_penalty_kernel(float* __restrict__ gin, int ld, int cols, const float* __restrict__ rows, int64_t rs, int row, int off_weight, float lambda,
-                                                         const float* __restrict__ lambda_r, float* __restrict__ out_losses, int B) {
+                                                         const float* __restrict__ lambda_r, float* __restrict__ out_losses, int B, const int32_t* __restrict__ pen_r) {
   __shared__ float red[32];
   const int r = blockIdx.x;
+  if (pen_r && pen_r[r] == 0) return;
   if (lambda_r) lambda = lambda_r[r];
   float loss = 0.f;
   for (int b = threadIdx.x; b < B; b += blockDim.x) {
@@ -312,10 +351,12 @@ __global__ void add_kernel(float* __restrict__ a, const float* __restrict__ b, i
   if (t < n) a[t] += b[t];
 }
 // models.py:177-180 on combined logits
-__global__ void gailx_reward_kernel(PassView v, LossParams p, int reward_function, float* __restrict__ reward, int64_t reward_rs, int reward_ld, float* __restrict__ logits, int R) {
+__global__ void gailx_reward_kernel(PassView v, LossParams p, int reward_function, const int32_t* __restrict__ reward_function_r, float* __restrict__ reward, int64_t reward_rs,
+                                    int reward_ld, float* __restrict__ logits, int R) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= (int64_t)R * p.B) return;
   const int r = (int)(t / p.B), b = (int)(t % p.B);
+  if (reward_function_r) reward_function = reward_function_r[r];
   float omt;
   const float f = pass_logit(v, p, r, b, &omt);
   if (logits) logits[t] = f;
@@ -342,6 +383,8 @@ struct NetEval {        // one spectral-norm access + forward of one net on one 
   const il_mlp* net;
   float *u, *v;
   int u_stride, v_stride;
+  const int32_t* sn_r;  // per-replica spectral-norm flags
+  Live live;            // the replicas this access is live for
   il_mlp eff;           // effective parameters of this access (workspace), same layout as the net
   float* snap;
   int snap_stride;
@@ -364,8 +407,8 @@ int max_dim(const il_mlp* m) {
   return d;
 }
 
-void eval_carve(Carver& c, NetEval& e, const il_mlp* net, float* u, float* v, int us, int vs, int R, int B, bool need_grad) {
-  e.net = net; e.u = u; e.v = v; e.u_stride = us; e.v_stride = vs;
+void eval_carve(Carver& c, NetEval& e, const il_mlp* net, float* u, float* v, int us, int vs, const int32_t* sn_r, int R, int B, bool need_grad) {
+  e.net = net; e.u = u; e.v = v; e.u_stride = us; e.v_stride = vs; e.sn_r = sn_r; e.live = Live{nullptr, nullptr, -1};
   e.eff = *net;
   e.eff.params = c.take((int64_t)R * net->stride);
   e.snap_stride = snap_floats(net);
@@ -381,6 +424,7 @@ void eval_carve(Carver& c, NetEval& e, const il_mlp* net, float* u, float* v, in
 int eval_access(il_handle* h, NetEval& e, int R, int training, cudaStream_t st) {
   SnAccessParams p;
   p.net = *e.net; p.eff = e.eff; p.u = e.u; p.v = e.v; p.u_stride = e.u_stride; p.v_stride = e.v_stride; p.snap = e.snap; p.snap_stride = e.snap_stride; p.training = training;
+  p.sn_r = e.sn_r; p.live = e.live;
   IL_LAUNCH(h, sn_access_kernel, R, 256, (size_t)max_dim(e.net) * 4, st, p);
   return 0;
 }
@@ -390,6 +434,7 @@ int eval_project(il_handle* h, NetEval& e, int R, int64_t out_stride, cudaStream
            (void*)e.g_eff, (void*)e.snap, (void*)e.g_out);
   SnProjectParams p;
   p.eff = e.eff; p.g_eff = e.g_eff; p.snap = e.snap; p.snap_stride = e.snap_stride; p.has_sn = e.u != nullptr; p.g_out = e.g_out; p.out_stride = out_stride;
+  p.sn_r = e.sn_r; p.live = e.live;
   IL_LAUNCH(h, sn_project_kernel, R, 256, 0, st, p);
   return 0;
 }
@@ -496,6 +541,7 @@ int validate_disc(const il_gailx* d, const il_batch* b, const char* what) {
     IL_CHECK((d->h_u == nullptr) == (d->g_u == nullptr), "%s: spectral norm must cover both g and h", what);
   }
   IL_CHECK((d->g_u == nullptr) == (d->g_v == nullptr), "%s: spectral-norm buffers must both be set or both be null", what);
+  IL_CHECK(!d->spectral_norm_r || (d->g_u && d->g_v && (d->h.n_layers == 0 || (d->h_u && d->h_v))), "%s: spectral_norm_r needs the u / v buffers of every replica", what);
   IL_CHECK(b->row == row_layout(b->S, b->A).len && b->rows, "%s: bad batch", what);
   return 0;
 }
@@ -514,23 +560,43 @@ struct UpdLayout {
 // the gradient-penalty pass runs when grad_penalty > 0, or, with per-replica values, when the caller passes its noise (eps_gp)
 bool gp_enabled(const il_gailx_update_args* a) { return a->grad_penalty_r ? a->eps_gp != nullptr : a->grad_penalty > 0.f; }
 
+// The loss passes of one update, in order (Live kinds: 0 policy, 1 expert, 2 Mixup), then the penalty pass when gp. Without loss_function_r a
+// Mixup run has the Mixup pass only, a BCE / PUGAIL run the policy and expert passes; with it the policy and expert passes always run and the
+// Mixup pass runs when eps_mix is passed, so each replica's live accesses come in the order of its own single run.
+struct Schedule {
+  int n_loss, kind[3];
+  bool gp, mixup;
+};
+Schedule schedule(const il_gailx_update_args* a) {
+  Schedule s{};
+  const bool per_replica = a->loss_function_r != nullptr;
+  if (per_replica || a->loss_function != IL_LOSS_MIXUP) { s.kind[s.n_loss++] = 0; s.kind[s.n_loss++] = 1; }
+  if (per_replica ? a->eps_mix != nullptr : a->loss_function == IL_LOSS_MIXUP) s.kind[s.n_loss++] = 2;
+  s.mixup = s.kind[s.n_loss - 1] == 2;
+  s.gp = gp_enabled(a);
+  return s;
+}
+
 // evaluation slots: pass k (loss passes first, then the GP pass) x {g, h(s'), h(s)}
 void upd_layout(const il_gailx_update_args* a, char* base, UpdLayout* L) {
   Carver c{base, 0};
   const il_gailx& d = a->disc;
   const int R = a->R, B = a->policy.B, S = a->policy.S, A = a->policy.A, row = a->policy.row;
-  const bool shaping = d.h.n_layers > 0, gp = gp_enabled(a), mixup = a->loss_function == IL_LOSS_MIXUP;
-  const int n_loss_pass = mixup ? 1 : 2;
+  const Schedule sc = schedule(a);
+  const bool shaping = d.h.n_layers > 0, gp = sc.gp;
   L->n_ev = 0;
-  for (int k = 0; k < n_loss_pass + (gp ? 1 : 0); ++k) {
-    const bool is_gp = k == n_loss_pass;
-    eval_carve(c, L->ev[L->n_ev++], &d.g, d.g_u, d.g_v, d.g_u_stride, d.g_v_stride, R, B, true);
+  for (int k = 0; k < sc.n_loss + (gp ? 1 : 0); ++k) {
+    const bool is_gp = k == sc.n_loss;
+    const Live live{a->loss_function_r, a->penalty_pass_r, is_gp ? 3 : sc.kind[k]};
+    const int first = L->n_ev;
+    eval_carve(c, L->ev[L->n_ev++], &d.g, d.g_u, d.g_v, d.g_u_stride, d.g_v_stride, d.spectral_norm_r, R, B, true);
     if (shaping) {
-      eval_carve(c, L->ev[L->n_ev++], &d.h, d.h_u, d.h_v, d.h_u_stride, d.h_v_stride, R, B, !is_gp);  // h(s'): forward only in the GP pass (its input is not differentiated)
-      eval_carve(c, L->ev[L->n_ev++], &d.h, d.h_u, d.h_v, d.h_u_stride, d.h_v_stride, R, B, true);
+      eval_carve(c, L->ev[L->n_ev++], &d.h, d.h_u, d.h_v, d.h_u_stride, d.h_v_stride, d.spectral_norm_r, R, B, !is_gp);  // h(s'): forward only in the GP pass (its input is not differentiated)
+      eval_carve(c, L->ev[L->n_ev++], &d.h, d.h_u, d.h_v, d.h_u_stride, d.h_v_stride, d.spectral_norm_r, R, B, true);
     }
+    for (int j = first; j < L->n_ev; ++j) L->ev[j].live = live;
   }
-  L->mix_rows[0] = mixup ? c.take((int64_t)R * B * row) : nullptr;
+  L->mix_rows[0] = sc.mixup ? c.take((int64_t)R * B * row) : nullptr;
   L->mix_rows[1] = gp ? c.take((int64_t)R * B * row) : nullptr;
   L->gin = gp ? c.take((int64_t)R * B * (S + A)) : nullptr;
   L->g_flat = c.take(a->params_floats);
@@ -575,10 +641,13 @@ extern "C" int il_gailx_update(il_handle* h, const il_gailx_update_args* a, void
   IL_CHECK(R > 0 && a->expert.rows && a->expert.B == B && a->expert.S == S && a->expert.A == A, "il_gailx_update: policy / expert batch mismatch");
   IL_CHECK(a->opt.m && a->opt.v && a->opt.step && a->params_floats > 0, "il_gailx_update: null optimiser state");
   IL_CHECK(a->loss_function >= 0 && a->loss_function <= 2, "il_gailx_update: bad loss function %d", a->loss_function);
-  const bool shaping = d.h.n_layers > 0, gp = gp_enabled(a), mixup = a->loss_function == IL_LOSS_MIXUP, sublp = d.subtract_log_policy != 0;
+  const Schedule sc = schedule(a);
+  const bool shaping = d.h.n_layers > 0, gp = sc.gp, mixup = sc.mixup, sublp = d.subtract_log_policy != 0;
+  const int n_loss_pass = sc.n_loss;
   IL_CHECK(!(gp && !a->eps_gp) && !(mixup && !a->eps_mix), "il_gailx_update: missing eps_gp / eps_mix");
   IL_CHECK(!(gp && d.state_only), "il_gailx_update: grad_penalty with a state-only discriminator is undefined in the reference (autograd.grad on the unused action, training.py:125)");
-  IL_CHECK(!sublp || (mixup ? a->logp_mix != nullptr : (a->logp_policy && a->logp_expert)), "il_gailx_update: subtract_log_policy needs the log-policy inputs");
+  const float* logp_of[3] = {a->logp_policy, a->logp_expert, a->logp_mix};
+  for (int k = 0; k < n_loss_pass; ++k) IL_CHECK(!sublp || logp_of[sc.kind[k]], "il_gailx_update: subtract_log_policy needs the log-policy inputs of every pass that runs");
   IL_CHECK(a->workspace && a->workspace_bytes >= il_gailx_workspace_bytes(a), "il_gailx_update: workspace too small");
   UpdLayout L;
   upd_layout(a, static_cast<char*>(a->workspace), &L);
@@ -588,17 +657,19 @@ extern "C" int il_gailx_update(il_handle* h, const il_gailx_update_args* a, void
   IL_CUDA(cudaMemsetAsync(L.g_flat, 0, (size_t)a->params_floats * 4, st));
   IL_TRY(launch_tick(h, a->opt.step, nullptr, nullptr, st));
 
-  const int per_pass = shaping ? 3 : 1, n_loss_pass = mixup ? 1 : 2;
+  const int per_pass = shaping ? 3 : 1;
   const int64_t h_off = shaping ? d.h.params - d.g.params : 0;
   // ---- batches of the passes ------------------------------------------------------------------------------------------------
-  const float* pass_rows[3]; int64_t pass_rs[3];
-  if (mixup) {
-    il_batch ob = a->policy; ob.rows = L.mix_rows[0]; ob.replica_stride = (int64_t)B * row;
-    IL_TRY(il_gail_mix_batch(h, &a->expert, &a->policy, a->eps_mix, R, &ob, stream));
-    pass_rows[0] = L.mix_rows[0]; pass_rs[0] = (int64_t)B * row;
-  } else {
-    pass_rows[0] = a->policy.rows; pass_rs[0] = a->policy.replica_stride;
-    pass_rows[1] = a->expert.rows; pass_rs[1] = a->expert.replica_stride;
+  const float* pass_rows[4]; int64_t pass_rs[4];
+  for (int k = 0; k < n_loss_pass; ++k) {
+    if (sc.kind[k] == 2) {
+      il_batch ob = a->policy; ob.rows = L.mix_rows[0]; ob.replica_stride = (int64_t)B * row;
+      IL_TRY(il_gail_mix_batch(h, &a->expert, &a->policy, a->eps_mix, R, &ob, stream));
+      pass_rows[k] = L.mix_rows[0]; pass_rs[k] = (int64_t)B * row;
+    } else {
+      const il_batch& b = sc.kind[k] == 0 ? a->policy : a->expert;
+      pass_rows[k] = b.rows; pass_rs[k] = b.replica_stride;
+    }
   }
   if (gp) {
     il_batch ob = a->policy; ob.rows = L.mix_rows[1]; ob.replica_stride = (int64_t)B * row;
@@ -624,15 +695,16 @@ extern "C" int il_gailx_update(il_handle* h, const il_gailx_update_args* a, void
   LossParams lp{};
   lp.n_pass = n_loss_pass; lp.B = B; lp.row = row; lp.off_terminal = RL.terminal; lp.off_weight = RL.weight; lp.loss_function = a->loss_function; lp.shaping = shaping;
   lp.discount = d.discount; lp.discount_r = d.discount_r; lp.entropy_bonus = a->entropy_bonus; lp.entropy_bonus_r = a->entropy_bonus_r; lp.pos_class_prior = a->pos_class_prior; lp.nonnegative_margin = a->nonnegative_margin; lp.out_losses = a->out_losses;
+  lp.loss_function_r = a->loss_function_r; lp.pos_class_prior_r = a->pos_class_prior_r; lp.nonnegative_margin_r = a->nonnegative_margin_r;
   for (int k = 0; k < n_loss_pass; ++k) {
     PassView& v = lp.pass[k];
     NetEval* e = &L.ev[k * per_pass];
     v.rows = pass_rows[k]; v.rs = pass_rs[k];
     v.og = e[0].out; v.dg = e[0].dout;
     if (shaping) { v.ohn = e[1].out; v.ohs = e[2].out; v.dhn = e[1].dout; v.dhs = e[2].dout; }
-    v.logp = sublp ? (mixup ? a->logp_mix : (k == 0 ? a->logp_policy : a->logp_expert)) : nullptr;
-    v.eps = mixup ? a->eps_mix : nullptr;
-    v.kind = mixup ? 2 : k;
+    v.kind = sc.kind[k];
+    v.logp = sublp ? logp_of[v.kind] : nullptr;
+    v.eps = v.kind == 2 ? a->eps_mix : nullptr;
   }
   IL_LAUNCH(h, gailx_loss_kernel, R, 256, 0, st, lp);
   GX_STAGE(h, st, "loss");
@@ -655,7 +727,8 @@ extern "C" int il_gailx_update(il_handle* h, const il_gailx_update_args* a, void
     // keep for the double backward: with reward shaping g is linear (no chain) and h owns the scratch; without shaping there is only g.
     IL_TRY(gp_input_gradient(h, e[0], one, L.gb, L.gin, ld, 0, R, B, st));
     if (shaping) IL_TRY(gp_input_gradient(h, e[2], kh, L.gb, L.gin, ld, 1, R, B, st));
-    IL_LAUNCH(h, gp_penalty_kernel, R, 256, 0, st, L.gin, ld, ld, pass_rows[n_loss_pass], pass_rs[n_loss_pass], row, RL.weight, a->grad_penalty, a->grad_penalty_r, a->out_losses, B);
+    IL_LAUNCH(h, gp_penalty_kernel, R, 256, 0, st, L.gin, ld, ld, pass_rows[n_loss_pass], pass_rs[n_loss_pass], row, RL.weight, a->grad_penalty, a->grad_penalty_r, a->out_losses, B,
+              a->penalty_pass_r);
     GX_STAGE(h, st, "gp input gradients + penalty");
     if (shaping) {
       IL_TRY(gp_double_backward(h, e[2], kh, L.gb, L.gin, ld, R, B, st));
@@ -676,8 +749,8 @@ extern "C" int64_t il_gailx_reward_workspace_bytes(const il_gailx* d, int R, int
   if (!d || R <= 0 || B <= 0) return -1;
   Carver c{nullptr, 0};
   NetEval e;
-  eval_carve(c, e, &d->g, nullptr, nullptr, 0, 0, R, B, false);
-  if (d->h.n_layers > 0) { eval_carve(c, e, &d->h, nullptr, nullptr, 0, 0, R, B, false); eval_carve(c, e, &d->h, nullptr, nullptr, 0, 0, R, B, false); }
+  eval_carve(c, e, &d->g, nullptr, nullptr, 0, 0, nullptr, R, B, false);
+  if (d->h.n_layers > 0) { eval_carve(c, e, &d->h, nullptr, nullptr, 0, 0, nullptr, R, B, false); eval_carve(c, e, &d->h, nullptr, nullptr, 0, 0, nullptr, R, B, false); }
   return c.used;
 }
 
@@ -693,10 +766,10 @@ extern "C" int il_gailx_reward(il_handle* h, const il_gailx* d, int R, const il_
   const bool shaping = d->h.n_layers > 0;
   Carver c{static_cast<char*>(workspace), 0};
   NetEval ev[3];
-  eval_carve(c, ev[0], &d->g, d->g_u, d->g_v, d->g_u_stride, d->g_v_stride, R, B, false);
+  eval_carve(c, ev[0], &d->g, d->g_u, d->g_v, d->g_u_stride, d->g_v_stride, d->spectral_norm_r, R, B, false);
   if (shaping) {
-    eval_carve(c, ev[1], &d->h, d->h_u, d->h_v, d->h_u_stride, d->h_v_stride, R, B, false);
-    eval_carve(c, ev[2], &d->h, d->h_u, d->h_v, d->h_u_stride, d->h_v_stride, R, B, false);
+    eval_carve(c, ev[1], &d->h, d->h_u, d->h_v, d->h_u_stride, d->h_v_stride, d->spectral_norm_r, R, B, false);
+    eval_carve(c, ev[2], &d->h, d->h_u, d->h_v, d->h_u_stride, d->h_v_stride, d->spectral_norm_r, R, B, false);
   }
   for (int j = 0; j < (shaping ? 3 : 1); ++j) {  // eval mode (train.py:180,194): no power iteration, sigma from the stored (u, v)
     ev[j].X = MatView{batch->rows + (j == 1 ? RL.next_state : RL.state), batch->replica_stride, 1, row};
@@ -709,6 +782,6 @@ extern "C" int il_gailx_reward(il_handle* h, const il_gailx* d, int R, const il_
   v.rows = batch->rows; v.rs = batch->replica_stride; v.og = ev[0].out;
   if (shaping) { v.ohn = ev[1].out; v.ohs = ev[2].out; }
   v.logp = d->subtract_log_policy ? log_policy : nullptr;
-  IL_LAUNCH(h, gailx_reward_kernel, blocks((int64_t)R * B), 256, 0, st, v, lp, d->reward_function, reward, reward_rs, reward_ld, logits, R);
+  IL_LAUNCH(h, gailx_reward_kernel, blocks((int64_t)R * B), 256, 0, st, v, lp, d->reward_function, d->reward_function_r, reward, reward_rs, reward_ld, logits, R);
   return 0;
 }

@@ -422,8 +422,8 @@ class GAILDiscriminator(_Module):
   def __init__(self, state_size: int, action_size: int, imitation_cfg, discount, replicas: int = 1, rng: Optional[ReplicaRNG] = None, device=None,
                reward_function=None, spectral_norm=None, hidden_size=None):
     """reward_function / spectral_norm / hidden_size: None = the config's value; otherwise one value, or one value per replica (hyper-parameter
-    sweeps of the fused discriminator: replica r is initialised, trained and rewarded as a single run with its own values). With per-replica
-    widths the flat buffer keeps the stride of the widest replica; replica r's block starts with the layout of a single width-H_r run and the
+    sweeps: replica r is initialised, trained and rewarded as a single run with its own values). With per-replica widths (fused discriminator
+    only) the flat buffer keeps the stride of the widest replica; replica r's block starts with the layout of a single width-H_r run and the
     rest of it stays zero."""
     model_cfg = imitation_cfg.discriminator
     self.state_only = bool(imitation_cfg.state_only)
@@ -445,9 +445,10 @@ class GAILDiscriminator(_Module):
     self.general = self.reward_shaping or self.subtract_log_policy or model_cfg.depth != 1 or model_cfg.activation != 'relu'
     self._ws = None
     if self.general:
-      if len(set(rf_list)) > 1 or len(set(sn_list)) > 1 or len(set(h_list)) > 1:
-        raise ValueError('per-replica reward_function / spectral_norm / hidden_size need the fused discriminator (depth 1, relu, no shaping or log-policy term)')
-      self._init_general(model_cfg, rng, device, h_list[0])
+      if len(set(h_list)) > 1:
+        raise ValueError('per-replica hidden_size needs the fused discriminator (depth 1, relu, no shaping or log-policy term): the general one groups on it')
+      self._init_general(model_cfg, rng, device, h_list[0], sn_list)
+      self.set_choices(rf_list, sn_list)
       return
     d, H = (state_size if self.state_only else state_size + action_size), max(h_list)
     dims = [d, H, 1]
@@ -498,12 +499,13 @@ class GAILDiscriminator(_Module):
     return [f[:, w[0]:w[0] + H * d].view(R, H, d), f[:, b[0]:b[0] + H], f[:, w[1]:w[1] + H].view(R, 1, H), f[:, b[1]:b[1] + 1]]
 
   def set_choices(self, reward_function, spectral_norm):
-    """Per-replica reward function / spectral-norm flag of the fused discriminator (one value or R values; R equal values are the uniform path).
-    A replica without spectral norm never reads or writes its u / v rows. Trainer(fast_init=True) sets them after replicating replica 0."""
+    """Per-replica reward function / spectral-norm flag (one value or R values; R equal values are the uniform path). A replica without
+    spectral norm never reads or writes its u / v rows. Trainer(fast_init=True) sets them after replicating replica 0."""
     R = self.replicas
     rf_list, sn_list = _per_replica_choice(reward_function, R), [bool(x) for x in _per_replica_choice(spectral_norm, R)]
     for x in rf_list: assert x in _lib.REWARD, f'reward_function {x!r} not in {sorted(_lib.REWARD)}'
-    assert not any(sn_list) or self.u is not None, 'spectral norm needs the u / v buffers (construct with spectral_norm on for some replica)'
+    has_uv = (self.g_u if self.general else self.u) is not None
+    assert not any(sn_list) or has_uv, 'spectral norm needs the u / v buffers (construct with spectral_norm on for some replica)'
     self.reward_function, self.spectral_norm = rf_list[0], any(sn_list)
     self._reward_function_r = torch.tensor([_lib.REWARD[x] for x in rf_list], dtype=torch.int32, device=self.device) if len(set(rf_list)) > 1 else None
     if len(set(sn_list)) > 1:
@@ -511,10 +513,14 @@ class GAILDiscriminator(_Module):
       self._spectral_norm_r = torch.tensor(sn_list, dtype=torch.int32, device=self.device)
     else:
       self.spectral_norm_r, self._spectral_norm_r = None, None
-      if self.u is not None and not sn_list[0]: self.u, self.v = None, None
+      if has_uv and not sn_list[0]:
+        if self.general: self.g_u, self.g_v, self.h_u, self.h_v = None, None, None, None
+        else: self.u, self.v = None, None
 
   # ---- general configuration (models.py:157-162): flat [R, g | h] parameter buffer, per-net spectral-norm vectors ----------------
-  def _init_general(self, model_cfg, rng, device, H):
+  def _init_general(self, model_cfg, rng, device, H, sn_list):
+    """u / v rows exist for every replica when any replica uses spectral norm; replica r draws its own (shifting its later draws) only where
+    its flag is set, as its single run does, and the rows of the others stay zero."""
     R, S, A = self.replicas, self.state_size, self.action_size
     din, depth, act = (S if self.state_only else S + A), model_cfg.depth, model_cfg.activation
     self.activation = act
@@ -531,12 +537,12 @@ class GAILDiscriminator(_Module):
       self.h_mlp = ReplicaMLP(self.h_dims, act, R, 1, self.device)
       self.h_mlp.flat, self.h_mlp.stride = self.flat[:, g_total:], g_total + h_total
     self.mlp = self.g_mlp  # parameters() / generic helpers see the flat buffer through g
-    sn = self.spectral_norm
-    mk = lambda dims: (torch.zeros(R, sum(dims[1:]), device=self.device), torch.zeros(R, sum(dims[:-1]), device=self.device)) if sn else (None, None)
+    sn_any = self.spectral_norm
+    mk = lambda dims: (torch.zeros(R, sum(dims[1:]), device=self.device), torch.zeros(R, sum(dims[:-1]), device=self.device)) if sn_any else (None, None)
     self.g_u, self.g_v = mk(self.g_dims)
     self.h_u, self.h_v = mk(self.h_dims) if self.h_dims else (None, None)
 
-    def fcnn(dims):  # _create_fcnn (:48-69): per layer Linear() draws, orthogonal_, zero bias, then the u / v draws of spectral_norm
+    def fcnn(dims, sn):  # _create_fcnn (:48-69): per layer Linear() draws, orthogonal_, zero bias, then the u / v draws of spectral_norm
       params, us, vs = [], [], []
       for l in range(len(dims) - 1):
         layer = torch.nn.Linear(dims[l], dims[l + 1])
@@ -549,6 +555,7 @@ class GAILDiscriminator(_Module):
       return params, us, vs
 
     for r in range(R):
+      sn = sn_list[r]
       with (rng.replica(r) if rng is not None else _null_ctx()):
         if self.reward_shaping:  # :158-160: g is a plain nn.Linear (default init), then h
           lin = torch.nn.Linear(din, 1)
@@ -556,11 +563,11 @@ class GAILDiscriminator(_Module):
           if sn:
             u_, v_ = _spectral_norm_init(gp[0])
             gu, gv = [u_], [v_]
-          hp, hu, hv = fcnn(self.h_dims)
+          hp, hu, hv = fcnn(self.h_dims, sn)
           self.h_mlp.load_params(r, 0, hp)
           if sn: self.h_u[r].copy_(torch.cat(hu)); self.h_v[r].copy_(torch.cat(hv))
         else:
-          gp, gu, gv = fcnn(self.g_dims)
+          gp, gu, gv = fcnn(self.g_dims, sn)
         self.g_mlp.load_params(r, 0, gp)
         if sn: self.g_u[r].copy_(torch.cat(gu)); self.g_v[r].copy_(torch.cat(gv))
     self.training = True
@@ -573,11 +580,13 @@ class GAILDiscriminator(_Module):
       d.g_u, d.g_v, d.g_u_stride, d.g_v_stride = self.g_u.data_ptr(), self.g_v.data_ptr(), self.g_u.stride(0), self.g_v.stride(0)
       if self.h_mlp is not None: d.h_u, d.h_v, d.h_u_stride, d.h_v_stride = self.h_u.data_ptr(), self.h_v.data_ptr(), self.h_u.stride(0), self.h_v.stride(0)
     d.state_only, d.reward_function, d.subtract_log_policy = int(self.state_only), _lib.REWARD[self.reward_function], int(self.subtract_log_policy)
+    d.reward_function_r, d.spectral_norm_r = _lib.ptr(self._reward_function_r), _lib.ptr(self._spectral_norm_r)
     if isinstance(self.discount, (int, float)): d.discount = self.discount
     else: d.discount_r = self.discount.data_ptr()  # per-replica shaping discount: an [R] float32 device tensor
     return d
 
-  def _general_state_items(self):
+  def _general_state_items(self, spectral_norm: Optional[bool] = None):
+    sn = self.spectral_norm if spectral_norm is None else spectral_norm
     out = []
     for name, mlp, u, v, seq in (('g', self.g_mlp, self.g_u, self.g_v, not self.reward_shaping), ('h', self.h_mlp, self.h_u, self.h_v, True)):
       if mlp is None: continue
@@ -585,7 +594,7 @@ class GAILDiscriminator(_Module):
       for l in range(mlp.n_layers):
         pre = f'{name}.{2 * l}' if seq else name  # nn.Sequential indices: Linear, activation, Linear, ... (no dropout modules: models.py:160,162)
         od, idim = mlp.dims[l + 1], mlp.dims[l]
-        if self.spectral_norm:
+        if sn:
           out += [(f'{pre}.bias', views[2 * l + 1]), (f'{pre}.parametrizations.weight.original', views[2 * l]), (f'{pre}.parametrizations.weight.0._u', u[:, uo:uo + od]),
                   (f'{pre}.parametrizations.weight.0._v', v[:, vo:vo + idim])]
         else:
@@ -642,7 +651,7 @@ class GAILDiscriminator(_Module):
       if rows is not None: v[rows] = dst
 
   def _state_items(self, spectral_norm: Optional[bool] = None, hidden_size: Optional[int] = None):
-    if self.general: return self._general_state_items()
+    if self.general: return self._general_state_items(spectral_norm)
     if hidden_size is None and self.hidden_size_r is not None:
       raise ValueError('per-replica discriminator widths have no common layout: pass hidden_size (a replica block\'s width) and slice that block')
     d, H = self.mlp.dims[0], self.mlp.dims[1] if hidden_size is None else int(hidden_size)

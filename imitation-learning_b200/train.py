@@ -138,6 +138,13 @@ class Trainer:
                                                                                              'imitation.pos_class_prior', 'imitation.nonnegative_margin') if k in pr}))
     if 'imitation.loss_function' in pr: self.imitation_cfg.loss_function = list(pr['imitation.loss_function'])  # one name per replica
     self._grad_penalty_on = max(pr.get('imitation.grad_penalty', [cfg.imitation.get('grad_penalty', 0)])) > 0  # GAIL only (GAIL.yaml)
+    # the general discriminator's per-replica arrays (il_gailx_update_args), made once before any graph capture: the loss-function codes and the
+    # replicas that take the gradient-penalty pass (grad_penalty > 0; the others run as a single run without a penalty)
+    self.gail_penalty_pass = None
+    if self.algorithm == 'GAIL' and self.discriminator.general:
+      from .training import _choice_codes
+      if 'imitation.loss_function' in pr: _choice_codes(self.discriminator, 'loss_function', pr['imitation.loss_function'], _lib.LOSS)
+      if 'imitation.grad_penalty' in pr: self.gail_penalty_pass = torch.tensor([int(x > 0) for x in pr['imitation.grad_penalty']], dtype=torch.int32, device=dev)
     # the Mixup noise (training.py:106) is drawn for every replica when any replica uses Mixup: U(0, 1) when every alpha is 1, Beta(alpha_r, alpha_r)
     # otherwise (equal to the uniform draw where alpha_r is 1)
     self._mixup_on = self.algorithm == 'GAIL' and 'Mixup' in pr.get('imitation.loss_function', [cfg.imitation.get('loss_function')])
@@ -283,7 +290,7 @@ class Trainer:
         eps_mix = self.eps_mix
       self.discriminator.train()  # train.py:178-180
       adversarial_imitation_update(self.actor, self.discriminator, self.batch, self.expert_batch, self.discriminator_optimiser, self.imitation_cfg, eps_gp=self.eps_gp,
-                                   eps_mix=eps_mix, out_losses=self.gail_losses)
+                                   eps_mix=eps_mix, out_losses=self.gail_losses, penalty_pass=self.gail_penalty_pass)
       self.discriminator.eval()
     if self.algorithm in ('GAIL', 'GMMIL'):
       if cfg.imitation.mix_expert_data == 'mixed_batch':

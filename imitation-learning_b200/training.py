@@ -91,12 +91,18 @@ def sac_update(actor: SoftActor, critic: TwinCritic, log_alpha: Tensor, target_c
 
 
 def adversarial_imitation_update(actor: SoftActor, discriminator: GAILDiscriminator, transitions, expert_transitions, discriminator_optimiser: Adam, imitation_cfg,
-                                 eps_gp: Optional[Tensor] = None, eps_mix: Optional[Tensor] = None, out_losses: Optional[Tensor] = None):
+                                 eps_gp: Optional[Tensor] = None, eps_mix: Optional[Tensor] = None, out_losses: Optional[Tensor] = None,
+                                 penalty_pass: Optional[Tensor] = None):
   """training.py:85-134. `eps_gp` injects the U(0,1) draw of :118 and `eps_mix` the Beta draw of :106.
 
-  imitation_cfg.loss_function is a name or one name per replica; mixup_alpha, pos_class_prior and nonnegative_margin are floats or [R] values
-  (per-replica loss function, prior and margin need the fused discriminator). Without `eps_mix`, a scalar mixup_alpha draws as in the
-  reference (U(0, 1) on the device at 1, torch's Beta otherwise) and per-replica values draw Beta(alpha_r, alpha_r) on the device."""
+  imitation_cfg.loss_function is a name or one name per replica; mixup_alpha, pos_class_prior and nonnegative_margin are floats or [R] values.
+  Without `eps_mix`, a scalar mixup_alpha draws as in the reference (U(0, 1) on the device at 1, torch's Beta otherwise) and per-replica values
+  draw Beta(alpha_r, alpha_r) on the device.
+
+  penalty_pass ([R] int32 device tensor of 0 / 1, general discriminator only): replica r takes part in the gradient-penalty pass only where it
+  is 1, so a replica whose grad_penalty is 0 runs as a call without a penalty (Trainer passes grad_penalty > 0). None: with per-replica
+  grad_penalty every replica takes the pass, its spectral-norm power iterations included. The fused discriminator always skips the pass for
+  replicas at 0."""
   R, device = discriminator.replicas, discriminator.device
   pol, _ = _as_batch(transitions, device)
   exp, _ = _as_batch(expert_transitions, device)
@@ -117,9 +123,9 @@ def adversarial_imitation_update(actor: SoftActor, discriminator: GAILDiscrimina
   eps_gp, eps_mix = as_dev(eps_gp), as_dev(eps_mix)
   hyper = (grad_penalty, grad_penalty_r, entropy_bonus, entropy_bonus_r)
   if discriminator.general:
-    if loss_function is None or pos_class_prior_r is not None or nonnegative_margin_r is not None:
-      raise ValueError('per-replica loss_function / pos_class_prior / nonnegative_margin need the fused discriminator (depth 1, relu, no shaping or log-policy term)')
-    return _general_adversarial_update(actor, discriminator, pol, exp, discriminator_optimiser, imitation_cfg, hyper, eps_gp, eps_mix, out_losses)
+    loss_codes = None if loss_function is not None else _choice_codes(discriminator, 'loss_function', losses, _lib.LOSS)
+    pu = (pos_class_prior, pos_class_prior_r, nonnegative_margin, nonnegative_margin_r)
+    return _general_adversarial_update(actor, discriminator, pol, exp, discriminator_optimiser, losses, loss_codes, pu, hyper, eps_gp, eps_mix, out_losses, penalty_pass)
   a = _lib.GailUpdateArgs()
   a.disc, a.opt, a.policy, a.expert = discriminator.c_struct(), discriminator_optimiser.c_struct(), pol.c_struct(), exp.c_struct()
   a.eps_gp, a.eps_mix, a.R, a.loss_function, a.training = _lib.ptr(eps_gp), _lib.ptr(eps_mix), R, _lib.LOSS[losses[0]], int(discriminator.training)
@@ -130,29 +136,34 @@ def adversarial_imitation_update(actor: SoftActor, discriminator: GAILDiscrimina
   _lib.check(_lib.lib().il_gail_update(_lib.handle(), C.byref(a), _lib.stream()))
 
 
-def _general_adversarial_update(actor, disc: GAILDiscriminator, pol: TransitionBatch, exp: TransitionBatch, opt: Adam, imitation_cfg, hyper, eps_gp, eps_mix, out_losses):
+def _general_adversarial_update(actor, disc: GAILDiscriminator, pol: TransitionBatch, exp: TransitionBatch, opt: Adam, losses, loss_codes, pu, hyper, eps_gp, eps_mix,
+                                out_losses, penalty_pass):
   """training.py:85-134 for the non-default discriminator configurations (reward shaping, subtract_log_policy, depth > 1, tanh / sigmoid):
-  the log-policy inputs of make_gail_input (models.py:148, evaluated under no_grad) are computed first, then one il_gailx_update call."""
+  the log-policy inputs of make_gail_input (models.py:148, evaluated under no_grad) of every pass that runs are computed first, then one
+  il_gailx_update call. With per-replica loss functions (loss_codes) the policy and expert passes always run and the Mixup pass runs when any
+  replica is Mixup."""
   R, B, device, lib = disc.replicas, pol.B, disc.device, _lib.lib()
-  loss_function = imitation_cfg.loss_function
+  mixup = 'Mixup' in losses
+  passes = ('policy', 'expert') + (('mix', ) if mixup else ()) if loss_codes is not None else ('mix', ) if mixup else ('policy', 'expert')
+  if loss_codes is not None and not mixup: eps_mix = None  # the Mixup pass runs when eps_mix is passed
   logp = {}
   if disc.subtract_log_policy:
     lp = lambda tb: actor._run(tb.rows[..., :tb.S], given=tb.rows[..., tb.S:tb.S + tb.A], want=('log_prob', ))['log_prob']
-    if loss_function == 'Mixup':  # make_gail_input on the mixed state / action (training.py:107-108)
+    if 'policy' in passes: logp['policy'], logp['expert'] = lp(pol), lp(exp)
+    if 'mix' in passes:  # make_gail_input on the mixed state / action (training.py:107-108)
       mix = TransitionBatch(torch.empty_like(pol.rows), pol.S, pol.A, pol.absorbing)
       e, p_, m = exp.c_struct(), pol.c_struct(), mix.c_struct()
       _lib.check(lib.il_gail_mix_batch(_lib.handle(), C.byref(e), C.byref(p_), eps_mix.data_ptr(), R, C.byref(m), _lib.stream()))
       logp['mix'] = lp(mix)
-    else:
-      logp['policy'], logp['expert'] = lp(pol), lp(exp)
   a = _lib.GailxUpdateArgs()
   a.disc, a.opt, a.params_floats, a.policy, a.expert = disc.cx_struct(), opt.c_struct(), disc.flat.numel(), pol.c_struct(), exp.c_struct()
   a.eps_gp, a.eps_mix = _lib.ptr(eps_gp), _lib.ptr(eps_mix)
   a.logp_policy, a.logp_expert, a.logp_mix = _lib.ptr(logp.get('policy')), _lib.ptr(logp.get('expert')), _lib.ptr(logp.get('mix'))
-  a.R, a.loss_function, a.training = R, _lib.LOSS[loss_function], int(disc.training)
+  a.R, a.loss_function, a.training, a.loss_function_r = R, _lib.LOSS[losses[0]], int(disc.training), _lib.ptr(loss_codes)
   grad_penalty, grad_penalty_r, entropy_bonus, entropy_bonus_r = hyper
   a.grad_penalty, a.grad_penalty_r, a.entropy_bonus, a.entropy_bonus_r = grad_penalty, _lib.ptr(grad_penalty_r), entropy_bonus, _lib.ptr(entropy_bonus_r)
-  a.pos_class_prior, a.nonnegative_margin = float(imitation_cfg.pos_class_prior), float(imitation_cfg.nonnegative_margin)
+  a.pos_class_prior, a.pos_class_prior_r, a.nonnegative_margin, a.nonnegative_margin_r = pu[0], _lib.ptr(pu[1]), pu[2], _lib.ptr(pu[3])
+  a.penalty_pass_r = _lib.ptr(penalty_pass)
   a.out_losses = _lib.ptr(out_losses)
   need = lib.il_gailx_workspace_bytes(C.byref(a))
   ws = _workspace(disc, 'gailx', need, device)

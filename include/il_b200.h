@@ -366,6 +366,11 @@ typedef struct il_gailx {
   int32_t subtract_log_policy;      /* models.py:175 */
   float   discount;                 /* models.py:174 */
   const float* discount_r;          /* [R] per-replica shaping discount; NULL = discount */
+  /* [R] per-replica values as in il_gail, read by il_gailx_update and il_gailx_reward; NULL = the scalar / the g_u != NULL test.
+   * spectral_norm_r (0 / 1) needs g_u / g_v for every replica (and h_u / h_v with reward shaping); a replica at 0 never reads or writes its
+   * u / v rows and takes sigma = 1 (W_eff = W / 1), as a run without spectral norm computes. */
+  const int32_t* reward_function_r; /* IL_REWARD_* */
+  const int32_t* spectral_norm_r;
 } il_gailx;
 typedef struct il_gailx_update_args {
   il_gailx disc;
@@ -382,10 +387,22 @@ typedef struct il_gailx_update_args {
   float* out_losses;                /* [R, 2] (may be NULL) */
   void*   workspace;                /* il_gailx_workspace_bytes */
   int64_t workspace_bytes;
-  /* as in il_gail_update_args. The gradient-penalty pass of this program is batched over replicas: a replica whose value is 0 gets no
-   * penalty contribution, but its spectral-norm vectors still take the pass's power iteration, so sweeps keep grad_penalty uniform here. */
+  /* as in il_gail_update_args: with grad_penalty_r the gradient-penalty pass runs when eps_gp is passed. The pass is batched over replicas;
+   * which replicas take part in it is penalty_pass_r's choice (below). */
   const float* grad_penalty_r;
   const float* entropy_bonus_r;
+  /* [R] per-replica loss function (IL_LOSS_*), PUGAIL prior and margin; NULL = the scalar. With loss_function_r the program runs the policy
+   * and expert passes, then the Mixup pass when eps_mix is passed (the caller passes it when any replica is Mixup), then the penalty pass:
+   * a Mixup replica lives in the Mixup pass only, a BCE / PUGAIL replica in the policy and expert passes only. A replica's dead passes run
+   * no power iteration, leave its u / v alone and add nothing to its gradient, so each replica sees its single run's sequence of accesses.
+   * With subtract_log_policy the caller passes logp_policy and logp_expert, and logp_mix with eps_mix. */
+  const int32_t* loss_function_r;
+  const float* pos_class_prior_r;
+  const float* nonnegative_margin_r;
+  /* [R] 0 / 1: replica r takes part in the gradient-penalty pass (its spectral-norm accesses, power iterations included, its penalty loss and
+   * gradient) only where it is 1; elsewhere it runs as a uniform call without a penalty and its out_losses[r, 1] is left alone. NULL: every
+   * replica takes the pass when it runs (a replica whose grad_penalty_r is 0 then adds a zero penalty but takes the power iterations). */
+  const int32_t* penalty_pass_r;
 } il_gailx_update_args;
 int64_t il_gailx_workspace_bytes(const il_gailx_update_args* a);
 int il_gailx_update(il_handle* h, const il_gailx_update_args* a, void* stream);      /* training.py:85-134 */
