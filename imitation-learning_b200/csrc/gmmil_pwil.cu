@@ -199,7 +199,7 @@ __global__ void __launch_bounds__(256) pwil_reward_kernel(const il_pwil p, int R
       if (tid == 0) { w[best] = -1.f; dists[best] = INFINITY; }
     } else {  // models.py:246-248
       cost += weight * dd;
-      if (tid == 0) w[best] = (float)((double)w[best] - weight);
+      if (tid == 0) w[best] = w[best] - (float)weight;  // models.py:247 on a float32 tensor: the scalar is rounded to float32, then subtracted in float32
       weight = 0.0;
     }
     __syncthreads();

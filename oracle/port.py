@@ -436,7 +436,7 @@ class RewardRelabeller:
 def squared_distance_mean(x: Tensor, y: Tensor) -> Tensor:
   """models.py:25-28: pairwise MEAN (over features) squared difference, [n1, n2]. Computed blockwise so the
   [n1, n2, d] tensor of the reference is never held in full; the arithmetic per entry is the same."""
-  out = torch.empty(x.size(0), y.size(0))
+  out = torch.empty(x.size(0), y.size(0), dtype=x.dtype)
   for i in range(0, x.size(0), 64):
     out[i:i + 64] = (x[i:i + 64, None, :] - y[None, :, :]).pow(2).mean(dim=2)
   return out
