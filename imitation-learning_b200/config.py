@@ -9,7 +9,7 @@ import itertools
 import os
 import re
 from dataclasses import dataclass, field
-from typing import Any, Dict, List, Optional, Sequence, Tuple
+from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple
 
 import yaml
 
@@ -87,8 +87,9 @@ def load_config(overrides: Optional[List[str]] = None, conf_dir: str = CONF_DIR)
 
 # ---- multirun (Hydra's basic sweeper) ------------------------------------------------------------------------------------------
 MULTIRUN_FLAGS = ('-m', '--multirun')
-# Scalars that leave every tensor shape unchanged: a sweep over them runs as per-replica values of one program (Trainer(per_replica=...)).
-# Every other swept key is a grouping key: jobs that differ in one run as separate programs.
+# The keys that can take per-replica values (Trainer(per_replica=...)), in groups. PER_REPLICA_KEYS, built from these groups, gives each key's role
+# in a configuration and the values it accepts. Every other swept key is a grouping key: jobs that differ in one run as separate programs.
+# Scalars that leave every tensor shape unchanged: a sweep over them runs as per-replica values of one program.
 VECTORISED = ('training.learning_rate', 'training.weight_decay', 'reinforcement.discount', 'reinforcement.target_temperature', 'reinforcement.polyak_factor',
               'imitation.learning_rate', 'imitation.weight_decay', 'imitation.grad_penalty', 'imitation.entropy_bonus', 'bc_pretraining.learning_rate',
               'bc_pretraining.weight_decay')
@@ -96,17 +97,14 @@ VECTORISED = ('training.learning_rate', 'training.weight_decay', 'reinforcement.
 # replica branches on them). group_jobs gives the general discriminator (csrc/gail_general.cu) only the Mixup alpha per replica.
 PER_REPLICA_DISCRIMINATOR = ('imitation.loss_function', 'imitation.discriminator.reward_function', 'imitation.spectral_norm', 'imitation.mixup_alpha',
                              'imitation.pos_class_prior', 'imitation.nonnegative_margin')
-# The general discriminator's choices that sweep_groups makes per replica (general_discriminator_keys): its program runs every loss pass any
-# replica needs and masks each replica's dead passes, accesses and penalty pass out (il_gailx_update_args.loss_function_r / penalty_pass_r), so
-# each replica sees the sequence of power iterations and gradient sums of its single run.
+# The general discriminator's choices that sweep_groups makes per replica: its program runs every loss pass any replica needs and masks each
+# replica's dead passes, accesses and penalty pass out (il_gailx_update_args.loss_function_r / penalty_pass_r), so each replica sees the
+# sequence of power iterations and gradient sums of its single run.
 PER_REPLICA_GENERAL_DISCRIMINATOR = ('imitation.loss_function', 'imitation.discriminator.reward_function', 'imitation.spectral_norm', 'imitation.pos_class_prior',
                                      'imitation.nonnegative_margin', 'imitation.grad_penalty')
 # The fused GAIL discriminator's hidden size: a per-replica shape (each replica keeps a single run's layout inside the stride of the widest; one
 # launch per width class), with at most MAX_WIDTH_CLASSES distinct widths in one program. The general discriminator groups on it.
 PER_REPLICA_WIDTH = ('imitation.discriminator.hidden_size', )
-# Keys an algorithm never reads: jobs that differ only in them are the same run (GAILDiscriminator never passes its dropout to _create_fcnn,
-# models.py:157-162), so they neither split groups nor become per-replica values.
-UNUSED_KEYS = {'GAIL': ('imitation.discriminator.input_dropout', 'imitation.discriminator.dropout')}
 # Other algorithms' own search-space keys that change no shape and no random draw: AdRIL's update frequency and balanced sampling
 # (adril_relabel_kernel reads them per replica), PWIL's reward scale and bandwidth scale (pwil_reward_kernel), DRIL's quantile cutoff (the
 # per-replica threshold q, computed once after pre-training). PWIL's scales are per replica only with imitation.mix_expert_data == 'none':
@@ -121,12 +119,11 @@ PER_REPLICA_ALGORITHM = {'AdRIL': ('imitation.update_freq', 'imitation.balanced'
 PER_REPLICA_SEED = ('seed', )
 # RED's and DRIL's dropout rates and activation: per-replica values of the dropout program (csrc/dropout_nets.cu: the mask fill reads each replica's
 # rate, the activation passes each replica's activation). Only whether a rate is 0 is structural (the nn.Sequential indices and state_dict keys,
-# which mask draws happen, and for DRIL whether the dropout program runs at all), so sweep_groups groups on that presence (_dropout_presence) and
+# which mask draws happen, and for DRIL whether the dropout program runs at all), so sweep_groups groups on that presence and
 # Trainer(per_replica=...) refuses a mix of 0 and > 0 for one site. DRIL's activation is per replica only with a dropout site: without one the
 # policy runs on the fused MLP kernels, which take one activation. Like `seed`, these keys are per replica in sweep_groups only (per_replica_keys).
+# GAIL never reads the two rates (GAILDiscriminator never passes its dropout to _create_fcnn, models.py:157-162): there they are ignored.
 PER_REPLICA_DROPOUT = ('imitation.discriminator.input_dropout', 'imitation.discriminator.dropout', 'imitation.discriminator.activation')
-_ACTIVATIONS = ('relu', 'sigmoid', 'tanh')  # models.py:17 ACTIVATION_FUNCTIONS
-_CHOICES = {'imitation.loss_function': ('BCE', 'Mixup', 'PUGAIL'), 'imitation.discriminator.reward_function': ('AIRL', 'FAIRL', 'GAIL')}
 _SWEEP_FUNCTIONS = re.compile(r'^(range|choice|interval|glob|sort|shuffle|tag)\s*\(')
 
 
@@ -201,56 +198,18 @@ def expand_sweep(argv: Sequence[str]) -> Tuple[bool, List[SweepJob]]:
   return True, [SweepJob(i, list(c)) for i, c in enumerate(itertools.product(*choices))]
 
 
-def general_discriminator(cfg: Config) -> bool:
-  """Whether a GAIL configuration runs on the general discriminator (csrc/gail_general.cu): reward shaping, the log-policy term, depth != 1 or an
-  activation other than relu (models.GAILDiscriminator.general)."""
-  d = cfg.imitation.get('discriminator') or {}
-  return cfg.get('algorithm') == 'GAIL' and bool(d.get('reward_shaping') or d.get('subtract_log_policy') or d.get('depth', 1) != 1 or d.get('activation', 'relu') != 'relu')
+# ---- the per-replica key table -------------------------------------------------------------------------------------------------
+# A key's role in one configuration (PerReplicaKey.role). A key without one is a grouping key: jobs that differ in it run as separate programs.
+BOTH = 'both'        # per replica in group_jobs and sweep_groups (vectorised_keys)
+SWEEP = 'sweep'      # per replica in sweep_groups only (per_replica_keys): group_jobs groups on it
+IGNORED = 'ignored'  # no path of the configuration reads it: jobs that differ only in it are the same run
 
 
-def vectorised_keys(cfg: Config) -> Tuple[str, ...]:
-  """VECTORISED minus the keys a path of this configuration cannot take per replica, plus the discriminator choices for GAIL and the
-  algorithm's own keys of PER_REPLICA_ALGORITHM: for the general GAIL discriminator (csrc/gail_general.cu) this partition keeps grad_penalty
-  and every choice but mixup_alpha grouping keys (sweep_groups makes them per replica through general_discriminator_keys); PWIL takes its scales per replica only without expert-data mixing (the expert memory's relabelled rewards
-  depend on them and are shared)."""
-  gail, general = cfg.get('algorithm') == 'GAIL', general_discriminator(cfg)
-  keys = tuple(k for k in VECTORISED if not (general and k == 'imitation.grad_penalty'))
-  if gail: keys += ('imitation.mixup_alpha', ) if general else PER_REPLICA_DISCRIMINATOR + PER_REPLICA_WIDTH
-  alg = cfg.get('algorithm')
-  if alg in PER_REPLICA_ALGORITHM and not (alg == 'PWIL' and cfg.imitation.get('mix_expert_data', 'none') != 'none'): keys += PER_REPLICA_ALGORITHM[alg]
-  return keys
-
-
-def per_replica_keys(cfg: Config) -> Tuple[str, ...]:
-  """Every key Trainer(per_replica=...) takes in this configuration: vectorised_keys plus `seed` where it can be per replica (seed_per_replica),
-  RED's / DRIL's dropout keys (dropout_keys) and the general GAIL discriminator's choices (general_discriminator_keys)."""
-  return vectorised_keys(cfg) + (PER_REPLICA_SEED if seed_per_replica(cfg) else ()) + dropout_keys(cfg) + general_discriminator_keys(cfg)
-
-
-def general_discriminator_keys(cfg: Config) -> Tuple[str, ...]:
-  """PER_REPLICA_GENERAL_DISCRIMINATOR for a GAIL configuration on the general discriminator, else nothing. Like `seed` and the dropout keys,
-  these are per replica in sweep_groups only: group_jobs keeps them grouping keys."""
-  return PER_REPLICA_GENERAL_DISCRIMINATOR if general_discriminator(cfg) else ()
-
-
-def dropout_keys(cfg: Config) -> Tuple[str, ...]:
-  """The keys of PER_REPLICA_DROPOUT this configuration takes per replica: all three for RED; for DRIL the rates, and the activation when the
-  policy has a dropout site."""
-  alg = cfg.get('algorithm')
-  if alg == 'RED': return PER_REPLICA_DROPOUT
-  if alg != 'DRIL': return ()
-  d = cfg.imitation.get('discriminator') or {}
-  return PER_REPLICA_DROPOUT if any(_positive(d.get(k)) for k in ('input_dropout', 'dropout')) else PER_REPLICA_DROPOUT[:2]
-
-
-def _positive(x: Any) -> bool:
-  return isinstance(x, (int, float)) and not isinstance(x, bool) and x > 0
-
-
-def _dropout_presence(cfg: Config, keys) -> Tuple:
-  """Whether each dropout site whose rate is a per-replica key is present (rate > 0): the structural part of a rate, a grouping key."""
-  d = cfg.imitation.get('discriminator') or {}
-  return tuple((k, _positive(d.get(k.rsplit('.', 1)[1]))) for k in PER_REPLICA_DROPOUT[:2] if k in keys)
+def general_discriminator(discriminator: Optional[Dict[str, Any]]) -> bool:
+  """Whether a GAIL discriminator with this config (imitation.discriminator) runs on the general program (csrc/gail_general.cu) rather than the
+  fused one (csrc/gail.cu): reward shaping, the log-policy term, depth != 1 or an activation other than relu."""
+  d = discriminator or {}
+  return bool(d.get('reward_shaping') or d.get('subtract_log_policy') or d.get('depth', 1) != 1 or d.get('activation', 'relu') != 'relu')
 
 
 def needs_expert_memory(cfg: Config) -> bool:
@@ -258,9 +217,100 @@ def needs_expert_memory(cfg: Config) -> bool:
   return cfg.get('algorithm') != 'SAC' or cfg.bc_pretraining.get('iterations', 0) > 0 or bool(cfg.imitation.get('bc_aux_loss', False))
 
 
+def _refuse(why: str):
+  raise ValueError(why)
+
+
+def _number(what: str = '', ok=lambda x: True):
+  """A number, as a float that ok accepts."""
+  def check(x):
+    if isinstance(x, (bool, str)): _refuse('not a number')
+    try:
+      v = float(x)
+    except (TypeError, ValueError):
+      _refuse('not a number')
+    return v if ok(v) else _refuse(f'not {what}')
+  return check
+
+
+# The conditions under which a key's role differs between configurations (the comments on the key groups above give the reasons)
+_positive = lambda x: isinstance(x, (int, float)) and not isinstance(x, bool) and x > 0
+_algorithm = lambda *names: lambda cfg: cfg.get('algorithm') in names
+_general = lambda cfg: cfg.get('algorithm') == 'GAIL' and general_discriminator(cfg.imitation.get('discriminator'))
+_fused = lambda cfg: cfg.get('algorithm') == 'GAIL' and not _general(cfg)
+_pwil_without_expert_mixing = lambda cfg: cfg.get('algorithm') == 'PWIL' and cfg.imitation.get('mix_expert_data', 'none') == 'none'
+_dropout_program = lambda cfg: cfg.get('algorithm') == 'RED' or (cfg.get('algorithm') == 'DRIL' and any(_positive(get_key(cfg, k)) for k in PER_REPLICA_DROPOUT[:2]))
+_device_rng = lambda cfg: bool(cfg.get('device_rng', True))
+_subsampled_expert_memory = lambda cfg: cfg.imitation.get('subsample', 1) > 1 and needs_expert_memory(cfg)
+# The values a key accepts: each check returns a replica's value in its canonical type or raises ValueError(why not)
+_names = lambda *names: lambda x: x if x in names else _refuse(f'not one of {", ".join(names)}')
+_flag = lambda x: x if isinstance(x, bool) else _refuse('not true / false')
+_integer = lambda what, ok: lambda x: x if isinstance(x, int) and not isinstance(x, bool) and ok(x) else _refuse(f'not {what}')
+_NON_NEGATIVE, _RATE = _number('>= 0', lambda x: x >= 0), _number('in [0, 1)', lambda x: 0 <= x < 1)
+# Every key whose values are not simply numbers: the reference's choices (train.py:42,44), activations (models.py:17) and ranges (train.py:37,39,48-49),
+# the seeds np.random.seed takes (train.py:51), and the dropout rates nn.Dropout takes without scaling by 1 / 0.
+_VALUES = {'imitation.grad_penalty': _NON_NEGATIVE, 'imitation.entropy_bonus': _NON_NEGATIVE, 'imitation.loss_function': _names('BCE', 'Mixup', 'PUGAIL'),
+           'imitation.discriminator.reward_function': _names('AIRL', 'FAIRL', 'GAIL'), 'imitation.spectral_norm': _flag,
+           'imitation.discriminator.hidden_size': _integer('a positive integer', lambda x: x > 0), 'imitation.update_freq': _integer('an integer >= 0', lambda x: x >= 0),
+           'imitation.balanced': _flag, 'imitation.quantile_cutoff': _number('in [0, 1]', lambda x: 0 <= x <= 1),
+           'seed': _integer('an integer in [0, 2**32)', lambda x: 0 <= x < 2**32), 'imitation.discriminator.input_dropout': _RATE,
+           'imitation.discriminator.dropout': _RATE, 'imitation.discriminator.activation': _names('relu', 'sigmoid', 'tanh')}
+# Each group of keys with its role and the configurations it holds in. A key in several rows takes the last role that holds.
+_ROLES = ((VECTORISED, BOTH, lambda cfg: True),
+          (PER_REPLICA_DISCRIMINATOR, BOTH, _algorithm('GAIL')),
+          (PER_REPLICA_GENERAL_DISCRIMINATOR, SWEEP, _general),
+          (PER_REPLICA_WIDTH, BOTH, _fused),
+          (PER_REPLICA_ALGORITHM['AdRIL'], BOTH, _algorithm('AdRIL')),
+          (PER_REPLICA_ALGORITHM['PWIL'], BOTH, _pwil_without_expert_mixing),
+          (PER_REPLICA_ALGORITHM['DRIL'], BOTH, _algorithm('DRIL')),
+          (PER_REPLICA_SEED, SWEEP, lambda cfg: _device_rng(cfg) and not _subsampled_expert_memory(cfg)),
+          (PER_REPLICA_DROPOUT[:2], SWEEP, _algorithm('RED', 'DRIL')),
+          (PER_REPLICA_DROPOUT[:2], IGNORED, _algorithm('GAIL')),
+          (PER_REPLICA_DROPOUT[2:], SWEEP, _dropout_program))
+
+
+@dataclass(frozen=True)
+class PerReplicaKey:
+  roles: Tuple[Tuple[str, Callable[[Config], bool]], ...]  # (role, the configurations it holds in), the last that holds wins
+  value: Callable[[Any], Any]                              # a replica's value -> its canonical value; ValueError for a value the key refuses
+  structural: bool                                         # whether `value > 0` is structural: sweep_groups groups on it, replicas may not mix 0 and > 0
+
+  def role(self, cfg: Config) -> Optional[str]:
+    return next((r for r, holds in reversed(self.roles) if holds(cfg)), None)
+
+
+# key -> its entry, in the order the rows first name the keys; the dropout rates are the keys whose presence is structural
+PER_REPLICA_KEYS = {k: PerReplicaKey(tuple((r, holds) for ks, r, holds in _ROLES if k in ks), _VALUES.get(k, _number()), k in PER_REPLICA_DROPOUT[:2])
+                    for keys, _, _ in _ROLES for k in keys}
+
+
+def _keys_with(cfg: Config, role: str) -> Tuple[str, ...]:
+  return tuple(k for k, e in PER_REPLICA_KEYS.items() if e.role(cfg) == role)
+
+
+def vectorised_keys(cfg: Config) -> Tuple[str, ...]:
+  """The keys per replica in both partitions of this configuration (group_jobs and sweep_groups)."""
+  return _keys_with(cfg, BOTH)
+
+
+def per_replica_keys(cfg: Config) -> Tuple[str, ...]:
+  """Every key Trainer(per_replica=...) takes in this configuration: vectorised_keys, then the keys per replica in sweep_groups only."""
+  return vectorised_keys(cfg) + _keys_with(cfg, SWEEP)
+
+
+def general_discriminator_keys(cfg: Config) -> Tuple[str, ...]:
+  """PER_REPLICA_GENERAL_DISCRIMINATOR for a GAIL configuration on the general discriminator, else nothing."""
+  return tuple(k for k in PER_REPLICA_GENERAL_DISCRIMINATOR if PER_REPLICA_KEYS[k].role(cfg) == SWEEP)
+
+
+def dropout_keys(cfg: Config) -> Tuple[str, ...]:
+  """The keys of PER_REPLICA_DROPOUT this configuration takes per replica."""
+  return tuple(k for k in PER_REPLICA_DROPOUT if PER_REPLICA_KEYS[k].role(cfg) == SWEEP)
+
+
 def seed_per_replica(cfg: Config) -> bool:
   """Whether `seed` can take per-replica values in this configuration (PER_REPLICA_SEED)."""
-  return bool(cfg.get('device_rng', True)) and not (cfg.imitation.get('subsample', 1) > 1 and needs_expert_memory(cfg))
+  return PER_REPLICA_KEYS['seed'].role(cfg) == SWEEP
 
 
 def group_jobs(jobs: List[SweepJob], conf_dir: str = CONF_DIR) -> List[SweepGroup]:
@@ -276,8 +326,8 @@ def sweep_groups(jobs: List[SweepJob], conf_dir: str = CONF_DIR) -> List[SweepGr
 
 
 def _partition(jobs: List[SweepJob], conf_dir: str, keys_of) -> List[SweepGroup]:
-  """Jobs that agree on every swept key outside keys_of(config) form one group, in the order of their first job; the swept keys inside it
-  become per-job values."""
+  """Jobs that agree on every swept key outside keys_of(config) and on whether each structural key inside it is > 0 form one group, in the order
+  of their first job; the swept keys inside it become per-job values. Keys the configuration ignores separate no jobs."""
   swept = {}
   for j in jobs:
     for o in j.overrides:
@@ -288,9 +338,9 @@ def _partition(jobs: List[SweepJob], conf_dir: str, keys_of) -> List[SweepGroup]
   for j in jobs:
     ov = dict(o.partition('=')[::2] for o in j.overrides)
     cfg = load_config(j.overrides, conf_dir)
-    keys = keys_of(cfg)
-    vec = set(keys) | set(UNUSED_KEYS.get(cfg.get('algorithm'), ()))
-    key = tuple((k, ov.get(k)) for k in swept if k not in vec) + _dropout_presence(cfg, [k for k in swept if k in keys])
+    keys, ignored = keys_of(cfg), _keys_with(cfg, IGNORED)
+    key = tuple((k, ov.get(k)) for k in swept if k not in keys and k not in ignored)
+    key += tuple((k, _positive(get_key(cfg, k))) for k in swept if k in keys and PER_REPLICA_KEYS[k].structural)
     g = groups.setdefault(key, SweepGroup([]))
     g.jobs.append(j)
   for g in groups.values():
@@ -320,55 +370,19 @@ def _check_width_classes(k: str, vals: Sequence[Any]):
   if n > MAX_WIDTH_CLASSES: raise SweepError(f'{k}: {n} distinct widths in one program; the fused discriminator takes at most {MAX_WIDTH_CLASSES}')
 
 
-def _per_replica_value(k: str, x: Any) -> Any:
-  """A per-replica value as the config holds it: a name of _CHOICES[k], a bool for spectral_norm, a positive int for a width, a non-negative
-  int for a seed, a float otherwise."""
-  if k in PER_REPLICA_WIDTH:
-    if isinstance(x, bool) or not isinstance(x, int) or x <= 0: raise SweepError(f'{k}={x!r}: not a positive integer')
-    return x
-  if k in PER_REPLICA_SEED:  # np.random.seed (train.py:51) takes 0 <= seed < 2**32
-    if isinstance(x, bool) or not isinstance(x, int) or not 0 <= x < 2**32: raise SweepError(f'{k}={x!r}: not an integer in [0, 2**32)')
-    return x
-  if k in _CHOICES:
-    if x not in _CHOICES[k]: raise SweepError(f'{k}={x!r}: not one of {", ".join(_CHOICES[k])}')  # train.py:42,44
-    return x
-  if k == 'imitation.spectral_norm':
-    if not isinstance(x, bool): raise SweepError(f'{k}={x!r}: not true / false')
-    return x
-  if isinstance(x, (bool, str)): raise SweepError(f'{k}={x!r}: not a number')
-  return float(x)
+def _replica_value(k: str, x: Any, r: int) -> Any:
+  """Replica r's value x of per-replica key k in the key's canonical type; a value the key does not accept raises SweepError."""
+  try:
+    return PER_REPLICA_KEYS[k].value(x)
+  except ValueError as e:
+    raise SweepError(f'replica {r}: {k}={x!r}: {e}') from None
 
 
 def replica_values(k: str, per_job: Sequence[Any], R: int) -> List[Any]:
   """The J * R replica values of a group from its J job values: job j's value for each of its R replicas, except a seed, where replica i of
   job j takes s_j + i (a seed sweep with replicas=R runs each job as the replicas=R run of its seed)."""
   if k not in PER_REPLICA_SEED: return [v for v in per_job for _ in range(R)]
-  return [_per_replica_value(k, s) + i for s in per_job for i in range(R)]
-
-
-def _algorithm_value(k: str, x: Any, r: int) -> Any:
-  """A value of PER_REPLICA_ALGORITHM for replica r, as the reference types or asserts it: update_freq an int >= 0 (train.py:37), balanced a
-  bool, quantile_cutoff in [0, 1] (train.py:39), the PWIL scales numbers."""
-  if k == 'imitation.update_freq':
-    if isinstance(x, bool) or not isinstance(x, int) or x < 0: raise SweepError(f'replica {r}: {k}={x!r}: not an integer >= 0')
-    return x
-  if k == 'imitation.balanced':
-    if not isinstance(x, bool): raise SweepError(f'replica {r}: {k}={x!r}: not true / false')
-    return x
-  if isinstance(x, bool) or not isinstance(x, (int, float)): raise SweepError(f'replica {r}: {k}={x!r}: not a number')
-  if k == 'imitation.quantile_cutoff' and not 0 <= x <= 1: raise SweepError(f'replica {r}: {k}={x!r}: not in [0, 1]')
-  return float(x)
-
-
-def _dropout_value(k: str, x: Any, r: int) -> Any:
-  """A value of PER_REPLICA_DROPOUT for replica r: an activation of models.py:17, or a rate in [0, 1) (nn.Dropout refuses p outside [0, 1], and
-  p = 1 scales by 1 / 0; the scalar path refuses it too)."""
-  if k == 'imitation.discriminator.activation':
-    if x not in _ACTIVATIONS: raise SweepError(f'replica {r}: {k}={x!r}: not one of {", ".join(_ACTIVATIONS)}')
-    return x
-  if isinstance(x, bool) or not isinstance(x, (int, float)): raise SweepError(f'replica {r}: {k}={x!r}: not a number')
-  if not 0 <= x < 1: raise SweepError(f'replica {r}: {k}={x!r}: not in [0, 1)')
-  return float(x)
+  return [_replica_value(k, s, j * R) + i for j, s in enumerate(per_job) for i in range(R)]
 
 
 def _check_gail_replicas(cfg: Config, arrays: Dict[str, List[Any]], R: int):
@@ -384,19 +398,18 @@ def _check_gail_replicas(cfg: Config, arrays: Dict[str, List[Any]], R: int):
 
 def split_per_replica(cfg: Config, per_replica: Optional[Dict[str, Sequence[Any]]], R: int) -> Tuple[Config, Dict[str, List[Any]]]:
   """(config, arrays) for Trainer(per_replica=...): a key whose R values are all equal becomes that scalar in a copy of the config (the
-  uniform path, bit for bit); the others stay per-replica lists. Keys outside per_replica_keys(cfg) and values the reference's asserts refuse
-  (train.py:37-49, per replica) are refused."""
+  uniform path, bit for bit); the others stay per-replica lists. Keys outside per_replica_keys(cfg), values outside their PER_REPLICA_KEYS
+  entry's and those the reference's GAIL asserts refuse (train.py:42-47, per replica) are refused."""
   cfg = copy.deepcopy(cfg)
   arrays = {}
   allowed = per_replica_keys(cfg)
   for k, vals in (per_replica or {}).items():
     if k not in allowed: raise SweepError(f'{k} cannot take per-replica values in this configuration (per-replica keys: {", ".join(allowed)})')
-    per_alg = k in PER_REPLICA_ALGORITHM.get(cfg.get('algorithm'), ())
-    vals = [_dropout_value(k, x, r) if k in PER_REPLICA_DROPOUT else _algorithm_value(k, x, r) if per_alg else _per_replica_value(k, x) for r, x in enumerate(vals)]
+    vals = [_replica_value(k, x, r) for r, x in enumerate(vals)]
     if len(vals) != R: raise SweepError(f'{k}: {len(vals)} values for {R} replicas')
     if k in PER_REPLICA_WIDTH: _check_width_classes(k, vals)
-    if k in PER_REPLICA_DROPOUT[:2] and len({x > 0 for x in vals}) > 1:
-      raise SweepError(f'{k}: replicas mix rate 0 and rate > 0 ({vals}); whether a dropout site exists is a grouping key, only its rate is per replica')
+    if PER_REPLICA_KEYS[k].structural and len({x > 0 for x in vals}) > 1:
+      raise SweepError(f'{k}: replicas mix rate 0 and rate > 0 ({vals}); whether it is > 0 is a grouping key, only its value is per replica')
     if all(x == vals[0] for x in vals): set_key(cfg, k, vals[0])
     else: arrays[k] = vals
   if cfg.get('algorithm') == 'GAIL': _check_gail_replicas(cfg, arrays, R)

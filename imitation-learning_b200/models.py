@@ -14,6 +14,7 @@ import torch
 from torch import Tensor
 
 from . import _lib
+from .config import general_discriminator
 from .memory import ReplayMemory, TransitionBatch
 from .net import ReplicaMLP, ReplicaRNG, init_fcnn_params, _null_ctx
 
@@ -442,7 +443,7 @@ class GAILDiscriminator(_Module):
     self.hidden_size_r, self._width_classes, self._replica_order = None, [], None
     # the default configuration (GAIL.yaml:10-17: one relu hidden layer, no shaping, no log-policy term) runs in the fused one-CTA-per-replica
     # kernel (csrc/gail.cu); every other configuration of models.py:157-175 runs as the replica-batched GEMM program of csrc/gail_general.cu
-    self.general = self.reward_shaping or self.subtract_log_policy or model_cfg.depth != 1 or model_cfg.activation != 'relu'
+    self.general = general_discriminator(model_cfg)
     self._ws = None
     if self.general:
       if len(set(h_list)) > 1:

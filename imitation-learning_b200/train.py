@@ -7,8 +7,8 @@ graphs and replayed without host involvement. Replica r is a reference-equivalen
 (`per_replica={'seed': [...]}`, a seed sweep) replica r draws every random number as the single run with seed[r] does, so it is that run.
 
 `Trainer(per_replica={key: R values})` gives the replicas their own values of the shape-preserving hyper-parameters
-(config.VECTORISED, for GAIL the discriminator choices of config.PER_REPLICA_DISCRIMINATOR and its hidden size, config.PER_REPLICA_WIDTH,
-the AdRIL / PWIL / DRIL keys of config.PER_REPLICA_ALGORITHM, and RED's / DRIL's dropout rates and activation, config.PER_REPLICA_DROPOUT); `main` runs a multirun sweep (`-m key=a,b,...`) as groups of such Trainers, one replica block per job.
+(config.PER_REPLICA_KEYS gives each key, the configurations in which it is per replica and the values it accepts); `main` runs a multirun sweep
+(`-m key=a,b,...`) as groups of such Trainers, one replica block per job.
 """
 from __future__ import annotations
 
@@ -34,9 +34,8 @@ from .optim import Adam, AdamW
 ACCELERATED = ['AdRIL', 'BC', 'DRIL', 'SAC', 'GAIL', 'GMMIL', 'PWIL', 'RED']
 
 
-def check_config(cfg: Config, per_replica: Optional[Dict[str, Sequence]] = None):
-  """train.py:28-48; the AdRIL / DRIL asserts hold for every replica's value in `per_replica` (config.split_per_replica's arrays)."""
-  pr = per_replica or {}
+def check_config(cfg: Config):
+  """train.py:28-48 (config.split_per_replica checks the per-replica values)."""
   assert cfg.algorithm in ['AdRIL', 'BC', 'DRIL', 'GAIL', 'GMMIL', 'PWIL', 'RED', 'SAC']
   assert cfg.env in ENVS
   cfg.memory.size = min(cfg.steps, cfg.memory.size)
@@ -46,8 +45,8 @@ def check_config(cfg: Config, per_replica: Optional[Dict[str, Sequence]] = None)
   assert cfg.imitation.mix_expert_data in ['none', 'mixed_batch', 'prefill_memory']
   if cfg.algorithm == 'AdRIL':  # train.py:35-37
     assert cfg.imitation.mix_expert_data == 'mixed_batch'
-    assert all(f >= 0 for f in pr.get('imitation.update_freq', [cfg.imitation.update_freq]))
-  if cfg.algorithm == 'DRIL': assert all(0 <= q <= 1 for q in pr.get('imitation.quantile_cutoff', [cfg.imitation.quantile_cutoff]))  # train.py:38-39
+    assert cfg.imitation.update_freq >= 0
+  if cfg.algorithm == 'DRIL': assert 0 <= cfg.imitation.quantile_cutoff <= 1  # train.py:38-39
   if cfg.algorithm == 'GAIL':
     assert cfg.imitation.mix_expert_data != 'prefill_memory'
     assert cfg.imitation.discriminator.reward_function in ['AIRL', 'FAIRL', 'GAIL']
@@ -72,8 +71,7 @@ class Trainer:
     if per_replica: cfg, self.per_replica = split_per_replica(cfg, per_replica, R)
     seeds = self.seeds = self.per_replica.get('seed')  # None: uniform mode (one program seed, replica r initialised from seed + r)
     if seeds is not None and fast_init: raise SweepError('per-replica seeds need each replica\'s own initial weights; fast_init replicates replica 0\'s')
-    for k in ('imitation.grad_penalty', 'imitation.entropy_bonus'): assert min(self.per_replica.get(k, [0.0])) >= 0, k  # train.py:48-49
-    check_config(cfg, self.per_replica)
+    check_config(cfg)
     self.cfg = cfg
     self.R = R
     self.device = dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
