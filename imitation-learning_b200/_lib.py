@@ -16,6 +16,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'csrc', 'libil_b200.so')
 MAX_LAYERS = 6
 MAX_WIDTH_CLASSES = 8  # IL_MAX_WIDTH_CLASSES: distinct discriminator widths of one il_gail
+IQM_MAX_N = 8192  # IL_IQM_MAX_N: values per il_iqm group
+BOOTSTRAP_MAX_N = 8192  # IL_BOOTSTRAP_MAX_N: envs x runs of il_bootstrap_iqm
 ACT = {'relu': 0, 'tanh': 1, 'sigmoid': 2}
 REWARD = {'AIRL': 0, 'GAIL': 1, 'FAIRL': 2}
 LOSS = {'BCE': 0, 'Mixup': 1, 'PUGAIL': 2}
@@ -184,6 +186,10 @@ SIGNATURES = {
   'il_nccl_comm_create': (C.c_int, [vp, C.c_int, C.c_int, P(vp)]),
   'il_nccl_comm_destroy': (C.c_int, [vp]),
   'il_return_allreduce': (C.c_int, [vp, vp, vp, i64, vp, vp]),
+  'il_iqm': (C.c_int, [vp, vp, i64, C.c_int, vp, vp]),
+  'il_bootstrap_iqm_workspace_bytes': (i64, [C.c_int, C.c_int, C.c_int]),
+  'il_bootstrap_iqm': (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, u64, vp, vp, vp, i64, vp]),
+  'il_percentile_interval': (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_double, C.c_double, vp, vp]),
 }
 
 # Optional trailing arguments added to an entry after it first shipped, with the defaults that keep the earlier behaviour (NULL / 0): calls that

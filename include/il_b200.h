@@ -505,6 +505,28 @@ int il_nccl_comm_create(const uint8_t* id128, int rank, int world, void** comm);
 int il_nccl_comm_destroy(void* comm);
 int il_return_allreduce(il_handle* h, void* nccl_comm, const float* returns, int64_t n, float* out3, void* stream);
 
+/* ---- seed-sweep statistics (scripts/print_plot_seed_sweep_results.py: the IQM and its stratified-bootstrap interval) ------------- */
+/* fp64 throughout; every sum runs in an order fixed by the sizes, so results repeat bit for bit. No allocation, no host synchronisation
+ * (graph capture is not a goal of these entries). Scores must be finite for the results to be the statistics named below (il_b200.results
+ * refuses other input). A NaN still gives a defined result: values are ranked in numpy's sort order (NaN above +inf, ties by index), so
+ * every sort slot is written and a trimmed mean is NaN exactly when a NaN falls inside its window. */
+#define IL_IQM_MAX_N 8192                /* values per il_iqm group (= IL_BOOTSTRAP_MAX_N, so one point estimate covers what the bootstrap takes) */
+#define IL_BOOTSTRAP_MAX_N 8192          /* envs x runs of il_bootstrap_iqm */
+/* out[g] = scipy.stats.trim_mean(x[g, :], 0.25) for G contiguous groups of n doubles: the mean of the order statistics [lc, n - lc),
+ * lc = floor(n / 4). Used for the IQM over evaluation episodes of each run (scripts/print_plot_seed_sweep_results.py:44). */
+int il_iqm(il_handle* h, const double* x, int64_t G, int n, double* out, void* stream);
+/* Stratified bootstrap of the IQM (rliable get_interval_estimates with aggregate_iqm): scores [T, envs, runs]; out [reps, T], out[rep, t]
+ * = the IQM (as il_iqm) of the N = envs x runs values scores[t, e, idx[rep, t, e, k]], k < runs. The indices are `indices`
+ * [reps, T, envs, runs] (int32 in [0, runs); an out-of-range index makes that output NaN) or, when NULL, drawn on the device: draw k of
+ * (rep, t, e) is lane k % 4 of Philox4x32-10 at counter (k / 4, e, t, rep) under key `seed`, mapped to a run by (u * runs) >> 32 (each run
+ * has probability floor or ceil of 2^32 / runs over 2^32: relative bias below runs / 2^32). Workspace: il_bootstrap_iqm_workspace_bytes
+ * (-1 for sizes it refuses). */
+int64_t il_bootstrap_iqm_workspace_bytes(int T, int envs, int runs);
+int il_bootstrap_iqm(il_handle* h, const double* scores, int T, int envs, int runs, int reps, uint64_t seed, const int32_t* indices, double* out,
+                     void* workspace, int64_t workspace_bytes, void* stream);
+/* out2 [2, T]: numpy.percentile(dist[:, t], q_lo) and (.., q_hi) with numpy's default linear interpolation, for dist [reps, T]. */
+int il_percentile_interval(il_handle* h, const double* dist, int reps, int T, double q_lo, double q_hi, double* out2, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
