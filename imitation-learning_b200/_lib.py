@@ -18,6 +18,7 @@ MAX_LAYERS = 6
 MAX_WIDTH_CLASSES = 8  # IL_MAX_WIDTH_CLASSES: distinct discriminator widths of one il_gail
 IQM_MAX_N = 8192  # IL_IQM_MAX_N: values per il_iqm group
 BOOTSTRAP_MAX_N = 8192  # IL_BOOTSTRAP_MAX_N: envs x runs of il_bootstrap_iqm
+GP_MAX_D, GP_MAX_N, GP_MAX_M, GP_MAX_Q = 64, 4096, 1 << 22, 1024  # IL_GP_MAX_*: il_gp_posterior / il_gp_select caps
 ACT = {'relu': 0, 'tanh': 1, 'sigmoid': 2}
 REWARD = {'AIRL': 0, 'GAIL': 1, 'FAIRL': 2}
 LOSS = {'BCE': 0, 'Mixup': 1, 'PUGAIL': 2}
@@ -190,6 +191,9 @@ SIGNATURES = {
   'il_bootstrap_iqm_workspace_bytes': (i64, [C.c_int, C.c_int, C.c_int]),
   'il_bootstrap_iqm': (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, u64, vp, vp, vp, i64, vp]),
   'il_percentile_interval': (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_double, C.c_double, vp, vp]),
+  'il_gp_posterior': (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_int, vp, i64, P(C.c_double), C.c_double, C.c_double, vp, vp, vp, vp]),
+  'il_gp_select_workspace_bytes': (i64, [C.c_int, C.c_int, i64, C.c_int]),
+  'il_gp_select': (C.c_int, [vp, C.c_int, C.c_int, vp, i64, P(C.c_double), C.c_double, C.c_double, vp, vp, vp, vp, C.c_int, C.c_double, C.c_int, vp, vp, vp, i64, vp]),
 }
 
 # Optional trailing arguments added to an entry after it first shipped, with the defaults that keep the earlier behaviour (NULL / 0): calls that

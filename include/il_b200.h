@@ -527,6 +527,31 @@ int il_bootstrap_iqm(il_handle* h, const double* scores, int T, int envs, int ru
 /* out2 [2, T]: numpy.percentile(dist[:, t], q_lo) and (.., q_hi) with numpy's default linear interpolation, for dist [reps, T]. */
 int il_percentile_interval(il_handle* h, const double* dist, int reps, int T, double q_lo, double q_hi, double* out2, void* stream);
 
+/* ---- hyper-parameter search (train_all.py -m): Gaussian-process posterior and greedy batch selection ------------------------------ */
+/* fp64 throughout. The GP is zero-mean with kernel k(x, x') = s2 (1 + sqrt5 r + 5 r^2 / 3) exp(-sqrt5 r), r^2 = sum_k ((x_k - x'_k) / l_k)^2,
+ * and Gaussian noise `noise` (sigma_n^2). `lengthscales` [d] is a HOST pointer; all other arrays are device arrays. Sizes outside the caps,
+ * non-positive or non-finite hyper-parameters and null pointers are refused; the data arrays must be finite (il_b200/hpo.py checks). */
+#define IL_GP_MAX_D 64                   /* encoded dimensions */
+#define IL_GP_MAX_N 4096                 /* observed trials in one fit */
+#define IL_GP_MAX_M (1 << 22)            /* candidates */
+#define IL_GP_MAX_Q 1024                 /* picks of one il_gp_select */
+/* For M candidates Ct [d, M] (column m is candidate m) and observed X [n, d], the Cholesky factor L [n, n] (row-major, lower) of
+ * K(X, X) + noise I and alpha = (K + noise I)^-1 y: mu[m] = k(x_m, X) . alpha, V[i, m] = (L^-1 k(X, x_m))[i] for i < n (rows of M doubles),
+ * var[m] = s2 - |V[:, m]|^2, the latent variance. k(x_m, X) is formed on the fly; V is solved by blocked forward substitution. */
+int il_gp_posterior(il_handle* h, const double* X, const double* alpha, const double* L, int n, int d, const double* Ct, int64_t M,
+                    const double* lengthscales, double outputscale, double noise, double* mu, double* var, double* V, void* stream);
+/* q greedy expected-improvement picks with the kriging believer, from il_gp_posterior's mu, var and V (V must have n + q rows). Pick j is
+ * the first index of the largest EI = (mu - f*) Phi(z) + sigma phi(z), z = (mu - f*) / sigma, over candidates not yet picked whose group
+ * (group [M]) is admitted: with max_groups G > 0, once G distinct groups are picked only those groups stay admissible (0: unlimited).
+ * f* starts at f_star (the largest posterior mean over the observed points) and becomes max(f*, mu(x_w)) after each pick w. Then, for every
+ * candidate, c = k(x, x_w) - V[:, x] . V[:, x_w] over rows [0, n + j), var -= c^2 / (var(x_w) + noise), V[n + j, x] = c / sqrt(var(x_w) + noise):
+ * the posterior of the GP refitted with x_w observed at its mean, hyper-parameters held. picks [q] int32 (-1 once no candidate is
+ * admissible), ei [q] (NaN there). var and rows [n, n + q) of V are overwritten. Workspace: il_gp_select_workspace_bytes (-1 if refused). */
+int64_t il_gp_select_workspace_bytes(int n, int d, int64_t M, int q);
+int il_gp_select(il_handle* h, int n, int d, const double* Ct, int64_t M, const double* lengthscales, double outputscale, double noise, const double* mu,
+                 double* var, double* V, const int32_t* group, int max_groups, double f_star, int q, int32_t* picks, double* ei, void* workspace,
+                 int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
