@@ -126,6 +126,31 @@ __device__ __forceinline__ float softplusf(float x) {  // torch softplus (beta 1
 }
 __device__ __forceinline__ float sigmoidf(float x) { return 1.f / (1.f + expf(-x)); }
 
+// ---- AdamW (torch _single_tensor_adam: Python-double scalars, then cast to the tensor dtype) ----------------------
+struct AdamW {
+  float step_size, bc2_sqrt;  // lr / (1 - beta1^t), sqrt(1 - beta2^t)
+  float decay, w1, w2, beta2, eps;  // 1 - lr * wd (one rounding: the fused multiply-add the expression always compiled to), 1 - beta1, 1 - beta2
+  bool has_wd;
+};
+// the two step-dependent scalars, computed by one thread and staged by the caller (shared memory or registers)
+__device__ __forceinline__ void adamw_bias_correction(double lr, double beta1, double beta2, int64_t step, float& step_size, float& bc2_sqrt) {
+  const double t = (double)step;
+  step_size = (float)(lr / (1.0 - pow(beta1, t)));
+  bc2_sqrt = (float)sqrt(1.0 - pow(beta2, t));
+}
+__device__ __forceinline__ AdamW adamw_coefs(float step_size, float bc2_sqrt, double lr, double wd, double beta1, double beta2, double eps) {
+  return AdamW{step_size, bc2_sqrt, (float)fma(-lr, wd, 1.0), (float)(1.0 - beta1), (float)(1.0 - beta2), (float)beta2, (float)eps, wd != 0.0};
+}
+// one element; step_size / decay / has_wd are passed separately so per-replica tables can override them
+__device__ __forceinline__ void adamw_update(const AdamW& c, float& p, float& m, float& v, float g, float step_size, float decay, bool has_wd) {
+  if (has_wd) p = __fmul_rn(p, decay);                                          // param.mul_(1 - lr * weight_decay)
+  m = __fadd_rn(m, __fmul_rn(c.w1, __fsub_rn(g, m)));                           // exp_avg.lerp_(grad, 1 - beta1)
+  v = __fadd_rn(__fmul_rn(v, c.beta2), __fmul_rn(__fmul_rn(c.w2, g), g));       // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value=1 - beta2)
+  const float denom = __fadd_rn(__fdiv_rn(sqrtf(v), c.bc2_sqrt), c.eps);        // (exp_avg_sq.sqrt() / bias_correction2_sqrt).add_(eps)
+  p = __fadd_rn(p, __fmul_rn(-step_size, __fdiv_rn(m, denom)));                 // param.addcdiv_(exp_avg, denom, value=-step_size)
+}
+__device__ __forceinline__ void adamw_update(const AdamW& c, float& p, float& m, float& v, float g) { adamw_update(c, p, m, v, g, c.step_size, c.decay, c.has_wd); }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -4,12 +4,11 @@
 //                    entropy bonus, spectral-norm power iterations per train-mode forward (a12) and their
 //                    backward projection, AdamW — everything in shared memory, parameters touched once.
 //   il_gail_reward : eval-mode forward + reward (models.py:177-180).
-#include "common.cuh"
+#include "gail_loss.cuh"
 
 namespace {
 
 constexpr int THREADS = 256;
-enum PassKind { PASS_POLICY = 0, PASS_EXPERT = 1, PASS_MIX = 2 };
 
 struct GailDims {
   int S, A, d, H, B, row, ldx, ldz, RB, HD;
@@ -104,6 +103,191 @@ __device__ float spectral_sigma(const float* W, float* u, float* v, float* tvec,
   return s;
 }
 
+// Loads replica r's parameters (zeroing the gradient accumulators G1, G2, gb1), b2 and, with spectral norm, its (u, v); returns u2. The
+// per-replica choices (sweeps) are staged in s.scal and re-read where used: the register budget of the tiled variants has no room for them
+// (scal[0:2] is the AdamW scratch at the end).
+template <class Smem, class Params>
+__device__ __forceinline__ float gail_load(const Smem& s, const Params& p, const float* prm, int r, int H, int d, bool sn_r, float& b2) {
+  const il_gail_update_args& a = p.a;
+  const int tid = threadIdx.x;
+  for (int i = tid; i < H * d; i += THREADS) { s.W1[i] = prm[p.off_w1 + i]; s.G1[i] = 0.f; }
+  for (int h = tid; h < H; h += THREADS) {
+    s.b1[h] = prm[p.off_b1 + h]; s.w2[h] = prm[p.off_w2 + h]; s.G2[h] = 0.f; s.gb1[h] = 0.f;
+    if (sn_r) { s.u1[h] = a.disc.u[(int64_t)r * a.disc.u_stride + h]; s.v2[h] = a.disc.v[(int64_t)r * a.disc.v_stride + d + h]; }
+  }
+  if (sn_r) for (int j = tid; j < d; j += THREADS) s.v1[j] = a.disc.v[(int64_t)r * a.disc.v_stride + j];
+  b2 = prm[p.off_b2];
+  const float u2 = sn_r ? a.disc.u[(int64_t)r * a.disc.u_stride + H] : 1.f;
+  if (tid == 0) {
+    s.scal[2] = __int_as_float(a.loss_function_r ? a.loss_function_r[r] : a.loss_function);
+    s.scal[3] = a.pos_class_prior_r ? a.pos_class_prior_r[r] : a.pos_class_prior;
+    s.scal[4] = a.nonnegative_margin_r ? a.nonnegative_margin_r[r] : a.nonnegative_margin;
+    s.scal[5] = sn_r ? 1.f : 0.f;
+    s.scal[6] = __int_as_float(r);
+  }
+  __syncthreads();
+  return u2;
+}
+
+// The passes of an update (training.py:94-127): [policy, expert] or [Mixup], then the gradient-penalty mix (gp_pass, -1 without). Returns their number.
+__device__ __forceinline__ int gail_schedule(int loss_function, float grad_penalty, const float* eps_mix, const float* eps_gp, int kinds[3], const float* pass_eps[3], int& gp_pass) {
+  int n_pass = 0;
+  gp_pass = -1;
+  if (loss_function == IL_LOSS_MIXUP) { kinds[n_pass] = PASS_MIX; pass_eps[n_pass++] = eps_mix; }
+  else { kinds[n_pass++] = PASS_POLICY; kinds[n_pass++] = PASS_EXPERT; }
+  if (grad_penalty > 0.f) { gp_pass = n_pass; kinds[n_pass] = PASS_MIX; pass_eps[n_pass++] = eps_gp; }
+  return n_pass;
+}
+
+// Phase 1: one power iteration per layer per train-mode forward (one per pass); slot k of s.slots keeps pass k's (u1, v1, v2, sigma1, sigma2, u2).
+template <class Smem>
+__device__ __forceinline__ void gail_power_iterations(const Smem& s, int n_pass, int H, int d, bool training, float& u2) {
+  const int SF = gail_slot_floats(H, d), tid = threadIdx.x;
+  auto sn = [&] { return s.scal[5] != 0.f; };
+  for (int k = 0; k < n_pass; ++k) {
+    float* slot = s.slots + k * SF;
+    float sig1 = 1.f, sig2 = 1.f;
+    if (sn()) {
+      sig1 = spectral_sigma(s.W1, s.u1, s.v1, s.tvec, s.red, H, d, training);
+      // layer 2 is a [1, H] matrix: u2 scalar, v2 [H]
+      float t = 0.f;
+      if (training) {
+        for (int h = tid; h < H; h += THREADS) t = fmaf(s.w2[h], s.v2[h], t);
+        t = bsum(t, s.red);
+        u2 = t / fmaxf(fabsf(t), 1e-12f);
+        for (int h = tid; h < H; h += THREADS) s.tvec[h] = s.w2[h] * u2;
+        __syncthreads();
+        const float dn = fmaxf(sqrtf(sq_norm(s.tvec, H, s.red)), 1e-12f);
+        for (int h = tid; h < H; h += THREADS) s.v2[h] = s.tvec[h] / dn;
+        __syncthreads();
+      }
+      t = 0.f;
+      for (int h = tid; h < H; h += THREADS) t = fmaf(s.w2[h], s.v2[h], t);
+      sig2 = u2 * bsum(t, s.red);
+    }
+    for (int h = tid; h < H; h += THREADS) { slot[h] = s.u1[h]; slot[H + d + h] = s.v2[h]; }
+    for (int j = tid; j < d; j += THREADS) slot[H + j] = s.v1[j];
+    if (tid == 0) { slot[2 * H + d] = sig1; slot[2 * H + d + 1] = sig2; slot[2 * H + d + 2] = u2; }
+    __syncthreads();
+  }
+}
+
+// The loss outputs, the AdamW step of every parameter (train.py:84) and the write-back of the power-iteration state (the in-place buffers of the
+// parametrization). The replica index (order[blockIdx.x] in a width-class launch) and the pointers derived from it are re-derived from shared
+// memory: kept live from the start in registers they cost the tiled variants spills.
+template <class Smem, class Params>
+__device__ __forceinline__ void gail_finish(const Smem& s, const Params& p, int H, int d, float pu_gate, float loss_bce, float loss_gp, float gb2, float u2) {
+  const il_gail_update_args& a = p.a;
+  const int tid = threadIdx.x;
+  const int rr = __float_as_int(s.scal[6]);
+  // PUGAIL with the clamp active: policy_loss = -margin (training.py:102); its gated terms were left out of loss_bce above
+  if (pu_gate == 0.f) loss_bce -= s.scal[4];
+  if (tid == 0 && a.out_losses) { a.out_losses[rr * 2 + 0] = loss_bce; a.out_losses[rr * 2 + 1] = loss_gp; }
+
+  // ---- AdamW (train.py:84; torch _single_tensor_adam) -----------------------------------------------------------
+  const double lr = a.opt.lr_r ? a.opt.lr_r[rr] : a.opt.lr, wd = a.opt.weight_decay_r ? a.opt.weight_decay_r[rr] : a.opt.weight_decay;
+  if (tid == 0) adamw_bias_correction(lr, a.opt.beta1, a.opt.beta2, *a.opt.step, s.scal[0], s.scal[1]);
+  __syncthreads();
+  const AdamW c = adamw_coefs(s.scal[0], s.scal[1], lr, wd, a.opt.beta1, a.opt.beta2, a.opt.eps);
+  float* prm = a.disc.g.params + (int64_t)rr * a.disc.g.stride;
+  float* am = a.opt.m + (int64_t)rr * a.disc.g.stride;
+  float* avv = a.opt.v + (int64_t)rr * a.disc.g.stride;
+  auto adam = [&](int64_t off, float grad) {
+    float pi = prm[off], mi = am[off], vi = avv[off];
+    adamw_update(c, pi, mi, vi, grad);
+    prm[off] = pi; am[off] = mi; avv[off] = vi;
+  };
+  for (int i = tid; i < H * d; i += THREADS) adam(p.off_w1 + i, s.G1[i]);
+  for (int h = tid; h < H; h += THREADS) { adam(p.off_b1 + h, s.gb1[h]); adam(p.off_w2 + h, s.G2[h]); }
+  if (tid == 0) adam(p.off_b2, gb2);
+  if (s.scal[5] != 0.f) {
+    for (int h = tid; h < H; h += THREADS) { a.disc.u[(int64_t)rr * a.disc.u_stride + h] = s.u1[h]; a.disc.v[(int64_t)rr * a.disc.v_stride + d + h] = s.v2[h]; }
+    for (int j = tid; j < d; j += THREADS) a.disc.v[(int64_t)rr * a.disc.v_stride + j] = s.v1[j];
+    if (tid == 0) a.disc.u[(int64_t)rr * a.disc.u_stride + H] = u2;
+  }
+}
+
+// Phase 2 (PUGAIL only): the clamp of training.py:102 needs the batch scalar before any gradient. For pass k = 0 (policy), 1 (expert):
+// set_effective(k) writes that pass's W / sigma, forward(k, b0, nb) runs rows [b0, b0 + nb) (sample weights into s.CO) and returns their logits.
+template <class Smem, class SetEffective, class Forward>
+__device__ __forceinline__ float gail_pu_phase(const Smem& s, int B, int RB, float invB, SetEffective set_effective, Forward forward) {
+  const int tid = threadIdx.x;
+  float sums[2] = {0.f, 0.f};  // sum w_p softplus(f_p), sum w_e softplus(f_e)
+  for (int k = 0; k < 2; ++k) {
+    set_effective(k);
+    __syncthreads();
+    float part = 0.f;
+    for (int b0 = 0; b0 < B; b0 += RB) {
+      const int nb = min(RB, B - b0);
+      const float* f = forward(k, b0, nb);
+      for (int b = tid; b < nb; b += THREADS) part += s.CO[b] * softplusf(f[b]);
+      __syncthreads();
+    }
+    sums[k] = bsum(part, s.red);
+  }
+  return gail_pu_gate(sums[0], sums[1], s.scal[3], s.scal[4], invB);
+}
+
+// End of one pass: its spectral-norm backward dL/dW = (G - <G, W_eff> u v^T) / sigma (SURVEY §8a a12) accumulated into G1 / G2 (gb1 unprojected),
+// then gb2 and the pass's loss. slot holds the pass's (u1, v1, v2) and sigma1 / sigma2 / u2k its scalars; for_g1(f) calls f(e, g, w_eff) for
+// this thread's elements e < H * d of dL/dW1e and W1e.
+template <class Smem, class ForG1>
+__device__ __forceinline__ void gail_project_pass(const Smem& s, const float* slot, int H, int d, float sig1, float sig2, float u2k, bool is_gp, float gb2k,
+                                                  float loss_part, float invB, float& gb2, float& loss_bce, float& loss_gp, ForG1 for_g1) {
+  const int tid = threadIdx.x;
+  auto sn = [&] { return s.scal[5] != 0.f; };
+  float inner1 = 0.f, inner2 = 0.f;
+  if (sn()) {
+    for_g1([&](int, float g, float w) { inner1 = fmaf(g, w, inner1); });
+    inner1 = bsum(inner1, s.red);
+    for (int h = tid; h < H; h += THREADS) inner2 = fmaf(s.G2k[h], s.w2e[h], inner2);
+    inner2 = bsum(inner2, s.red);
+  }
+  for_g1([&](int e, float g, float) {
+    const int h = e / d, j = e % d;
+    s.G1[e] += sn() ? (g - inner1 * slot[h] * slot[H + j]) / sig1 : g;
+  });
+  for (int h = tid; h < H; h += THREADS) {
+    s.G2[h] += sn() ? (s.G2k[h] - inner2 * u2k * slot[H + d + h]) / sig2 : s.G2k[h];
+    s.gb1[h] += s.gb1k[h];
+  }
+  gb2k = bsum(gb2k, s.red);
+  gb2 += gb2k;
+  loss_part = bsum(loss_part, s.red);
+  if (is_gp) loss_gp = loss_part * invB; else loss_bce += loss_part * invB;
+  __syncthreads();
+}
+
+// The reward kernels' setup: replica r's W1, b1, w2 (and with spectral norm u1, v1, v2) into shared memory; returns b2 and the eval-mode
+// sigma of both layers, from the stored (u, v) without a power iteration (train.py:180,194; 1 without spectral norm).
+__device__ __forceinline__ float gail_reward_load(const GailRewParams& p, int r, int H, int d, float* W1, float* b1, float* w2, float* u1, float* v1, float* v2,
+                                                  float* tvec, float* red, float& sig1, float& sig2) {
+  const int tid = threadIdx.x;
+  const float* prm = p.disc.g.params + (int64_t)r * p.disc.g.stride;
+  const bool sn = p.disc.u != nullptr && (!p.disc.spectral_norm_r || p.disc.spectral_norm_r[r] != 0);
+  for (int i = tid; i < H * d; i += THREADS) W1[i] = prm[p.off_w1 + i];
+  for (int h = tid; h < H; h += THREADS) {
+    b1[h] = prm[p.off_b1 + h]; w2[h] = prm[p.off_w2 + h];
+    if (sn) { u1[h] = p.disc.u[(int64_t)r * p.disc.u_stride + h]; v2[h] = p.disc.v[(int64_t)r * p.disc.v_stride + d + h]; }
+  }
+  if (sn) for (int j = tid; j < d; j += THREADS) v1[j] = p.disc.v[(int64_t)r * p.disc.v_stride + j];
+  const float b2 = prm[p.off_b2];
+  __syncthreads();
+  sig1 = 1.f; sig2 = 1.f;
+  if (sn) {
+    sig1 = spectral_sigma(W1, u1, v1, tvec, red, H, d, false);
+    float t = 0.f;
+    for (int h = tid; h < H; h += THREADS) t = fmaf(w2[h], v2[h], t);
+    sig2 = p.disc.u[(int64_t)r * p.disc.u_stride + H] * bsum(t, red);
+  }
+  return b2;
+}
+// logit f of row b of replica r (batch B), and its reward (models.py:177-180), where the caller asked for them
+__device__ __forceinline__ void gail_reward_store(const GailRewParams& p, int r, int B, int b, float f, int reward_function) {
+  if (p.logits) p.logits[(int64_t)r * B + b] = f;
+  if (p.reward) p.reward[(int64_t)r * p.reward_rs + (int64_t)b * p.reward_ld] = gail_reward_of_logit(f, reward_function);
+}
+
 // Loads rows [b0, b0 + nb) of a pass into X (features) and CO (sample weight w); DF receives the mixing epsilon.
 __device__ void load_rows(const GailDims& g, const float* pol, const float* exp_, const float* eps, int kind, int b0, int nb, float* X, float* CO, float* DF) {
   const RowLayout L = row_layout(g.S, g.A);
@@ -164,7 +348,7 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_kernel(const GailUpdPa
   const il_gail_update_args& a = p.a;
   const int r = p.order ? p.order[blockIdx.x] : blockIdx.x, tid = threadIdx.x;
   const int H = g.H, d = g.d, B = g.B;
-  float* prm = a.disc.g.params + (int64_t)r * a.disc.g.stride;
+  const float* prm = a.disc.g.params + (int64_t)r * a.disc.g.stride;
   const bool sn_r = a.disc.u != nullptr && (!a.disc.spectral_norm_r || a.disc.spectral_norm_r[r] != 0);  // a replica at 0 never touches its u / v slots
   const float* pol = a.policy.rows + (int64_t)r * a.policy.replica_stride;
   const float* exp_ = a.expert.rows + (int64_t)r * a.expert.replica_stride;
@@ -174,91 +358,32 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_kernel(const GailUpdPa
   // branches of a uniform run with 0
   const float grad_penalty = a.grad_penalty_r ? a.grad_penalty_r[r] : a.grad_penalty, entropy_bonus = a.entropy_bonus_r ? a.entropy_bonus_r[r] : a.entropy_bonus;
   const float invB = 1.f / (float)B;
-
-  // ---- load parameters / buffers -------------------------------------------------------------------------
-  for (int i = tid; i < H * d; i += THREADS) { s.W1[i] = prm[p.off_w1 + i]; s.G1[i] = 0.f; }
-  for (int h = tid; h < H; h += THREADS) {
-    s.b1[h] = prm[p.off_b1 + h]; s.w2[h] = prm[p.off_w2 + h]; s.G2[h] = 0.f; s.gb1[h] = 0.f;
-    if (sn_r) { s.u1[h] = a.disc.u[(int64_t)r * a.disc.u_stride + h]; s.v2[h] = a.disc.v[(int64_t)r * a.disc.v_stride + d + h]; }
-  }
-  if (sn_r) for (int j = tid; j < d; j += THREADS) s.v1[j] = a.disc.v[(int64_t)r * a.disc.v_stride + j];
-  const float b2 = prm[p.off_b2];
-  float u2 = sn_r ? a.disc.u[(int64_t)r * a.disc.u_stride + H] : 1.f;
-  // the per-replica choices (sweeps) live in shared memory and are re-read where used: the register budget of the tiled variants has no room
-  // for them (scal[0:2] is the AdamW scratch at the end)
-  if (tid == 0) {
-    s.scal[2] = __int_as_float(a.loss_function_r ? a.loss_function_r[r] : a.loss_function);
-    s.scal[3] = a.pos_class_prior_r ? a.pos_class_prior_r[r] : a.pos_class_prior;
-    s.scal[4] = a.nonnegative_margin_r ? a.nonnegative_margin_r[r] : a.nonnegative_margin;
-    s.scal[5] = sn_r ? 1.f : 0.f;
-    s.scal[6] = __int_as_float(r);
-  }
-  __syncthreads();
+  float b2, u2 = gail_load(s, p, prm, r, H, d, sn_r, b2);
   auto loss_function = [&] { return __float_as_int(s.scal[2]); };
-  auto sn = [&] { return s.scal[5] != 0.f; };
 
-  // ---- pass schedule (training.py:94-127): [policy, expert] or [mixup], then the gradient-penalty mix -----
-  int kinds[3], n_pass = 0;
+  int kinds[3], gp_pass;
   const float* pass_eps[3] = {nullptr, nullptr, nullptr};
-  int gp_pass = -1;
-  if (loss_function() == IL_LOSS_MIXUP) { kinds[n_pass] = PASS_MIX; pass_eps[n_pass++] = eps_mix; }
-  else { kinds[n_pass++] = PASS_POLICY; kinds[n_pass++] = PASS_EXPERT; }
-  if (grad_penalty > 0.f) { gp_pass = n_pass; kinds[n_pass] = PASS_MIX; pass_eps[n_pass++] = eps_gp; }
+  const int n_pass = gail_schedule(loss_function(), grad_penalty, eps_mix, eps_gp, kinds, pass_eps, gp_pass);
 
-  // ---- phase 1: one power iteration per layer per train-mode forward; remember (u, v, sigma) of each ------
   const int SF = gail_slot_floats(H, d);
-  for (int k = 0; k < n_pass; ++k) {
-    float* slot = s.slots + k * SF;
-    float sig1 = 1.f, sig2 = 1.f;
-    if (sn()) {
-      sig1 = spectral_sigma(s.W1, s.u1, s.v1, s.tvec, s.red, H, d, a.training != 0);
-      // layer 2 is a [1, H] matrix: u2 scalar, v2 [H]
-      float t = 0.f;
-      if (a.training) {
-        for (int h = tid; h < H; h += THREADS) t = fmaf(s.w2[h], s.v2[h], t);
-        t = bsum(t, s.red);
-        u2 = t / fmaxf(fabsf(t), 1e-12f);
-        for (int h = tid; h < H; h += THREADS) s.tvec[h] = s.w2[h] * u2;
-        __syncthreads();
-        const float dn = fmaxf(sqrtf(sq_norm(s.tvec, H, s.red)), 1e-12f);
-        for (int h = tid; h < H; h += THREADS) s.v2[h] = s.tvec[h] / dn;
-        __syncthreads();
-      }
-      t = 0.f;
-      for (int h = tid; h < H; h += THREADS) t = fmaf(s.w2[h], s.v2[h], t);
-      sig2 = u2 * bsum(t, s.red);
-    }
-    for (int h = tid; h < H; h += THREADS) { slot[h] = s.u1[h]; slot[H + d + h] = s.v2[h]; }
-    for (int j = tid; j < d; j += THREADS) slot[H + j] = s.v1[j];
-    if (tid == 0) { slot[2 * H + d] = sig1; slot[2 * H + d + 1] = sig2; slot[2 * H + d + 2] = u2; }
-    __syncthreads();
-  }
+  gail_power_iterations(s, n_pass, H, d, a.training != 0, u2);
 
-  // ---- phase 2 (PUGAIL only): the clamp of training.py:102 needs the batch scalar before any gradient ------
   float pu_gate = 1.f;
   float loss_bce = 0.f, loss_gp = 0.f;
-  if (loss_function() == IL_LOSS_PUGAIL) {
-    float sums[2] = {0.f, 0.f};  // sum w_p softplus(f_p), sum w_e softplus(f_e)
-    for (int k = 0; k < 2; ++k) {
-      const float* slot = s.slots + k * SF;
-      const float sig1 = slot[2 * H + d], sig2 = slot[2 * H + d + 1];
-      for (int i = tid; i < H * d; i += THREADS) s.W1e[i] = s.W1[i] / sig1;
-      for (int h = tid; h < H; h += THREADS) s.w2e[h] = s.w2[h] / sig2;
-      __syncthreads();
-      float part = 0.f;
-      for (int b0 = 0; b0 < B; b0 += g.RB) {
-        const int nb = min(g.RB, B - b0);
-        load_rows(g, pol, exp_, nullptr, kinds[k], b0, nb, s.X, s.CO, s.DF);
-        __syncthreads();
-        forward_chunk(g, s, nb, b2, s.DF);
-        for (int b = tid; b < nb; b += THREADS) part += s.CO[b] * softplusf(s.DF[b]);
-        __syncthreads();
-      }
-      sums[k] = bsum(part, s.red);
-    }
-    const float inner = s.scal[3] * (sums[1] * invB) - sums[0] * invB;
-    pu_gate = inner >= -s.scal[4] ? 1.f : 0.f;  // torch.clamp(min=) passes gradient where x >= min
-  }
+  if (loss_function() == IL_LOSS_PUGAIL)
+    pu_gate = gail_pu_phase(s, B, g.RB, invB,
+                            [&](int k) {
+                              const float* slot = s.slots + k * SF;
+                              const float sig1 = slot[2 * H + d], sig2 = slot[2 * H + d + 1];
+                              for (int i = tid; i < H * d; i += THREADS) s.W1e[i] = s.W1[i] / sig1;
+                              for (int h = tid; h < H; h += THREADS) s.w2e[h] = s.w2[h] / sig2;
+                            },
+                            [&](int k, int b0, int nb) {
+                              load_rows(g, pol, exp_, nullptr, kinds[k], b0, nb, s.X, s.CO, s.DF);
+                              __syncthreads();
+                              forward_chunk(g, s, nb, b2, s.DF);
+                              return s.DF;
+                            });
 
   // ---- phase 3: forward + backward per pass, projected through that pass's spectral norm --------------------
   float g1k[NE];
@@ -282,21 +407,8 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_kernel(const GailUpdPa
         // DF holds eps (mixup) on entry; forward writes logits into GX[0..nb) scratch first
         forward_chunk(g, s, nb, b2, s.GX);
         for (int b = tid; b < nb; b += THREADS) {
-          const float f = s.GX[b], w = s.CO[b], sg = sigmoidf(f);
-          float df;
-          if (loss_function() == IL_LOSS_MIXUP) {  // training.py:112
-            const float e = s.DF[b];
-            df = w * (sg - e) * invB;
-            loss_part += e * w * softplusf(-f) + (1.f - e) * w * softplusf(f);
-          } else if (loss_function() == IL_LOSS_BCE) {  // training.py:98-99
-            df = kind == PASS_EXPERT ? w * (sg - 1.f) * invB : w * sg * invB;
-            loss_part += kind == PASS_EXPERT ? w * softplusf(-f) : w * softplusf(f);
-          } else {  // PUGAIL, training.py:101-102
-            const float pr = s.scal[3];
-            df = kind == PASS_EXPERT ? pr * w * (sg - 1.f) * invB + pu_gate * pr * w * sg * invB : -pu_gate * w * sg * invB;
-            loss_part += kind == PASS_EXPERT ? pr * w * softplusf(-f) + pu_gate * pr * w * softplusf(f) : -pu_gate * w * softplusf(f);
-          }
-          if (entropy_bonus > 0.f) df += entropy_bonus * w * f * sg * (1.f - sg) * invB;  // training.py:130-132
+          const bool mix = loss_function() == IL_LOSS_MIXUP;
+          const float df = gail_loss_row(s.GX[b], s.CO[b], mix, mix ? s.DF[b] : 0.f, loss_function(), kind == PASS_EXPERT, s.scal[3], pu_gate, entropy_bonus, invB, loss_part);
           s.DF[b] = df;
           gb2k += df;
         }
@@ -396,75 +508,15 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_kernel(const GailUpdPa
         __syncthreads();
       }
     }
-    // ---- spectral-norm backward: dL/dW = (G - <G, W_eff> u v^T) / sigma (SURVEY §8a a12), accumulate over passes
-    float inner1 = 0.f, inner2 = 0.f;
-    if (sn()) {
+    gail_project_pass(s, slot, H, d, sig1, sig2, u2k, is_gp, gb2k, loss_part, invB, gb2, loss_bce, loss_gp, [&](auto f) {  // dL/dW1e in registers
 #pragma unroll
       for (int i = 0; i < NE; ++i) {
         const int e = tid + i * THREADS;
-        if (e < H * d) inner1 = fmaf(g1k[i], s.W1e[e], inner1);
+        if (e < H * d) f(e, g1k[i], s.W1e[e]);
       }
-      inner1 = bsum(inner1, s.red);
-      for (int h = tid; h < H; h += THREADS) inner2 = fmaf(s.G2k[h], s.w2e[h], inner2);
-      inner2 = bsum(inner2, s.red);
-    }
-#pragma unroll
-    for (int i = 0; i < NE; ++i) {
-      const int e = tid + i * THREADS;
-      if (e < H * d) {
-        const int h = e / d, j = e % d;
-        s.G1[e] += sn() ? (g1k[i] - inner1 * slot[h] * slot[H + j]) / sig1 : g1k[i];
-      }
-    }
-    for (int h = tid; h < H; h += THREADS) {
-      s.G2[h] += sn() ? (s.G2k[h] - inner2 * u2k * slot[H + d + h]) / sig2 : s.G2k[h];
-      s.gb1[h] += s.gb1k[h];
-    }
-    gb2k = bsum(gb2k, s.red);
-    gb2 += gb2k;
-    loss_part = bsum(loss_part, s.red);
-    if (is_gp) loss_gp = loss_part * invB; else loss_bce += loss_part * invB;
-    __syncthreads();
+    });
   }
-  // the replica index (order[blockIdx.x] in a width-class launch) and the pointers derived from it are re-derived from shared memory here:
-  // kept live from the start in registers they cost the tiled variants spills
-  const int rr = __float_as_int(s.scal[6]);
-  // PUGAIL with the clamp active: policy_loss = -margin (training.py:102); its gated terms were left out of loss_bce above
-  if (pu_gate == 0.f) loss_bce -= s.scal[4];
-  if (tid == 0 && a.out_losses) { a.out_losses[rr * 2 + 0] = loss_bce; a.out_losses[rr * 2 + 1] = loss_gp; }
-
-  // ---- AdamW (train.py:84; torch _single_tensor_adam) -----------------------------------------------------------
-  const double lr = a.opt.lr_r ? a.opt.lr_r[rr] : a.opt.lr, wd = a.opt.weight_decay_r ? a.opt.weight_decay_r[rr] : a.opt.weight_decay;
-  if (tid == 0) {
-    const double t = (double)*a.opt.step;
-    s.scal[0] = (float)(lr / (1.0 - pow(a.opt.beta1, t)));
-    s.scal[1] = (float)sqrt(1.0 - pow(a.opt.beta2, t));
-  }
-  __syncthreads();
-  const float step_size = s.scal[0], bc2_sqrt = s.scal[1];
-  const float decay = (float)(1.0 - lr * wd), w1 = (float)(1.0 - a.opt.beta1), w2c = (float)(1.0 - a.opt.beta2), beta2 = (float)a.opt.beta2,
-              eps = (float)a.opt.eps;
-  const bool has_wd = wd != 0.0;
-  prm = a.disc.g.params + (int64_t)rr * a.disc.g.stride;
-  float* am = a.opt.m + (int64_t)rr * a.disc.g.stride;
-  float* avv = a.opt.v + (int64_t)rr * a.disc.g.stride;
-  auto adam = [&](int64_t off, float grad) {
-    float pi = prm[off], mi = am[off], vi = avv[off];
-    if (has_wd) pi = __fmul_rn(pi, decay);
-    mi = __fadd_rn(mi, __fmul_rn(w1, __fsub_rn(grad, mi)));
-    vi = __fadd_rn(__fmul_rn(vi, beta2), __fmul_rn(__fmul_rn(w2c, grad), grad));
-    const float denom = __fadd_rn(__fdiv_rn(sqrtf(vi), bc2_sqrt), eps);
-    pi = __fadd_rn(pi, __fmul_rn(-step_size, __fdiv_rn(mi, denom)));
-    prm[off] = pi; am[off] = mi; avv[off] = vi;
-  };
-  for (int i = tid; i < H * d; i += THREADS) adam(p.off_w1 + i, s.G1[i]);
-  for (int h = tid; h < H; h += THREADS) { adam(p.off_b1 + h, s.gb1[h]); adam(p.off_w2 + h, s.G2[h]); }
-  if (tid == 0) adam(p.off_b2, gb2);
-  if (sn()) {  // persist the power-iteration state (in-place buffers of the parametrization)
-    for (int h = tid; h < H; h += THREADS) { a.disc.u[(int64_t)rr * a.disc.u_stride + h] = s.u1[h]; a.disc.v[(int64_t)rr * a.disc.v_stride + d + h] = s.v2[h]; }
-    for (int j = tid; j < d; j += THREADS) a.disc.v[(int64_t)rr * a.disc.v_stride + j] = s.v1[j];
-    if (tid == 0) a.disc.u[(int64_t)rr * a.disc.u_stride + H] = u2;
-  }
+  gail_finish(s, p, H, d, pu_gate, loss_bce, loss_gp, gb2, u2);
 }
 
 
@@ -489,6 +541,14 @@ __host__ __device__ inline int64_t tiled_carve(const TDims& g, float* base, TSme
   t.red = take(32); t.scal = take(32); t.part = take(4 * THREADS);
   if (s) *s = t;
   return o * 4;
+}
+// The tiled kernels' dims for a layout of gail_dims; row chunks of at most max_rb rows, a multiple of 16 so that the tile loops (H / 4 x RB / 4
+// tiles) have warp-uniform trip counts.
+__host__ inline TDims tiled_dims(const GailDims& g, int max_rb) {
+  TDims t;
+  t.S = g.S; t.A = g.A; t.d = g.d; t.DP = (g.d + 3) / 4 * 4; t.H = g.H; t.B = g.B; t.row = g.row; t.LDZ = g.H + 4; t.HD = g.HD;
+  t.RB = g.B < max_rb ? (g.B + 15) / 16 * 16 : max_rb;
+  return t;
 }
 struct GailTiledParams {
   il_gail_update_args a;
@@ -619,7 +679,7 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
   const il_gail_update_args& a = p.a;
   const int r = p.order ? p.order[blockIdx.x] : blockIdx.x, tid = threadIdx.x;
   const int H = g.H, d = g.d, B = g.B, DP = g.DP, LDZ = g.LDZ;
-  float* prm = a.disc.g.params + (int64_t)r * a.disc.g.stride;
+  const float* prm = a.disc.g.params + (int64_t)r * a.disc.g.stride;
   const bool sn_r = a.disc.u != nullptr && (!a.disc.spectral_norm_r || a.disc.spectral_norm_r[r] != 0);  // a replica at 0 never touches its u / v slots
   const float* pol = a.policy.rows + (int64_t)r * a.policy.replica_stride;
   const float* exp_ = a.expert.rows + (int64_t)r * a.expert.replica_stride;
@@ -629,62 +689,15 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
   // branches of a uniform run with 0
   const float grad_penalty = a.grad_penalty_r ? a.grad_penalty_r[r] : a.grad_penalty, entropy_bonus = a.entropy_bonus_r ? a.entropy_bonus_r[r] : a.entropy_bonus;
   const float invB = 1.f / (float)B;
-
-  for (int i = tid; i < H * d; i += THREADS) { s.W1[i] = prm[p.off_w1 + i]; s.G1[i] = 0.f; }
-  for (int h = tid; h < H; h += THREADS) {
-    s.b1[h] = prm[p.off_b1 + h]; s.w2[h] = prm[p.off_w2 + h]; s.G2[h] = 0.f; s.gb1[h] = 0.f;
-    if (sn_r) { s.u1[h] = a.disc.u[(int64_t)r * a.disc.u_stride + h]; s.v2[h] = a.disc.v[(int64_t)r * a.disc.v_stride + d + h]; }
-  }
-  if (sn_r) for (int j = tid; j < d; j += THREADS) s.v1[j] = a.disc.v[(int64_t)r * a.disc.v_stride + j];
-  const float b2 = prm[p.off_b2];
-  float u2 = sn_r ? a.disc.u[(int64_t)r * a.disc.u_stride + H] : 1.f;
-  // the per-replica choices (sweeps) live in shared memory and are re-read where used: the register budget of the tiled variants has no room
-  // for them (scal[0:2] is the AdamW scratch at the end)
-  if (tid == 0) {
-    s.scal[2] = __int_as_float(a.loss_function_r ? a.loss_function_r[r] : a.loss_function);
-    s.scal[3] = a.pos_class_prior_r ? a.pos_class_prior_r[r] : a.pos_class_prior;
-    s.scal[4] = a.nonnegative_margin_r ? a.nonnegative_margin_r[r] : a.nonnegative_margin;
-    s.scal[5] = sn_r ? 1.f : 0.f;
-    s.scal[6] = __int_as_float(r);
-  }
-  __syncthreads();
+  float b2, u2 = gail_load(s, p, prm, r, H, d, sn_r, b2);
   auto loss_function = [&] { return __float_as_int(s.scal[2]); };
-  auto sn = [&] { return s.scal[5] != 0.f; };
 
-  int kinds[3], n_pass = 0;
+  int kinds[3], gp_pass;
   const float* pass_eps[3] = {nullptr, nullptr, nullptr};
-  int gp_pass = -1;
-  if (loss_function() == IL_LOSS_MIXUP) { kinds[n_pass] = PASS_MIX; pass_eps[n_pass++] = eps_mix; }
-  else { kinds[n_pass++] = PASS_POLICY; kinds[n_pass++] = PASS_EXPERT; }
-  if (grad_penalty > 0.f) { gp_pass = n_pass; kinds[n_pass] = PASS_MIX; pass_eps[n_pass++] = eps_gp; }
+  const int n_pass = gail_schedule(loss_function(), grad_penalty, eps_mix, eps_gp, kinds, pass_eps, gp_pass);
 
-  // ---- phase 1: power iterations (identical to gail_update_kernel) -------------------------------------------------------------
   const int SF = gail_slot_floats(H, d);
-  for (int k = 0; k < n_pass; ++k) {
-    float* slot = s.slots + k * SF;
-    float sig1 = 1.f, sig2 = 1.f;
-    if (sn()) {
-      sig1 = spectral_sigma(s.W1, s.u1, s.v1, s.tvec, s.red, H, d, a.training != 0);
-      float t = 0.f;
-      if (a.training) {
-        for (int h = tid; h < H; h += THREADS) t = fmaf(s.w2[h], s.v2[h], t);
-        t = bsum(t, s.red);
-        u2 = t / fmaxf(fabsf(t), 1e-12f);
-        for (int h = tid; h < H; h += THREADS) s.tvec[h] = s.w2[h] * u2;
-        __syncthreads();
-        const float dn = fmaxf(sqrtf(sq_norm(s.tvec, H, s.red)), 1e-12f);
-        for (int h = tid; h < H; h += THREADS) s.v2[h] = s.tvec[h] / dn;
-        __syncthreads();
-      }
-      t = 0.f;
-      for (int h = tid; h < H; h += THREADS) t = fmaf(s.w2[h], s.v2[h], t);
-      sig2 = u2 * bsum(t, s.red);
-    }
-    for (int h = tid; h < H; h += THREADS) { slot[h] = s.u1[h]; slot[H + d + h] = s.v2[h]; }
-    for (int j = tid; j < d; j += THREADS) slot[H + j] = s.v1[j];
-    if (tid == 0) { slot[2 * H + d] = sig1; slot[2 * H + d + 1] = sig2; slot[2 * H + d + 2] = u2; }
-    __syncthreads();
-  }
+  gail_power_iterations(s, n_pass, H, d, a.training != 0, u2);
 
   auto set_effective = [&](const float* slot) {  // W1e [H][DP] and its transpose [DP][H], zero padded; w2e
     const float sig1 = slot[2 * H + d], sig2 = slot[2 * H + d + 1];
@@ -696,27 +709,16 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
     }
     for (int h = tid; h < H; h += THREADS) s.w2e[h] = s.w2[h] / sig2;
   };
-  // ---- phase 2 (PUGAIL): batch scalar of the clamp ---------------------------------------------------------------------------------
   float pu_gate = 1.f, loss_bce = 0.f, loss_gp = 0.f;
-  if (loss_function() == IL_LOSS_PUGAIL) {
-    float sums[2] = {0.f, 0.f};
-    for (int k = 0; k < 2; ++k) {
-      set_effective(s.slots + k * SF);
-      __syncthreads();
-      float part = 0.f;
-      for (int b0 = 0; b0 < B; b0 += g.RB) {
-        const int nb = min(g.RB, B - b0);
-        tiled_load_rows(g, pol, exp_, nullptr, kinds[k], b0, nb, s.X, s.CO, s.DF);
-        __syncthreads();
-        tiled_hidden_logits(g, s.X, s.W1eT, s.b1, s.Z, s.w2e, b2, s.F);
-        __syncthreads();
-        for (int b = tid; b < nb; b += THREADS) part += s.CO[b] * softplusf(s.F[b]);
-        __syncthreads();
-      }
-      sums[k] = bsum(part, s.red);
-    }
-    pu_gate = (s.scal[3] * (sums[1] * invB) - sums[0] * invB) >= -s.scal[4] ? 1.f : 0.f;
-  }
+  if (loss_function() == IL_LOSS_PUGAIL)
+    pu_gate = gail_pu_phase(s, B, g.RB, invB, [&](int k) { set_effective(s.slots + k * SF); },
+                            [&](int k, int b0, int nb) {
+                              tiled_load_rows(g, pol, exp_, nullptr, kinds[k], b0, nb, s.X, s.CO, s.DF);
+                              __syncthreads();
+                              tiled_hidden_logits(g, s.X, s.W1eT, s.b1, s.Z, s.w2e, b2, s.F);
+                              __syncthreads();
+                              return s.F;
+                            });
 
   // ---- phase 3: forward + backward per pass ---------------------------------------------------------------------------------------
   TileMap wm[NT];
@@ -771,20 +773,8 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
         for (int b = tid; b < g.RB; b += THREADS) {
           float df = 0.f;
           if (b < nb) {
-            const float f = s.F[b], w = s.CO[b], sg = sigmoidf(f);
-            if (loss_function() == IL_LOSS_MIXUP) {
-              const float e = s.DF[b];
-              df = w * (sg - e) * invB;
-              loss_part += e * w * softplusf(-f) + (1.f - e) * w * softplusf(f);
-            } else if (loss_function() == IL_LOSS_BCE) {
-              df = kind == PASS_EXPERT ? w * (sg - 1.f) * invB : w * sg * invB;
-              loss_part += kind == PASS_EXPERT ? w * softplusf(-f) : w * softplusf(f);
-            } else {
-              const float pr = s.scal[3];
-              df = kind == PASS_EXPERT ? pr * w * (sg - 1.f) * invB + pu_gate * pr * w * sg * invB : -pu_gate * w * sg * invB;
-              loss_part += kind == PASS_EXPERT ? pr * w * softplusf(-f) + pu_gate * pr * w * softplusf(f) : -pu_gate * w * softplusf(f);
-            }
-            if (entropy_bonus > 0.f) df += entropy_bonus * w * f * sg * (1.f - sg) * invB;
+            const bool mix = loss_function() == IL_LOSS_MIXUP;
+            df = gail_loss_row(s.F[b], s.CO[b], mix, mix ? s.DF[b] : 0.f, loss_function(), kind == PASS_EXPERT, s.scal[3], pu_gate, entropy_bonus, invB, loss_part);
             gb2k += df;
           }
           s.DF[b] = df;  // padded rows: 0
@@ -905,68 +895,14 @@ __global__ void __launch_bounds__(THREADS, 2) gail_update_tiled_kernel(const Gai
       }
     }
     __syncthreads();
-    // ---- spectral-norm backward: dL/dW = (G - <G, W_eff> u v^T) / sigma, accumulated over the passes
-    float inner1 = 0.f, inner2 = 0.f;
-    if (sn()) {
-      for (int e = tid; e < H * d; e += THREADS) inner1 = fmaf(s.G1k[(e / d) * DP + e % d], s.W1e[(e / d) * DP + e % d], inner1);
-      inner1 = bsum(inner1, s.red);
-      for (int h = tid; h < H; h += THREADS) inner2 = fmaf(s.G2k[h], s.w2e[h], inner2);
-      inner2 = bsum(inner2, s.red);
-    }
-    for (int e = tid; e < H * d; e += THREADS) {
-      const int h = e / d, j = e % d;
-      const float gk = s.G1k[h * DP + j];
-      s.G1[e] += sn() ? (gk - inner1 * slot[h] * slot[H + j]) / sig1 : gk;
-    }
-    for (int h = tid; h < H; h += THREADS) {
-      s.G2[h] += sn() ? (s.G2k[h] - inner2 * u2k * slot[H + d + h]) / sig2 : s.G2k[h];
-      s.gb1[h] += s.gb1k[h];
-    }
-    gb2k = bsum(gb2k, s.red);
-    gb2 += gb2k;
-    loss_part = bsum(loss_part, s.red);
-    if (is_gp) loss_gp = loss_part * invB; else loss_bce += loss_part * invB;
-    __syncthreads();
+    gail_project_pass(s, slot, H, d, sig1, sig2, u2k, is_gp, gb2k, loss_part, invB, gb2, loss_bce, loss_gp, [&](auto f) {  // dL/dW1e in G1k [H][DP]
+      for (int e = tid; e < H * d; e += THREADS) {
+        const int q = (e / d) * DP + e % d;
+        f(e, s.G1k[q], s.W1e[q]);
+      }
+    });
   }
-  // the replica index (order[blockIdx.x] in a width-class launch) and the pointers derived from it are re-derived from shared memory here:
-  // kept live from the start in registers they cost the tiled variants spills
-  const int rr = __float_as_int(s.scal[6]);
-  // PUGAIL with the clamp active: policy_loss = -margin (training.py:102); its gated terms were left out of loss_bce above
-  if (pu_gate == 0.f) loss_bce -= s.scal[4];
-  if (tid == 0 && a.out_losses) { a.out_losses[rr * 2 + 0] = loss_bce; a.out_losses[rr * 2 + 1] = loss_gp; }
-
-  // ---- AdamW (train.py:84; torch _single_tensor_adam) -----------------------------------------------------------
-  const double lr = a.opt.lr_r ? a.opt.lr_r[rr] : a.opt.lr, wd = a.opt.weight_decay_r ? a.opt.weight_decay_r[rr] : a.opt.weight_decay;
-  if (tid == 0) {
-    const double t = (double)*a.opt.step;
-    s.scal[0] = (float)(lr / (1.0 - pow(a.opt.beta1, t)));
-    s.scal[1] = (float)sqrt(1.0 - pow(a.opt.beta2, t));
-  }
-  __syncthreads();
-  const float step_size = s.scal[0], bc2_sqrt = s.scal[1];
-  const float decay = (float)(1.0 - lr * wd), w1c = (float)(1.0 - a.opt.beta1), w2c = (float)(1.0 - a.opt.beta2), beta2 = (float)a.opt.beta2,
-              eps = (float)a.opt.eps;
-  const bool has_wd = wd != 0.0;
-  prm = a.disc.g.params + (int64_t)rr * a.disc.g.stride;
-  float* am = a.opt.m + (int64_t)rr * a.disc.g.stride;
-  float* avv = a.opt.v + (int64_t)rr * a.disc.g.stride;
-  auto adam = [&](int64_t off, float grad) {
-    float pi = prm[off], mi = am[off], vi = avv[off];
-    if (has_wd) pi = __fmul_rn(pi, decay);
-    mi = __fadd_rn(mi, __fmul_rn(w1c, __fsub_rn(grad, mi)));
-    vi = __fadd_rn(__fmul_rn(vi, beta2), __fmul_rn(__fmul_rn(w2c, grad), grad));
-    const float denom = __fadd_rn(__fdiv_rn(sqrtf(vi), bc2_sqrt), eps);
-    pi = __fadd_rn(pi, __fmul_rn(-step_size, __fdiv_rn(mi, denom)));
-    prm[off] = pi; am[off] = mi; avv[off] = vi;
-  };
-  for (int i = tid; i < H * d; i += THREADS) adam(p.off_w1 + i, s.G1[i]);
-  for (int h = tid; h < H; h += THREADS) { adam(p.off_b1 + h, s.gb1[h]); adam(p.off_w2 + h, s.G2[h]); }
-  if (tid == 0) adam(p.off_b2, gb2);
-  if (sn()) {
-    for (int h = tid; h < H; h += THREADS) { a.disc.u[(int64_t)rr * a.disc.u_stride + h] = s.u1[h]; a.disc.v[(int64_t)rr * a.disc.v_stride + d + h] = s.v2[h]; }
-    for (int j = tid; j < d; j += THREADS) a.disc.v[(int64_t)rr * a.disc.v_stride + j] = s.v1[j];
-    if (tid == 0) a.disc.u[(int64_t)rr * a.disc.u_stride + H] = u2;
-  }
+  gail_finish(s, p, H, d, pu_gate, loss_bce, loss_gp, gb2, u2);
 }
 
 __global__ void __launch_bounds__(THREADS) gail_reward_kernel(const GailRewParams p) {
@@ -975,24 +911,9 @@ __global__ void __launch_bounds__(THREADS) gail_reward_kernel(const GailRewParam
   GailSmem s;
   gail_carve(g, sm, &s);
   const int r = p.order ? p.order[blockIdx.x] : blockIdx.x, tid = threadIdx.x, H = g.H, d = g.d, B = g.B;
-  const float* prm = p.disc.g.params + (int64_t)r * p.disc.g.stride;
-  const bool sn = p.disc.u != nullptr && (!p.disc.spectral_norm_r || p.disc.spectral_norm_r[r] != 0);
   const int reward_function = p.disc.reward_function_r ? p.disc.reward_function_r[r] : p.disc.reward_function;
-  for (int i = tid; i < H * d; i += THREADS) s.W1[i] = prm[p.off_w1 + i];
-  for (int h = tid; h < H; h += THREADS) {
-    s.b1[h] = prm[p.off_b1 + h]; s.w2[h] = prm[p.off_w2 + h];
-    if (sn) { s.u1[h] = p.disc.u[(int64_t)r * p.disc.u_stride + h]; s.v2[h] = p.disc.v[(int64_t)r * p.disc.v_stride + d + h]; }
-  }
-  if (sn) for (int j = tid; j < d; j += THREADS) s.v1[j] = p.disc.v[(int64_t)r * p.disc.v_stride + j];
-  const float b2 = prm[p.off_b2];
-  __syncthreads();
-  float sig1 = 1.f, sig2 = 1.f;
-  if (sn) {  // eval mode: no power iteration, sigma from the stored (u, v) (train.py:180,194)
-    sig1 = spectral_sigma(s.W1, s.u1, s.v1, s.tvec, s.red, H, d, false);
-    float t = 0.f;
-    for (int h = tid; h < H; h += THREADS) t = fmaf(s.w2[h], s.v2[h], t);
-    sig2 = p.disc.u[(int64_t)r * p.disc.u_stride + H] * bsum(t, s.red);
-  }
+  float sig1, sig2;
+  const float b2 = gail_reward_load(p, r, H, d, s.W1, s.b1, s.w2, s.u1, s.v1, s.v2, s.tvec, s.red, sig1, sig2);
   for (int i = tid; i < H * d; i += THREADS) s.W1e[i] = s.W1[i] / sig1;
   for (int h = tid; h < H; h += THREADS) s.w2e[h] = s.w2[h] / sig2;
   __syncthreads();
@@ -1003,14 +924,7 @@ __global__ void __launch_bounds__(THREADS) gail_reward_kernel(const GailRewParam
     __syncthreads();
     forward_chunk(g, s, nb, b2, s.DF);
     for (int b = tid; b < nb; b += THREADS) {
-      const float f = s.DF[b];
-      if (p.logits) p.logits[(int64_t)r * B + b0 + b] = f;
-      if (p.reward) {  // models.py:177-180
-        const float D = sigmoidf(f);
-        float hh = reward_function == IL_REWARD_GAIL ? -log1pf(-D + 1e-6f) : logf(D + 1e-6f) - log1pf(-D + 1e-6f);
-        if (reward_function == IL_REWARD_FAIRL) hh = expf(hh) * -hh;
-        p.reward[(int64_t)r * p.reward_rs + (int64_t)(b0 + b) * p.reward_ld] = hh;
-      }
+      gail_reward_store(p, r, B, b0 + b, s.DF[b], reward_function);
     }
     __syncthreads();
   }
@@ -1033,24 +947,9 @@ __global__ void __launch_bounds__(THREADS, 3) gail_reward_tiled_kernel(const Gai
   float *W1 = take(g.HD), *W1eT = take(DP * H), *b1 = take(H), *w2 = take(H), *w2e = take(H), *u1 = take(H), *v2 = take(H), *spare = take(H), *v1 = take(d), *tvec = take(H > d ? H : d);
   float *X = take(g.RB * DP), *Z = take(g.RB * g.LDZ), *F = take(g.RB), *CO = take(g.RB), *DF = take(g.RB), *red = take(32);
   (void)spare;
-  const float* prm = p.disc.g.params + (int64_t)r * p.disc.g.stride;
-  const bool sn = p.disc.u != nullptr && (!p.disc.spectral_norm_r || p.disc.spectral_norm_r[r] != 0);
   const int reward_function = p.disc.reward_function_r ? p.disc.reward_function_r[r] : p.disc.reward_function;
-  for (int i = tid; i < H * d; i += THREADS) W1[i] = prm[p.off_w1 + i];
-  for (int h = tid; h < H; h += THREADS) {
-    b1[h] = prm[p.off_b1 + h]; w2[h] = prm[p.off_w2 + h];
-    if (sn) { u1[h] = p.disc.u[(int64_t)r * p.disc.u_stride + h]; v2[h] = p.disc.v[(int64_t)r * p.disc.v_stride + d + h]; }
-  }
-  if (sn) for (int j = tid; j < d; j += THREADS) v1[j] = p.disc.v[(int64_t)r * p.disc.v_stride + j];
-  const float b2 = prm[p.off_b2];
-  __syncthreads();
-  float sig1 = 1.f, sig2 = 1.f;
-  if (sn) {  // eval mode: no power iteration, sigma from the stored (u, v) (train.py:180,194)
-    sig1 = spectral_sigma(W1, u1, v1, tvec, red, H, d, false);
-    float t = 0.f;
-    for (int h = tid; h < H; h += THREADS) t = fmaf(w2[h], v2[h], t);
-    sig2 = p.disc.u[(int64_t)r * p.disc.u_stride + H] * bsum(t, red);
-  }
+  float sig1, sig2;
+  const float b2 = gail_reward_load(p, r, H, d, W1, b1, w2, u1, v1, v2, tvec, red, sig1, sig2);
   for (int i = tid; i < H * DP; i += THREADS) {
     const int h = i / DP, j = i % DP;
     W1eT[j * H + h] = j < d ? W1[h * d + j] / sig1 : 0.f;
@@ -1065,14 +964,7 @@ __global__ void __launch_bounds__(THREADS, 3) gail_reward_tiled_kernel(const Gai
     tiled_hidden_logits(g, X, W1eT, b1, Z, w2e, b2, F);
     __syncthreads();
     for (int b = tid; b < nb; b += THREADS) {
-      const float f = F[b];
-      if (p.logits) p.logits[(int64_t)r * B + b0 + b] = f;
-      if (p.reward) {  // models.py:177-180
-        const float D = sigmoidf(f);
-        float hh = reward_function == IL_REWARD_GAIL ? -log1pf(-D + 1e-6f) : logf(D + 1e-6f) - log1pf(-D + 1e-6f);
-        if (reward_function == IL_REWARD_FAIRL) hh = expf(hh) * -hh;
-        p.reward[(int64_t)r * p.reward_rs + (int64_t)(b0 + b) * p.reward_ld] = hh;
-      }
+      gail_reward_store(p, r, B, b0 + b, F[b], reward_function);
     }
   }
 }
@@ -1154,8 +1046,7 @@ int gail_update_plan(il_handle* h, const il_gail_update_args* a, const WidthClas
     GailTiledParams& tp = pl->tp;
     tp.a = *a;
     TDims& t = tp.g;
-    t.S = p.g.S; t.A = p.g.A; t.d = p.g.d; t.DP = (p.g.d + 3) / 4 * 4; t.H = p.g.H; t.B = p.g.B; t.row = p.g.row; t.LDZ = p.g.H + 4; t.HD = (p.g.H * p.g.d + 3) / 4 * 4;
-    t.RB = a->policy.B < 128 ? (a->policy.B + 15) / 16 * 16 : 128;  // multiple of 16: the tile loops (H / 4 x RB / 4 tiles) have warp-uniform trip counts
+    t = tiled_dims(p.g, 128);
     tp.off_w1 = off[0]; tp.off_b1 = off[1]; tp.off_w2 = off[2]; tp.off_b2 = off[3];
     tp.order = wc.order;
     tsm = tiled_carve(t, nullptr, nullptr);
@@ -1204,9 +1095,7 @@ int gail_reward_launch(il_handle* h, const il_gail* disc, const WidthClass& wc, 
   if (h->gail_tiled && p.g.d <= 32 && (p.g.H == 32 || p.g.H == 64 || p.g.H == 128) && p.g.row % 4 == 0) {
     GailRewTiledParams tp;
     tp.r = p;
-    TDims& t = tp.g;
-    t.S = p.g.S; t.A = p.g.A; t.d = p.g.d; t.DP = (p.g.d + 3) / 4 * 4; t.H = p.g.H; t.B = p.g.B; t.row = p.g.row; t.LDZ = p.g.H + 4; t.HD = (p.g.H * p.g.d + 3) / 4 * 4;
-    t.RB = batch->B < 64 ? (batch->B + 15) / 16 * 16 : 64;
+    const TDims& t = tp.g = tiled_dims(p.g, 64);
     const int64_t tsm = reward_tiled_floats(t) * 4;
     if (tsm <= 72 * 1024) {
       IL_LAUNCH(h, gail_reward_tiled_kernel, wc.blocks, THREADS, (size_t)tsm, st, tp);

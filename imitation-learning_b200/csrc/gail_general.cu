@@ -11,6 +11,7 @@
 //       dW_{l+1} += delta_{l+1}^T ubar_l,  dbar_{l+1} = ubar_l W_{l+1}^T,  and through s'(z_l):  zbar_l = dbar_l * u_l * s''(y_l)
 //       back-propagated like an ordinary loss gradient (zero for relu);
 //   * gradients w.r.t. W_eff are projected through each access: dW = (G - <G, W_eff> u v^T) / sigma (SURVEY §8a a12).
+#include "gail_loss.cuh"
 #include "mlp.cuh"
 
 namespace {
@@ -47,17 +48,17 @@ __host__ __device__ inline SnLayout sn_layout(const int32_t* dims, int L) {
   return s;
 }
 
-// Whether replica r takes part in one pass of the update (sweeps of the loss function and of the gradient penalty). kind: 0 policy, 1 expert,
-// 2 Mixup, 3 penalty, -1 every replica. A Mixup replica lives in the Mixup pass only, a BCE / PUGAIL one in the policy and expert passes.
+// Whether replica r takes part in one pass of the update (sweeps of the loss function and of the gradient penalty); PASS_ANY: every replica.
+// A Mixup replica lives in the Mixup pass only, a BCE / PUGAIL one in the policy and expert passes.
 struct Live {
   const int32_t* loss_r;  // loss_function_r (nullptr: every loss pass is live)
   const int32_t* pen_r;   // penalty_pass_r (nullptr: the penalty pass is live)
-  int kind;
+  int kind;               // PassKind
 };
 __device__ __forceinline__ bool live_at(const Live& l, int r) {
-  if (l.kind == 3) return !l.pen_r || l.pen_r[r] != 0;
-  if (l.kind < 0 || !l.loss_r) return true;
-  return (l.loss_r[r] == IL_LOSS_MIXUP) == (l.kind == 2);
+  if (l.kind == PASS_PENALTY) return !l.pen_r || l.pen_r[r] != 0;
+  if (l.kind == PASS_ANY || !l.loss_r) return true;
+  return (l.loss_r[r] == IL_LOSS_MIXUP) == (l.kind == PASS_MIX);
 }
 
 // One spectral-norm access of every layer of R nets. One CTA per replica. eff receives W / sigma (or W / 1 without spectral norm)
@@ -186,7 +187,7 @@ struct PassView {        // one discriminator forward (models.py:172-175) on a b
   float* dg;             // [R, B] out: dLoss / d g-output;  dhn, dhs likewise
   float* dhn;
   float* dhs;
-  int kind;              // 0 policy, 1 expert, 2 mixup
+  int kind;              // PASS_POLICY, PASS_EXPERT or PASS_MIX
 };
 struct LossParams {
   PassView pass[3];
@@ -234,7 +235,7 @@ __global__ void __launch_bounds__(256) gailx_loss_kernel(const LossParams p) {
     }
     sp = block_sum(sp, red);
     se = block_sum(se, red);
-    pu_gate = (prior * (se * invB) - sp * invB) >= -nonnegative_margin ? 1.f : 0.f;
+    pu_gate = gail_pu_gate(sp, se, prior, nonnegative_margin, invB);
   }
   float loss = 0.f;
   for (int k = 0; k < p.n_pass; ++k) {
@@ -248,22 +249,10 @@ __global__ void __launch_bounds__(256) gailx_loss_kernel(const LossParams p) {
         continue;
       }
       float omt;
-      const float f = pass_logit(v, p, r, b, &omt), sg = sigmoidf(f);
+      const float f = pass_logit(v, p, r, b, &omt);
       const float w = v.rows[(int64_t)r * v.rs + (int64_t)b * p.row + p.off_weight];
-      float df;
-      if (v.kind == 2) {
-        const float e = v.eps[(int64_t)r * B + b];
-        df = w * (sg - e) * invB;
-        loss += e * w * softplusf(-f) + (1.f - e) * w * softplusf(f);
-      } else if (loss_function == IL_LOSS_BCE) {
-        df = v.kind == 1 ? w * (sg - 1.f) * invB : w * sg * invB;
-        loss += v.kind == 1 ? w * softplusf(-f) : w * softplusf(f);
-      } else {
-        const float pr = prior;
-        df = v.kind == 1 ? pr * w * (sg - 1.f) * invB + pu_gate * pr * w * sg * invB : -pu_gate * w * sg * invB;
-        loss += v.kind == 1 ? pr * w * softplusf(-f) + pu_gate * pr * w * softplusf(f) : -pu_gate * w * softplusf(f);
-      }
-      if (entropy_bonus > 0.f) df += entropy_bonus * w * f * sg * (1.f - sg) * invB;
+      const bool mix = v.kind == PASS_MIX;
+      const float df = gail_loss_row(f, w, mix, mix ? v.eps[(int64_t)r * B + b] : 0.f, loss_function, v.kind == PASS_EXPERT, prior, pu_gate, entropy_bonus, invB, loss);
       const int64_t i = (int64_t)r * B + b;
       v.dg[i] = df;
       if (p.shaping) { v.dhn[i] = df * omt * discount; v.dhs[i] = -df * omt; }
@@ -360,12 +349,7 @@ __global__ void gailx_reward_kernel(PassView v, LossParams p, int reward_functio
   float omt;
   const float f = pass_logit(v, p, r, b, &omt);
   if (logits) logits[t] = f;
-  if (reward) {
-    const float D = sigmoidf(f);
-    float hh = reward_function == IL_REWARD_GAIL ? -log1pf(-D + 1e-6f) : logf(D + 1e-6f) - log1pf(-D + 1e-6f);
-    if (reward_function == IL_REWARD_FAIRL) hh = expf(hh) * -hh;
-    reward[(int64_t)r * reward_rs + (int64_t)b * reward_ld] = hh;
-  }
+  if (reward) reward[(int64_t)r * reward_rs + (int64_t)b * reward_ld] = gail_reward_of_logit(f, reward_function);
 }
 
 // ---- host-side program ----------------------------------------------------------------------------------------------------------
@@ -408,7 +392,7 @@ int max_dim(const il_mlp* m) {
 }
 
 void eval_carve(Carver& c, NetEval& e, const il_mlp* net, float* u, float* v, int us, int vs, const int32_t* sn_r, int R, int B, bool need_grad) {
-  e.net = net; e.u = u; e.v = v; e.u_stride = us; e.v_stride = vs; e.sn_r = sn_r; e.live = Live{nullptr, nullptr, -1};
+  e.net = net; e.u = u; e.v = v; e.u_stride = us; e.v_stride = vs; e.sn_r = sn_r; e.live = Live{nullptr, nullptr, PASS_ANY};
   e.eff = *net;
   e.eff.params = c.take((int64_t)R * net->stride);
   e.snap_stride = snap_floats(net);
@@ -560,7 +544,7 @@ struct UpdLayout {
 // the gradient-penalty pass runs when grad_penalty > 0, or, with per-replica values, when the caller passes its noise (eps_gp)
 bool gp_enabled(const il_gailx_update_args* a) { return a->grad_penalty_r ? a->eps_gp != nullptr : a->grad_penalty > 0.f; }
 
-// The loss passes of one update, in order (Live kinds: 0 policy, 1 expert, 2 Mixup), then the penalty pass when gp. Without loss_function_r a
+// The loss passes of one update, in order (policy, expert, Mixup), then the penalty pass when gp. Without loss_function_r a
 // Mixup run has the Mixup pass only, a BCE / PUGAIL run the policy and expert passes; with it the policy and expert passes always run and the
 // Mixup pass runs when eps_mix is passed, so each replica's live accesses come in the order of its own single run.
 struct Schedule {
@@ -570,9 +554,9 @@ struct Schedule {
 Schedule schedule(const il_gailx_update_args* a) {
   Schedule s{};
   const bool per_replica = a->loss_function_r != nullptr;
-  if (per_replica || a->loss_function != IL_LOSS_MIXUP) { s.kind[s.n_loss++] = 0; s.kind[s.n_loss++] = 1; }
-  if (per_replica ? a->eps_mix != nullptr : a->loss_function == IL_LOSS_MIXUP) s.kind[s.n_loss++] = 2;
-  s.mixup = s.kind[s.n_loss - 1] == 2;
+  if (per_replica || a->loss_function != IL_LOSS_MIXUP) { s.kind[s.n_loss++] = PASS_POLICY; s.kind[s.n_loss++] = PASS_EXPERT; }
+  if (per_replica ? a->eps_mix != nullptr : a->loss_function == IL_LOSS_MIXUP) s.kind[s.n_loss++] = PASS_MIX;
+  s.mixup = s.kind[s.n_loss - 1] == PASS_MIX;
   s.gp = gp_enabled(a);
   return s;
 }
@@ -587,7 +571,7 @@ void upd_layout(const il_gailx_update_args* a, char* base, UpdLayout* L) {
   L->n_ev = 0;
   for (int k = 0; k < sc.n_loss + (gp ? 1 : 0); ++k) {
     const bool is_gp = k == sc.n_loss;
-    const Live live{a->loss_function_r, a->penalty_pass_r, is_gp ? 3 : sc.kind[k]};
+    const Live live{a->loss_function_r, a->penalty_pass_r, is_gp ? PASS_PENALTY : sc.kind[k]};
     const int first = L->n_ev;
     eval_carve(c, L->ev[L->n_ev++], &d.g, d.g_u, d.g_v, d.g_u_stride, d.g_v_stride, d.spectral_norm_r, R, B, true);
     if (shaping) {
@@ -646,7 +630,7 @@ extern "C" int il_gailx_update(il_handle* h, const il_gailx_update_args* a, void
   const int n_loss_pass = sc.n_loss;
   IL_CHECK(!(gp && !a->eps_gp) && !(mixup && !a->eps_mix), "il_gailx_update: missing eps_gp / eps_mix");
   IL_CHECK(!(gp && d.state_only), "il_gailx_update: grad_penalty with a state-only discriminator is undefined in the reference (autograd.grad on the unused action, training.py:125)");
-  const float* logp_of[3] = {a->logp_policy, a->logp_expert, a->logp_mix};
+  const float* logp_of[3] = {a->logp_policy, a->logp_expert, a->logp_mix};  // by PassKind
   for (int k = 0; k < n_loss_pass; ++k) IL_CHECK(!sublp || logp_of[sc.kind[k]], "il_gailx_update: subtract_log_policy needs the log-policy inputs of every pass that runs");
   IL_CHECK(a->workspace && a->workspace_bytes >= il_gailx_workspace_bytes(a), "il_gailx_update: workspace too small");
   UpdLayout L;
@@ -662,12 +646,12 @@ extern "C" int il_gailx_update(il_handle* h, const il_gailx_update_args* a, void
   // ---- batches of the passes ------------------------------------------------------------------------------------------------
   const float* pass_rows[4]; int64_t pass_rs[4];
   for (int k = 0; k < n_loss_pass; ++k) {
-    if (sc.kind[k] == 2) {
+    if (sc.kind[k] == PASS_MIX) {
       il_batch ob = a->policy; ob.rows = L.mix_rows[0]; ob.replica_stride = (int64_t)B * row;
       IL_TRY(il_gail_mix_batch(h, &a->expert, &a->policy, a->eps_mix, R, &ob, stream));
       pass_rows[k] = L.mix_rows[0]; pass_rs[k] = (int64_t)B * row;
     } else {
-      const il_batch& b = sc.kind[k] == 0 ? a->policy : a->expert;
+      const il_batch& b = sc.kind[k] == PASS_POLICY ? a->policy : a->expert;
       pass_rows[k] = b.rows; pass_rs[k] = b.replica_stride;
     }
   }
@@ -704,7 +688,7 @@ extern "C" int il_gailx_update(il_handle* h, const il_gailx_update_args* a, void
     if (shaping) { v.ohn = e[1].out; v.ohs = e[2].out; v.dhn = e[1].dout; v.dhs = e[2].dout; }
     v.kind = sc.kind[k];
     v.logp = sublp ? logp_of[v.kind] : nullptr;
-    v.eps = v.kind == 2 ? a->eps_mix : nullptr;
+    v.eps = v.kind == PASS_MIX ? a->eps_mix : nullptr;
   }
   IL_LAUNCH(h, gailx_loss_kernel, R, 256, 0, st, lp);
   GX_STAGE(h, st, "loss");

@@ -441,37 +441,23 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
                             const AdamReplicas rp) {
   extern __shared__ AdamCoef adam_tab[];
   __shared__ float s_step_size, s_bc2_sqrt;
-  if (threadIdx.x == 0) {  // torch _single_tensor_adam: Python-double scalars, then cast to the tensor dtype
-    const double t = (double)*step;
-    const double bc1 = 1.0 - pow(beta1_d, t), bc2 = 1.0 - pow(beta2_d, t);
-    s_step_size = (float)(lr / bc1);
-    s_bc2_sqrt = (float)sqrt(bc2);
-  }
+  if (threadIdx.x == 0) adamw_bias_correction(lr, beta1_d, beta2_d, *step, s_step_size, s_bc2_sqrt);
   adam_fill_table(adam_tab, rp, lr, wd, beta1_d, step, tau);
   __syncthreads();
-  const float step_size = s_step_size, bc2_sqrt = s_bc2_sqrt;
-  const float decay = (float)(1.0 - lr * wd), w1 = (float)(1.0 - beta1_d), w2 = (float)(1.0 - beta2_d);
-  const float beta2 = (float)beta2_d, eps = (float)eps_d;
-  const bool has_wd = wd != 0.0;
-  auto upd = [&](float& pi, float& mi, float& vi, float gi, float ss, float dc, bool wdf) {
-    if (wdf) pi = __fmul_rn(pi, dc);                                           // param.mul_(1 - lr * weight_decay)
-    mi = __fadd_rn(mi, __fmul_rn(w1, __fsub_rn(gi, mi)));                      // exp_avg.lerp_(grad, 1 - beta1)
-    vi = __fadd_rn(__fmul_rn(vi, beta2), __fmul_rn(__fmul_rn(w2, gi), gi));    // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value=1 - beta2)
-    const float denom = __fadd_rn(__fdiv_rn(sqrtf(vi), bc2_sqrt), eps);        // (exp_avg_sq.sqrt() / bias_correction2_sqrt).add_(eps)
-    pi = __fadd_rn(pi, __fmul_rn(-ss, __fdiv_rn(mi, denom)));                  // param.addcdiv_(exp_avg, denom, value=-step_size)
-  };
+  const AdamW c = adamw_coefs(s_step_size, s_bc2_sqrt, lr, wd, beta1_d, beta2_d, eps_d);
   // n is a multiple of 4 and all buffers are 16-byte aligned (flat parameter layout): 128-bit streams
   const int64_t n4 = n >> 2;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-    float ss = step_size, dc = decay, ta = tau, omt = one_minus_tau;
-    bool wdf = has_wd;
+    float ss = c.step_size, dc = c.decay, ta = tau, omt = one_minus_tau;
+    bool wdf = c.has_wd;
     if (rp.R) {
-      const AdamCoef c = adam_tab[adam_replica(i << 2, rp)];
-      ss = c.step_size; dc = c.decay; wdf = c.decay != 1.f; ta = c.tau; omt = c.one_minus_tau;
+      const AdamCoef rc = adam_tab[adam_replica(i << 2, rp)];
+      ss = rc.step_size; dc = rc.decay; wdf = rc.decay != 1.f; ta = rc.tau; omt = rc.one_minus_tau;
     }
     float4 pv = reinterpret_cast<float4*>(p)[i], mv = reinterpret_cast<float4*>(m)[i], vv = reinterpret_cast<float4*>(v)[i];
     const float4 gv = reinterpret_cast<const float4*>(g)[i];
-    upd(pv.x, mv.x, vv.x, gv.x, ss, dc, wdf); upd(pv.y, mv.y, vv.y, gv.y, ss, dc, wdf); upd(pv.z, mv.z, vv.z, gv.z, ss, dc, wdf); upd(pv.w, mv.w, vv.w, gv.w, ss, dc, wdf);
+    adamw_update(c, pv.x, mv.x, vv.x, gv.x, ss, dc, wdf); adamw_update(c, pv.y, mv.y, vv.y, gv.y, ss, dc, wdf);
+    adamw_update(c, pv.z, mv.z, vv.z, gv.z, ss, dc, wdf); adamw_update(c, pv.w, mv.w, vv.w, gv.w, ss, dc, wdf);
     reinterpret_cast<float4*>(p)[i] = pv; reinterpret_cast<float4*>(m)[i] = mv; reinterpret_cast<float4*>(v)[i] = vv;
     if (target) {  // fused update_target_network (models.py:81)
       const float tau = ta, one_minus_tau = omt;
@@ -483,7 +469,7 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
   }
   for (int64_t i = (n4 << 2) + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {  // tail (< 4 elements; uniform only)
     float pi = p[i], mi = m[i], vi = v[i];
-    upd(pi, mi, vi, g[i], step_size, decay, has_wd);
+    adamw_update(c, pi, mi, vi, g[i]);
     p[i] = pi; m[i] = mi; v[i] = vi;
     if (target) target[i] = __fadd_rn(__fmul_rn(target[i], tau), __fmul_rn(one_minus_tau, pi));
   }
@@ -520,9 +506,7 @@ __global__ void __launch_bounds__(ADAM_CONSUMERS + 32) adam_tma_kernel(float* __
   const int tid = threadIdx.x;
   adam_fill_table(tab, rp, lr, wd, beta1_d, step, tau);
   if (tid == 0) {
-    const double t = (double)*step;
-    s_step_size = (float)(lr / (1.0 - pow(beta1_d, t)));
-    s_bc2_sqrt = (float)sqrt(1.0 - pow(beta2_d, t));
+    adamw_bias_correction(lr, beta1_d, beta2_d, *step, s_step_size, s_bc2_sqrt);
     for (int s_ = 0; s_ < STAGES; ++s_) {
       asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(full0 + 8u * s_));
       asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(done0 + 8u * s_), "r"(ADAM_CONSUMERS));
@@ -568,16 +552,7 @@ __global__ void __launch_bounds__(ADAM_CONSUMERS + 32) adam_tma_kernel(float* __
     return;
   }
   // ---- compute threads ----
-  const float step_size = s_step_size, bc2_sqrt = s_bc2_sqrt;
-  const float decay = (float)(1.0 - lr * wd), w1 = (float)(1.0 - beta1_d), w2 = (float)(1.0 - beta2_d), beta2 = (float)beta2_d, eps = (float)eps_d;
-  const bool has_wd = wd != 0.0;
-  auto upd = [&](float& pi, float& mi, float& vi, float gi, float ss, float dc, bool wdf) {
-    if (wdf) pi = __fmul_rn(pi, dc);
-    mi = __fadd_rn(mi, __fmul_rn(w1, __fsub_rn(gi, mi)));
-    vi = __fadd_rn(__fmul_rn(vi, beta2), __fmul_rn(__fmul_rn(w2, gi), gi));
-    const float denom = __fadd_rn(__fdiv_rn(sqrtf(vi), bc2_sqrt), eps);
-    pi = __fadd_rn(pi, __fmul_rn(-ss, __fdiv_rn(mi, denom)));
-  };
+  const AdamW c = adamw_coefs(s_step_size, s_bc2_sqrt, lr, wd, beta1_d, beta2_d, eps_d);
   for (int64_t k = 0; k < my_tiles; ++k) {
     const int stage = (int)(k % STAGES);
     const int64_t tile = blockIdx.x + k * gridDim.x;
@@ -589,15 +564,16 @@ __global__ void __launch_bounds__(ADAM_CONSUMERS + 32) adam_tma_kernel(float* __
     float4* sv = reinterpret_cast<float4*>(buf + (stage * ADAM_STREAMS + 3) * TILE);
     float4* stg = reinterpret_cast<float4*>(buf + (stage * ADAM_STREAMS + 4) * TILE);
     for (int i = tid; i < nf4; i += ADAM_CONSUMERS) {
-      float ss = step_size, dc = decay, ta = tau, omt = one_minus_tau;
-      bool wdf = has_wd;
+      float ss = c.step_size, dc = c.decay, ta = tau, omt = one_minus_tau;
+      bool wdf = c.has_wd;
       if (rp.R) {  // a tile may straddle replica boundaries: look up per float4
-        const AdamCoef c = tab[adam_replica(tile * TILE + 4 * i, rp)];
-        ss = c.step_size; dc = c.decay; wdf = c.decay != 1.f; ta = c.tau; omt = c.one_minus_tau;
+        const AdamCoef rc = tab[adam_replica(tile * TILE + 4 * i, rp)];
+        ss = rc.step_size; dc = rc.decay; wdf = rc.decay != 1.f; ta = rc.tau; omt = rc.one_minus_tau;
       }
       float4 pv = sp[i], mv = smm[i], vv = sv[i];
       const float4 gv = sg[i];
-      upd(pv.x, mv.x, vv.x, gv.x, ss, dc, wdf); upd(pv.y, mv.y, vv.y, gv.y, ss, dc, wdf); upd(pv.z, mv.z, vv.z, gv.z, ss, dc, wdf); upd(pv.w, mv.w, vv.w, gv.w, ss, dc, wdf);
+      adamw_update(c, pv.x, mv.x, vv.x, gv.x, ss, dc, wdf); adamw_update(c, pv.y, mv.y, vv.y, gv.y, ss, dc, wdf);
+      adamw_update(c, pv.z, mv.z, vv.z, gv.z, ss, dc, wdf); adamw_update(c, pv.w, mv.w, vv.w, gv.w, ss, dc, wdf);
       sp[i] = pv; smm[i] = mv; sv[i] = vv;
       if (target) {  // fused update_target_network (models.py:81)
         const float tau = ta, one_minus_tau = omt;

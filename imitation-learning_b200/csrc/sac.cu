@@ -121,14 +121,10 @@ __global__ void sac_alpha_kernel(float* __restrict__ log_alpha, const float* __r
     const float alpha = expf(p);
     const float g = -alpha * s / (float)B;  // d/dlog_alpha of -mean(w (1-abs) alpha (log_pi + H)) ; equals the loss value
     if (out_losses) out_losses[r * 3 + 2] = g;
-    const double t = (double)*step;
-    const float step_size = (float)(lr / (1.0 - pow(beta1, t))), bc2_sqrt = (float)sqrt(1.0 - pow(beta2, t));
+    float step_size, bc2_sqrt;
+    adamw_bias_correction(lr, beta1, beta2, *step, step_size, bc2_sqrt);
     float mi = m[r], vi = v[r];
-    if (wd != 0.0) p = __fmul_rn(p, (float)(1.0 - lr * wd));
-    mi = __fadd_rn(mi, __fmul_rn((float)(1.0 - beta1), __fsub_rn(g, mi)));
-    vi = __fadd_rn(__fmul_rn(vi, (float)beta2), __fmul_rn(__fmul_rn((float)(1.0 - beta2), g), g));
-    const float denom = __fadd_rn(__fdiv_rn(sqrtf(vi), bc2_sqrt), (float)eps);
-    p = __fadd_rn(p, __fmul_rn(-step_size, __fdiv_rn(mi, denom)));
+    adamw_update(adamw_coefs(step_size, bc2_sqrt, lr, wd, beta1, beta2, eps), p, mi, vi, g);
     log_alpha[r] = p; m[r] = mi; v[r] = vi;
   }
 }
