@@ -32,7 +32,7 @@ import numpy as np
 import torch
 import yaml
 
-from . import _lib
+from . import _lib, checkpoint
 from .config import (BOTH, CONF_DIR, IGNORED, MULTIRUN_FLAGS, PER_REPLICA_KEYS, SWEEP, Config, SweepError, SweepJob, _parse, _reject_sweep, load_config,
                      replica_values, seed_per_replica, set_key, sweep_groups)
 
@@ -475,11 +475,25 @@ def trial_jobs(base: Sequence[str], trials: List[Dict[str, Any]], env: str, seed
   return [SweepJob(t['trial'], list(base) + [f'env={env}'] + t['overrides'] + [f'seed={seed0 + t["trial"] * R}']) for t in trials]
 
 
-def run_trials(base: Sequence[str], trials: List[Dict[str, Any]], out_dir: str, seed0: int, R: int) -> List[int]:
+def round_plan(out_dir: str, r: int, env_groups: Dict[str, List[List[int]]]) -> Dict[str, List[str]]:
+  """How a resumed search finishes round r: checkpoint.group_plan of every program (env -> the trial numbers of each of its programs). A
+  program is skipped once its trials have their metrics.pth and their scores are recorded in checkpoint/round<r>/scores.json; one with a
+  checkpoint continues from it; the rest run."""
+  root = os.path.join(out_dir, 'checkpoint', f'round{r}')
+  done = checkpoint.read_scores(root)
+  return {env: [checkpoint.group_plan([os.path.join(out_dir, str(j), env) for j in g], all(str(j) in done.get(env, {}) for j in g), os.path.join(root, env, f'group{k}'))
+                for k, g in enumerate(groups)] for env, groups in env_groups.items()}
+
+
+def run_trials(base: Sequence[str], trials: List[Dict[str, Any]], out_dir: str, seed0: int, R: int, round_index: Optional[int] = None, resume: bool = False) -> List[int]:
   """Trains the trials on every env (env after env; each env's trials as the programs of config.sweep_groups) and fills each trial's
-  `scores` {env: train() score}. Returns the number of programs per env."""
+  `scores` {env: train() score}. Returns the number of programs per env. round_index (checkpoint.interval set): program k of env e checkpoints
+  into <out_dir>/checkpoint/round<r>/<e>/group<k>, and the scores of finished programs go to checkpoint/round<r>/scores.json; resume: finish
+  the round as round_plan says."""
   from .environments import ENVS
   from .train import _train
+  root = None if round_index is None else os.path.join(out_dir, 'checkpoint', f'round{round_index}')
+  done = checkpoint.read_scores(root) if resume else {}
   programs = []
   for env in ENVS:
     jobs = trial_jobs(base, trials, env, seed0, R)
@@ -487,7 +501,11 @@ def run_trials(base: Sequence[str], trials: List[Dict[str, Any]], out_dir: str, 
     programs.append(len(groups))
     print(f'env {env}: {len(jobs)} trial(s) in {len(groups)} program(s)', flush=True)
     by_num = {t['trial']: t for t in trials}
-    for g in groups:
+    plan = round_plan(out_dir, round_index, {env: [[j.num for j in g.jobs] for g in groups]})[env] if resume else ['run'] * len(groups)
+    for k, g in enumerate(groups):
+      if plan[k] == 'skip':
+        for j in g.jobs: by_num[j.num]['scores'][env] = done[env][str(j.num)]
+        continue
       cfg = load_config(g.overrides)
       J = len(g.jobs)
       cfg.replicas = J * R
@@ -497,12 +515,21 @@ def run_trials(base: Sequence[str], trials: List[Dict[str, Any]], out_dir: str, 
         d = os.path.join(out_dir, str(j.num), env)
         os.makedirs(d, exist_ok=True)
         blocks.append((d + os.sep, f'trial {j.num} {env}: ', i * R, (i + 1) * R))
-      for j, s in zip(g.jobs, _train(cfg, blocks, per_replica)): by_num[j.num]['scores'][env] = s
+      gdir = os.path.join(root, env, f'group{k}') if root is not None and checkpoint.interval_of(cfg) else None
+      for j, s in zip(g.jobs, _train(cfg, blocks, per_replica, checkpoint_dir=gdir, overrides=g.overrides, resume=plan[k] == 'continue')): by_num[j.num]['scores'][env] = s
+      if root is not None:
+        done.setdefault(env, {}).update({str(j.num): by_num[j.num]['scores'][env] for j in g.jobs})
+        checkpoint.write_scores(root, done)
+        checkpoint.remove(gdir)
   return programs
 
 
-def search(argv: Sequence[str]) -> Dict[str, Any]:
-  """`train_all.py -m algorithm=<ALG> [fixed overrides] [hpo.<key>=value]`: the whole search; returns the hpo.json record."""
+def search(argv: Sequence[str], resume_dir: Optional[str] = None) -> Dict[str, Any]:
+  """`train_all.py -m algorithm=<ALG> [fixed overrides] [hpo.<key>=value]`: the whole search; returns the hpo.json record.
+
+  With checkpoint.interval the search directory also holds multirun.yaml (`argv`) and the checkpoints of the running round (run_trials).
+  resume_dir: continue that search: the rounds in its hpo.json are kept, the interrupted round is finished (round_plan), and later rounds
+  are proposed as before (a proposal depends only on the trials so far, hpo.seed and the round index)."""
   from . import distributed
   from .environments import ENVS
   if int(os.environ.get('WORLD_SIZE', '1')) > 1: raise NotImplementedError('a hyper-parameter search runs on one GPU; searches across ranks are not supported')
@@ -516,12 +543,20 @@ def search(argv: Sequence[str]) -> Dict[str, Any]:
   if not seed_per_replica(cfg0): raise SweepError('a search gives every trial its own seed, which this configuration cannot take per replica (device_rng=false, or a subsampled expert memory)')
   space = Space.of(cfg0.algorithm, base)
   R, seed0, sign = int(cfg0.get('replicas', 1)), int(cfg0.seed), -1.0 if hpo['minimize'] else 1.0
-  out_dir = os.path.join(cfg0.get('output_dir', './outputs'), f'{cfg0.algorithm}_all_sweeper', time.strftime('%m-%d_%H-%M-%S'))
+  interval = checkpoint.interval_of(cfg0)
+  out_dir = resume_dir or os.path.join(cfg0.get('output_dir', './outputs'), f'{cfg0.algorithm}_all_sweeper', time.strftime('%m-%d_%H-%M-%S'))
   os.makedirs(out_dir, exist_ok=True)
   record = dict(algorithm=cfg0.algorithm, overrides=base, hpo=hpo, envs=list(ENVS), searched=[p.key for p in space.params], group_keys=[p.key for p in space.group_params],
                 d=space.d, trials=[], rounds=[])
   print(f'search: {cfg0.algorithm}, {len(space.params)} searched key(s) in {space.d} dimension(s), grouping on {record["group_keys"] or "nothing"}', flush=True)
   best_after, n_sobol, reason = [], 0, None
+  if resume_dir:
+    record, best_after, n_sobol = completed_rounds(resume_dir, record, space, hpo, sign)
+    reason = stop_reason(best_after, len(record['trials']), hpo) if record['rounds'] else None
+    print(f'resuming at round {len(record["rounds"])} with {len(record["trials"])} finished trial(s)', flush=True)
+  elif interval:
+    with open(os.path.join(out_dir, 'multirun.yaml'), 'w') as f: yaml.safe_dump(list(argv), f)
+  resumed_round = len(record['rounds']) if resume_dir else None
   try:
     while reason is None:
       q = round_size(len(record['trials']), hpo)
@@ -542,7 +577,7 @@ def search(argv: Sequence[str]) -> Dict[str, Any]:
         os.makedirs(d, exist_ok=True)
         with open(os.path.join(d, 'overrides.yaml'), 'w') as f: yaml.safe_dump(list(base) + t['overrides'] + [f'seed={seed0 + t["trial"] * R}'], f)
       print(f'round {r} ({info["kind"]}): {len(trials)} trial(s)', flush=True)
-      info['programs_per_env'] = run_trials(base, trials, out_dir, seed0, R)
+      info['programs_per_env'] = run_trials(base, trials, out_dir, seed0, R, **(dict(round_index=r, resume=r == resumed_round) if interval else {}))
       for t in trials:
         t['objective'] = trial_objective([t['scores'][e] for e in ENVS])
         t['failed'] = not math.isfinite(t['objective'])
@@ -554,6 +589,7 @@ def search(argv: Sequence[str]) -> Dict[str, Any]:
       reason = stop_reason(best_after, len(record['trials']), hpo)
       if not trials: reason = 'no admissible candidate'
       with open(os.path.join(out_dir, 'hpo.json'), 'w') as f: json.dump(record, f, indent=1)
+      if interval: checkpoint.remove(os.path.join(out_dir, 'checkpoint', f'round{r}'))
   finally:
     distributed.shutdown()
   ok = [t for t in record['trials'] if not t['failed']]
@@ -566,6 +602,23 @@ def search(argv: Sequence[str]) -> Dict[str, Any]:
   print(f'search stopped ({reason}) after {len(record["trials"])} trial(s); {len(record["failed"])} failed', flush=True)
   if best is not None: print(f'best: trial {best["trial"]}: objective {best["objective"]:.4f}: {" ".join(best["overrides"])}', flush=True)
   return record
+
+
+def completed_rounds(out_dir: str, record: Dict[str, Any], space: Space, hpo: Dict[str, Any], sign: float) -> Tuple[Dict[str, Any], List[float], int]:
+  """(record, best objective after each round, Sobol points consumed) of the rounds a search in out_dir finished, from its hpo.json (the
+  fresh `record` when it finished none). A record of another configuration or other search settings is refused."""
+  path = os.path.join(out_dir, 'hpo.json')
+  if not os.path.isfile(path): return record, [], 0
+  with open(path) as f: saved = json.load(f)
+  for k in ('algorithm', 'overrides', 'hpo', 'envs', 'searched', 'group_keys', 'd'):
+    if saved.get(k) != record[k]: raise checkpoint.CheckpointError(f'{path}: {k} differs from the search\'s command line')
+  best_after, n_sobol, n = [], 0, 0
+  for r, info in enumerate(saved['rounds']):
+    if info['kind'] == 'sobol': n_sobol += sobol_round(space, round_size(n, hpo), hpo['seed'], n_sobol, hpo['max_groups'])[1]
+    n += sum(1 for t in saved['trials'] if t['round'] == r)
+    finite = [sign * t['objective'] for t in saved['trials'][:n] if not t['failed']]
+    best_after.append(max(finite) if finite else -math.inf)
+  return saved, best_after, n_sobol
 
 
 def train_all(argv: Sequence[str]) -> float:
@@ -591,4 +644,10 @@ def train_all(argv: Sequence[str]) -> float:
 def main(argv: Optional[Sequence[str]] = None):
   import sys
   argv = list(sys.argv[1:] if argv is None else argv)
+  target = [a for a in argv if a.startswith('resume=')]
+  if target:  # `train_all.py resume=<search dir>`
+    d, others = target[0].partition('=')[2], [a for a in argv if a != target[0]]
+    if others: raise SystemExit(f'resume refused: resume= takes no other override (the configuration comes from the search); got {" ".join(others)}')
+    if not os.path.isfile(os.path.join(d, 'multirun.yaml')): raise SystemExit(f'resume refused: {d} holds no checkpointed search (multirun.yaml)')
+    with open(os.path.join(d, 'multirun.yaml')) as f: return search(yaml.safe_load(f), resume_dir=d)
   return search(argv) if any(a in MULTIRUN_FLAGS for a in argv) else train_all(argv)

@@ -276,10 +276,14 @@ class SoftActor(_Module):
   def draw_masks(self, n: int) -> List[Optional[Tensor]]:
     """[input mask [R, n, S] or None, one [R, n, H] mask per hidden layer or None]: Bernoulli(1 - p) / (1 - p) draws on the device (Philox), the analogue
     of nn.Dropout's draws from torch's global stream."""
-    if self._drop_rng is None: self._drop_rng = _mask_rng(977, self.replicas, self.per_replica_masks, self.device)
     ch = self._choices
     sites = [(self.state_size, self.input_dropout, ch.input_dropout_r)] + [(self.mlp.dims[l + 1], self.dropout, ch.dropout_r) for l in range(self.mlp.n_layers - 1)]
-    return _masks_of(self._drop_rng, self.replicas, n, self.device, sites, 31)
+    return _masks_of(self.mask_source(), self.replicas, n, self.device, sites, 31)
+
+  def mask_source(self) -> _RNG:
+    """The device source of the dropout masks, made at its first use."""
+    if self._drop_rng is None: self._drop_rng = _mask_rng(977, self.replicas, self.per_replica_masks, self.device)
+    return self._drop_rng
 
   def _log_prob_dropout(self, state: Tensor, action: Tensor, repeat: int = 1, masks: Optional[List[Optional[Tensor]]] = None) -> Tensor:
     R, S, A = self.replicas, self.state_size, self.action_size
@@ -857,10 +861,14 @@ class REDDiscriminator(_Module):
     return self._ws
 
   def draw_masks(self, n: int) -> List[Optional[Tensor]]:
-    if self._rng is None: self._rng = _mask_rng(1979, self.replicas, self.per_replica_masks, self.device)
     ch, dims = self._choices, self.predictor.dims
     sites = [(dims[0], self.input_dropout, ch.input_dropout_r)] + [(dims[l + 1], self.dropout, ch.dropout_r) for l in range(self.predictor.n_layers - 1)]
-    return _masks_of(self._rng, self.replicas, n, self.device, sites, 32)
+    return _masks_of(self.mask_source(), self.replicas, n, self.device, sites, 32)
+
+  def mask_source(self) -> _RNG:
+    """The device source of the dropout masks, made at its first use."""
+    if self._rng is None: self._rng = _mask_rng(1979, self.replicas, self.per_replica_masks, self.device)
+    return self._rng
 
   def _batch_of(self, state: Tensor, action: Tensor) -> TransitionBatch:
     R = self.replicas

@@ -12,6 +12,7 @@ graphs and replayed without host involvement. Replica r is a reference-equivalen
 """
 from __future__ import annotations
 
+import copy
 import ctypes as C
 import os
 import sys
@@ -22,7 +23,7 @@ import numpy as np
 import torch
 from torch import Tensor
 
-from . import _lib, distributed
+from . import _lib, checkpoint, distributed
 from .config import PER_REPLICA_DROPOUT, Config, SweepError, SweepJob, expand_sweep, get_key, load_config, needs_expert_memory, replica_values, split_per_replica, sweep_groups
 from .environments import D4RLEnv, ENVS
 from .evaluation import evaluate_agent
@@ -208,6 +209,8 @@ class Trainer:
     self.metrics = dict(train_steps=[], train_returns=[], test_steps=[], test_returns=[], test_returns_normalized=[], update_steps=[], predicted_rewards=[], alphas=[],
                         entropies=[], Q_values=[])  # train.py:87
     self.score: List[float] = []
+    self.block_scores: List[List[float]] = []  # per output block (_train): the normalised evaluation means so far
+    self.active_time = 0.0  # seconds of training before this process resumed the run (check_time_usage)
     self.env.batch.reset(self.env.reset_noise(R), self.state)  # train.py:146
 
   def _pwil_relabel_expert(self):
@@ -408,10 +411,7 @@ class Trainer:
     self.step += 1
     if self._will_update(self.step):
       if not self.device_rng:  # host-drawn index uniforms (the reference draws its indices on the host: memory.py:54)
-        if getattr(self, '_pin', None) is None:
-          self._pin = [torch.empty(2, self.R, self.B, pin_memory=True) for _ in range(2)]  # double-buffered pinned staging
-          self._pin_ev = [None, None]
-          self._host_rng = np.random.default_rng(self.seed)  # per-rank stream: seed + first replica of this shard
+        self._host_stream()
         slot = self.step & 1
         if self._pin_ev[slot] is not None: self._pin_ev[slot].synchronize()  # the H2D copy that last used this buffer is done
         self._host_rng.random(out=self._pin[slot].numpy(), dtype=np.float32)
@@ -424,6 +424,13 @@ class Trainer:
       self.updates += 1
     else:
       self._run('step', self.rollout)
+
+  def _host_stream(self):
+    """device_rng=false: the host stream of the index uniforms and its double-buffered pinned staging, made at the first update."""
+    if getattr(self, '_pin', None) is None:
+      self._pin = [torch.empty(2, self.R, self.B, pin_memory=True) for _ in range(2)]  # double-buffered pinned staging
+      self._pin_ev = [None, None]
+      self._host_rng = np.random.default_rng(self.seed)  # per-rank stream: seed + first replica of this shard
 
   def total_launches(self) -> int:
     """Kernels launched by this library for this process (eager launches + kernels replayed through CUDA graphs)."""
@@ -448,6 +455,110 @@ class Trainer:
     """train.py:237: agent.pth contents."""
     return dict(actor=self.actor.state_dict(), critic=self.critic.state_dict(), log_alpha=self.log_alpha.detach().clone().cpu())
 
+  # ---- checkpoints (checkpoint.py) --------------------------------------------------------------------------------------------
+  # The discriminator's state per algorithm (dotted attribute paths; an attribute that is None or not yet made is left out)
+  _DISCRIMINATOR_STATE = {'GMMIL': ('gamma', ), 'PWIL': ('expert_weights', ), 'RED': ('predictor.flat', 'target.flat', 'sigma', '_rng.counter'),
+                          'DRIL': ('mlp.flat', '_q', '_drop_rng.counter'), 'AdRIL': ('_flag', ), 'SAC': (), 'BC': ()}
+
+  def _discriminator_state(self) -> Sequence[str]:
+    if self.algorithm != 'GAIL': return self._DISCRIMINATOR_STATE[self.algorithm]
+    return ('flat', 'g_u', 'g_v', 'h_u', 'h_v') if self.discriminator.general else ('mlp.flat', 'u', 'v')
+
+  def _state_tensors(self) -> Dict[str, Tensor]:
+    """Every device tensor a later loop iteration reads, by name: the live tensors that checkpoint_state copies and load_checkpoint_state
+    overwrites in place. Everything else on the device is set up by the constructor or rewritten before it is read (tests/test_gpu_resume.py
+    walks the Trainer to keep it so)."""
+    t = dict(actor=self.actor.mlp.flat, critic=self.critic.mlp.flat, target_critic=self.target_critic.mlp.flat, log_alpha=self.log_alpha)
+    for name in ('actor_optimiser', 'critic_optimiser', 'temperature_optimiser', 'discriminator_optimiser'):
+      o = getattr(self, name, None)
+      if o is not None: t.update({f'{name}.exp_avg': o.exp_avg, f'{name}.exp_avg_sq': o.exp_avg_sq, f'{name}.step_count': o.step_count})
+    for n in ('rows', '_idx', '_full', '_num_trajectories', '_rng_counter'): t[f'memory.{n}'] = getattr(self.memory, n)
+    if self.expert_memory is not None: t['expert_memory._rng_counter'] = self.expert_memory._rng_counter
+    for n in ('state', 'next_state', 'step_f', 'running_return', 'last_return', 'return_sum', 'episodes'): t[n] = getattr(self, n)
+    t['env.x'], t['env.t'] = self.env.batch.x, self.env.batch.t  # the training envs' physical state and step counters
+    if self.rng.counter is not None: t['rng.counter'] = self.rng.counter
+    for n in self._discriminator_state():
+      v = _attr(self.discriminator, n)
+      if v is not None: t[f'discriminator.{n}'] = v
+    return t
+
+  def _expert_digest(self) -> Optional[str]:
+    if self.expert_memory is None: return None
+    if getattr(self, '_expert_sha', None) is None:
+      from .checkpoint import expert_digest
+      self._expert_sha = expert_digest(self.expert_memory.rows)
+    return self._expert_sha
+
+  def checkpoint_state(self) -> Dict[str, object]:
+    """Host copies of all state a later loop iteration reads (the filled rows of each replay ring only), the host random streams and the
+    loop bookkeeping. load_checkpoint_state(checkpoint_state()) on a freshly constructed Trainer of the same configuration continues the run
+    bit for bit."""
+    m = self.memory
+    filled = m.size if bool(m._full.any()) else int(m._idx.max())
+    tensors = {k: (v[:, :filled] if k == 'memory.rows' else v).detach().to('cpu', copy=True).contiguous() for k, v in self._state_tensors().items()}
+    d = self.discriminator
+    host = dict(step=self.step, updates=self.updates, metrics=copy.deepcopy(self.metrics), scores=copy.deepcopy(self.block_scores), active_time=float(self.active_time),
+                env_gen=_gen_state(self.env._gen), eval_env_gen=_gen_state(self.eval_env._gen),
+                host_rng=None if getattr(self, '_host_rng', None) is None else self._host_rng.bit_generator.state,
+                torch_rng=torch.get_rng_state(), numpy_rng=np.random.get_state(), discriminator_training=getattr(d, 'training', None), sigma_set=getattr(d, '_sigma_set', None))
+    return dict(replicas=self.R, algorithm=self.algorithm, expert_digest=self._expert_digest(), tensors=tensors, host=host)
+
+  def load_checkpoint_state(self, state: Dict[str, object]):
+    """Restores checkpoint_state() into this freshly constructed Trainer, in place (copy_ into the existing tensors, whose pointers the C
+    structs, the evaluation cache and captured graphs hold), before its first step. A checkpoint of another algorithm, replica count or
+    expert memory is refused."""
+    from .checkpoint import CheckpointError
+    if self.step != 0 or self.graphs: raise CheckpointError('load a checkpoint into a fresh Trainer, before its first step')
+    if state['algorithm'] != self.algorithm or state['replicas'] != self.R:
+      raise CheckpointError(f'checkpoint of {state["algorithm"]} x {state["replicas"]} replica(s); this run is {self.algorithm} x {self.R}')
+    if state['expert_digest'] != self._expert_digest(): raise CheckpointError('the expert memory differs from the one the checkpoint was trained on')
+    saved, d, dev = state['tensors'], self.discriminator, self.device
+    # state made lazily by the first draws / updates of a run: made here, before any graph capture
+    if 'rng.counter' in saved: self.rng._ctr(dev)
+    if 'discriminator._rng.counter' in saved or 'discriminator._drop_rng.counter' in saved: d.mask_source()._ctr(dev)
+    if 'discriminator.gamma' in saved and d.gamma is None: d.gamma = torch.empty(saved['discriminator.gamma'].shape, device=dev)
+    if 'discriminator._q' in saved and getattr(d, '_q', None) is None: d._q = torch.empty(saved['discriminator._q'].shape, device=dev)
+    live = self._state_tensors()
+    if set(live) != set(saved): raise CheckpointError(f'checkpoint state {sorted(set(saved) ^ set(live))} does not match this run\'s')
+    for k, v in live.items():
+      src = saved[k]
+      if k == 'memory.rows':  # the filled part of each ring; the rest is as a fresh ring
+        if src.shape[0] != v.shape[0] or src.shape[1] > v.shape[1] or src.shape[2] != v.shape[2]: raise CheckpointError(f'{k}: {tuple(src.shape)} does not fit {tuple(v.shape)}')
+        v[:, :src.shape[1]].copy_(src)
+        v[:, src.shape[1]:].zero_()
+        continue
+      if src.shape != v.shape or src.dtype != v.dtype: raise CheckpointError(f'{k}: {src.dtype} {tuple(src.shape)} does not match {v.dtype} {tuple(v.shape)}')
+      v.copy_(src)
+    h = state['host']
+    if self.algorithm == 'DRIL': d.q = float(d._q[0]) if self.R == 1 else d._q
+    if h['discriminator_training'] is not None: d.training = h['discriminator_training']
+    if h['sigma_set'] is not None: d._sigma_set = h['sigma_set']
+    self.step, self.updates, self.metrics, self.block_scores, self.active_time = h['step'], h['updates'], h['metrics'], h['scores'], h['active_time']
+    _set_gen_state(self.env._gen, h['env_gen'])
+    _set_gen_state(self.eval_env._gen, h['eval_env_gen'])
+    if h['host_rng'] is not None:
+      self._host_stream()
+      self._host_rng.bit_generator.state = h['host_rng']
+    torch.set_rng_state(h['torch_rng'])
+    np.random.set_state(h['numpy_rng'])
+
+
+def _attr(obj, dotted: str):
+  for p in dotted.split('.'):
+    obj = getattr(obj, p, None)
+    if obj is None: return None
+  return obj
+
+
+def _gen_state(gen):
+  return gen.get_state() if isinstance(gen, torch.Generator) else [g.get_state() for g in gen]
+
+
+def _set_gen_state(gen, state):
+  if isinstance(gen, torch.Generator): gen.set_state(state)
+  else:
+    for g, s in zip(gen, state): g.set_state(s)
+
 
 def _block(x, lo: int, hi: int, total: int):
   """Replicas [lo, hi) of an output that a single-replica run writes without its replica axis (the reference's shapes)."""
@@ -456,26 +567,43 @@ def _block(x, lo: int, hi: int, total: int):
   return x[lo] if hi - lo == 1 else x[lo:hi]
 
 
-def train(cfg: Config, file_prefix: str = '') -> float:
+def train(cfg: Config, file_prefix: str = '', overrides: Sequence[str] = ()) -> float:
   """train.py:26-243 (accelerated algorithms). Multi-GPU: launched one process per GPU (torch.distributed.run); the
-  replica axis is split across ranks and evaluation returns are reduced over NCCL (distributed.py)."""
-  return _train(cfg, [(file_prefix, '', None, None)])[0]
+  replica axis is split across ranks and evaluation returns are reduced over NCCL (distributed.py). With checkpoint.interval, the run
+  checkpoints into <file_prefix's directory>/checkpoint (`overrides`, the command line, is recorded there)."""
+  ckpt_dir = os.path.join(os.path.dirname(file_prefix) or '.', 'checkpoint') if checkpoint.interval_of(cfg) else None
+  return _train(cfg, [(file_prefix, '', None, None)], checkpoint_dir=ckpt_dir, overrides=overrides)[0]
 
 
-def _train(cfg: Config, blocks, per_replica: Optional[Dict[str, Sequence[float]]] = None) -> List[float]:
+def _train(cfg: Config, blocks, per_replica: Optional[Dict[str, Sequence[float]]] = None, checkpoint_dir: Optional[str] = None, overrides: Sequence[str] = (),
+           resume: bool = False, stop_at: Optional[int] = None) -> Optional[List[float]]:
   """The loop of train(). `blocks`: (file prefix, console label, lo, hi) per output set; lo = None is the whole run (and its shards
-  across ranks), otherwise replicas [lo, hi) of a single-rank run — one job of a sweep, written and scored as its own run."""
+  across ranks), otherwise replicas [lo, hi) of a single-rank run — one job of a sweep, written and scored as its own run.
+
+  checkpoint_dir: where the checkpoints of checkpoint.interval go (checkpoint.py), each taken after its step's logging and evaluation;
+  resume: continue from the latest of them, skipping the pre-training phases its state already holds. stop_at (tests): return None right
+  after the checkpoint of that step, writing no output."""
+  interval = checkpoint.interval_of(cfg)
+  if interval and checkpoint_dir is None: raise checkpoint.CheckpointError('checkpoint.interval needs a checkpoint directory')
   rank, world = distributed.init('nccl')
   total = int(cfg.get('replicas', 1))
   lo, hi = distributed.shard(total, rank, world)
   trainer = Trainer(cfg, replicas=hi - lo, seed_offset=lo, per_replica=per_replica)
-  metrics, scores = trainer.metrics, [[] for _ in blocks]
+  trainer.block_scores = [[] for _ in blocks]
+  first = 1
+  if resume:
+    _, state = checkpoint.load(checkpoint_dir, rank, world)
+    trainer.load_checkpoint_state(state)
+    first = trainer.step + 1
+    if rank == 0: print(f'resuming at step {first} from {checkpoint.latest(checkpoint_dir)}', flush=True)
+  metrics, scores = trainer.metrics, trainer.block_scores
   cut = lambda x, b: _block(x, b[2], b[3], total)
   part = lambda x, b: x if b[2] is None else x[b[2]:b[3]]  # outputs that keep the replica axis at one replica
   flat_of = lambda b: (total if b[2] is None else b[3] - b[2]) == 1  # the reference's schema for a single replica (train.py:214-219)
   stats_of = lambda returns, b: distributed.return_statistics(returns if b[2] is None else returns[b[2]:b[3]])
-  start_time = time.time()
-  if cfg.bc_pretraining.iterations > 0:  # train.py:93-112
+  start_time = time.time() - trainer.active_time
+  if cfg.algorithm == 'BC' and interval and rank == 0: print('checkpoint.interval: algorithm=BC trains before the loop, which takes checkpoints; none is written', flush=True)
+  if not resume and cfg.bc_pretraining.iterations > 0:  # train.py:93-112
     trainer.bc_pretrain()
     if cfg.algorithm == 'BC':
       returns = trainer.evaluate()
@@ -491,8 +619,9 @@ def _train(cfg: Config, blocks, per_replica: Optional[Dict[str, Sequence[float]]
           torch.save(m, f'{b[0]}metrics.pth')
         out.append(float(np.mean(n_b)))
       return out
-  if cfg.algorithm in ('DRIL', 'RED'): trainer.pretrain_discriminator()  # train.py:117-133
-  for step in range(1, cfg.steps + 1):
+  if not resume and cfg.algorithm in ('DRIL', 'RED'): trainer.pretrain_discriminator()  # train.py:117-133
+  meta = dict(config=cfg, overrides=list(overrides), replicas=total, per_replica=per_replica or {})
+  for step in range(first, cfg.steps + 1):
     trainer.train_step()
     if cfg.logging.interval > 0 and step % cfg.logging.interval == 0 and trainer._will_update(step): trainer.log_aux()  # train.py:205: only inside the update branch
     if step % cfg.evaluation.interval == 0 and not cfg.check_time_usage:  # train.py:213
@@ -507,6 +636,10 @@ def _train(cfg: Config, blocks, per_replica: Optional[Dict[str, Sequence[float]]
         metrics['_blocks'][i]['test_returns'].append(r_b.reshape(-1).tolist() if flat else r_b.tolist())
         metrics['_blocks'][i]['test_returns_normalized'].append(n_b.reshape(-1).tolist() if flat else n_b.tolist())
         if rank == 0: print(f'{b[1]}step {step}: test return {mean:.3f} +- {std:.3f} over {n} episodes ({world} rank(s))', flush=True)
+    if interval and step % interval == 0:
+      trainer.active_time = time.time() - start_time
+      checkpoint.save(checkpoint_dir, step, trainer.checkpoint_state(), meta, rank, world, barrier=distributed.barrier)
+    if stop_at == step: return None
   trainer.score = scores[0]
   if cfg.check_time_usage: metrics['training_time'] = time.time() - start_time  # train.py:229-230
   eps = trainer.episodes.cpu().numpy()
@@ -533,22 +666,37 @@ def _train(cfg: Config, blocks, per_replica: Optional[Dict[str, Sequence[float]]
   return [float(np.mean(sc)) if sc else float('nan') for sc in scores]
 
 
-def run_sweep(jobs: List[SweepJob]) -> List[float]:
+def run_sweep(jobs: List[SweepJob], argv: Optional[Sequence[str]] = None, resume_dir: Optional[str] = None) -> List[float]:
   """A multirun on one GPU: the jobs are partitioned into groups (config.sweep_groups); a group of J jobs is exactly the run
   `train.py <group overrides> replicas=J*R` with job j's vectorised values given to replica block [jR, (j+1)R) — so replica jR+k starts
   like a run with seed `seed + jR + k`. A swept seed s_j is per replica instead: replica jR+k is the single run with seed s_j + k, so with
   replicas=1 job j is `train.py <its overrides>` bit for bit. Groups run one after another. Job j writes the single-run files of its replicas, plus
-  overrides.yaml, to <output_dir>/<ALG>_<ENV>_sweeper/<timestamp>/<j>/ (hydra.sweep.dir). Returns the per-job scores."""
+  overrides.yaml, to <output_dir>/<ALG>_<ENV>_sweeper/<timestamp>/<j>/ (hydra.sweep.dir). Returns the per-job scores.
+
+  With checkpoint.interval the sweep directory also holds multirun.yaml (`argv`), checkpoint/group<k>/ (the running group's checkpoint)
+  and checkpoint/scores.json (the scores of the finished groups). resume_dir: continue that sweep (checkpoint.sweep_plan): finished groups
+  are skipped, the interrupted one continues from its checkpoint, the rest run."""
   import yaml
   if int(os.environ.get('WORLD_SIZE', '1')) > 1: raise NotImplementedError('a multirun sweep runs on one GPU; sweeps across ranks are not supported')
   groups = sweep_groups(jobs)
+  cfgs = [load_config(g.overrides) for g in groups]
+  ckpt_on = any(checkpoint.interval_of(c) for c in cfgs)
   cfg0 = load_config(jobs[0].overrides)
-  base = os.path.join(cfg0.get('output_dir', './outputs'), f'{cfg0.algorithm}_{cfg0.env}_sweeper', time.strftime('%m-%d_%H-%M-%S'))
+  base = resume_dir or os.path.join(cfg0.get('output_dir', './outputs'), f'{cfg0.algorithm}_{cfg0.env}_sweeper', time.strftime('%m-%d_%H-%M-%S'))
+  root = os.path.join(base, 'checkpoint')
+  plan = checkpoint.sweep_plan(base, [[j.num for j in g.jobs] for g in groups]) if resume_dir else ['run'] * len(groups)
+  if ckpt_on and not resume_dir:
+    os.makedirs(base, exist_ok=True)
+    with open(os.path.join(base, 'multirun.yaml'), 'w') as f: yaml.safe_dump(list(argv or []), f)
   print(f'sweep: {len(jobs)} job(s) in {len(groups)} group(s)', flush=True)
+  done = {int(k): v for k, v in checkpoint.read_scores(root).items()} if resume_dir else {}
   scores: Dict[int, float] = {}
   try:
-    for g in groups:
-      cfg = load_config(g.overrides)
+    for k, (g, cfg) in enumerate(zip(groups, cfgs)):
+      if plan[k] == 'skip':
+        for j in g.jobs: scores[j.num] = done[j.num]
+        print(f'group of jobs {[j.num for j in g.jobs]}: finished before the resume', flush=True)
+        continue
       R, J = int(cfg.get('replicas', 1)), len(g.jobs)
       cfg.replicas = J * R
       per_replica = {k: replica_values(k, vals, R) for k, vals in g.per_job.items()}
@@ -559,22 +707,53 @@ def run_sweep(jobs: List[SweepJob]) -> List[float]:
         with open(os.path.join(d, 'overrides.yaml'), 'w') as f: yaml.safe_dump(j.overrides, f)
         blocks.append((d + os.sep, f'job {j.num}: ', i * R, (i + 1) * R))
       print(f'group of jobs {[j.num for j in g.jobs]}: {J} x {R} replica(s), per-replica {sorted(per_replica) or "none"}', flush=True)
-      for j, s in zip(g.jobs, _train(cfg, blocks, per_replica)): scores[j.num] = s
+      gdir = os.path.join(root, f'group{k}') if checkpoint.interval_of(cfg) else None
+      for j, s in zip(g.jobs, _train(cfg, blocks, per_replica, checkpoint_dir=gdir, overrides=g.overrides, resume=plan[k] == 'continue')): scores[j.num] = s
+      if ckpt_on:
+        checkpoint.write_scores(root, {str(n): s for n, s in scores.items()})
+        checkpoint.remove(gdir)
   finally:
     distributed.shutdown()
   for j in jobs: print(f'job {j.num}: {" ".join(j.overrides)}: score {scores[j.num]:.4f}', flush=True)
   return [scores[j.num] for j in jobs]
 
 
+def resume(target: str, others: Sequence[str] = ()):
+  """`train.py resume=<dir>`: continues the run or multirun in <dir> from its checkpoint, writing into the same directory. The configuration
+  comes from the checkpoint (a run's meta.json, a multirun's multirun.yaml); any other override, a missing checkpoint, another world size or
+  library version, or a file whose checksum does not match is refused."""
+  import yaml
+  if others: raise checkpoint.CheckpointError(f'resume= takes no other override (the configuration comes from the checkpoint); got {" ".join(others)}')
+  if os.path.isfile(os.path.join(target, 'multirun.yaml')):
+    with open(os.path.join(target, 'multirun.yaml')) as f: argv = yaml.safe_load(f)
+    _, jobs = expand_sweep(argv)
+    return run_sweep(jobs, argv, resume_dir=target)
+  meta = checkpoint.resume_run_meta(target, others, int(os.environ.get('WORLD_SIZE', '1')))
+  try:
+    return _train(Config(meta['config']), [(target.rstrip(os.sep) + os.sep, '', None, None)], checkpoint_dir=os.path.join(target, 'checkpoint'), overrides=meta['overrides'],
+                  resume=True)[0]
+  finally:
+    distributed.shutdown()
+
+
 def main(argv: Optional[List[str]] = None):
   """`python train.py algorithm=<ALG> env=<ENV> [key=value ...]` (train.py:21-23, 246): returns the score. With `-m` / `--multirun` and
-  comma-separated values (`reinforcement.discount=0.97,0.98,0.99`): Hydra's basic sweep, run by run_sweep; returns the per-job scores."""
-  multirun, jobs = expand_sweep(sys.argv[1:] if argv is None else argv)
-  if multirun: return run_sweep(jobs)
+  comma-separated values (`reinforcement.discount=0.97,0.98,0.99`): Hydra's basic sweep, run by run_sweep; returns the per-job scores.
+  `python train.py resume=<dir>`: continues a checkpointed run or multirun (resume)."""
+  argv = list(sys.argv[1:] if argv is None else argv)
+  target = [a for a in argv if a.startswith('resume=')]
+  if target:
+    try:
+      return resume(target[0].partition('=')[2], [a for a in argv if a != target[0]])
+    except checkpoint.CheckpointError as e:
+      raise SystemExit(f'resume refused: {e}')
+  multirun, jobs = expand_sweep(argv)
+  if multirun: return run_sweep(jobs, argv)
   cfg = load_config(jobs[0].overrides)
+  checkpoint.interval_of(cfg)
   out_dir = os.path.join(cfg.get('output_dir', './outputs'), f'{cfg.algorithm}_{cfg.env}', time.strftime('%m-%d_%H-%M-%S'))  # conf/train_config.yaml:54-60
   os.makedirs(out_dir, exist_ok=True)
   try:
-    return train(cfg, file_prefix=out_dir + os.sep)
+    return train(cfg, file_prefix=out_dir + os.sep, overrides=jobs[0].overrides)
   finally:
     distributed.shutdown()
